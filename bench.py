@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the SIFT hot path on B200 (contract in the task description / SURVEY.md 8d).
+"""Benchmark of the SIFT hot path on H100 (SURVEY.md 8d).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     torchrun --nproc-per-node N bench.py --gpus N ...          (one rank per GPU, no data-path collective)
 
 Workload ("step") = one pass of the hot path over a batch of FRAMES_PER_STEP synthetic 3840x2160
@@ -18,15 +18,19 @@ Printed JSON (rank 0, one line):
             result inside the timed region.  `e2e.pinned_ctypes` keeps the round-1 number (Python mirror,
             page-locked frames) for comparison.
   roofline  pyramid stage: algorithmic bytes per frame (68 B per octave-pixel, SURVEY 8d) / CUDA-event
-            time of the pyramid launches of one frame, against the measured HBM peak
-            (MEASURED_PEAKS.json); `dominant_kernel` = the octave-0 fused blur+DoG launches alone.
+            time of the pyramid launches of one frame, against the HBM peak (MEASURED_PEAKS.json when present,
+            else the H100 SXM data sheet's 3.35 TB/s); `dominant_kernel` = the octave-0 fused blur+DoG launches alone.
   cpu_baseline  the CPU oracle port (oracle/sift_oracle.c, OpenMP) timed on the first four frames of the workload;
   opencv_cpu    cv2.SIFT on the same frame, all host cores (the CPU baseline north_star names).
 `--impl reference` times the UNMODIFIED reference PopSift (oracle/_ref, CUDA, built from
-/root/reference) on the same frames through its own public API (host buffers in, host features out); with
+the reference's sources) on the same frames through its own public API (host buffers in, host features out); with
 --gpus N rank 0 starts one reference process per GPU (each on its own per-GPU batch: weak scaling, like our arm) and reports the aggregate.
 Every rank (and every child process it starts) is bound to the CPUs of its GPU's NUMA node before any
 page-locked allocation.
+--dump-outputs DIR writes what the timed path returned for the frames of its last step (rank 0): keypoints.npy
+(float32 rows frame, octave, x, y, sigma, theta per feature orientation, sorted within each frame), descriptors.npy
+(a seeded sample of their descriptor rows, float32) with descriptor_rows.npy (the sampled row numbers) and
+counts.npy (features, descriptors per frame).
 """
 from __future__ import annotations
 
@@ -152,7 +156,7 @@ def octave_pixels():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe).
+    """nvidia-smi clocks / throttle reasons DURING the timed region.
     The sampler is started ahead of the region; only samples stamped inside [t0, t1] are used."""
 
     FIELDS = ["timestamp", "clocks.sm", "clocks.max.sm", "power.draw", "clocks_event_reasons.hw_slowdown",
@@ -209,18 +213,40 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm), "samples_total": n_all}
 
 
-# one `ncu --set full --clock-control none` capture of tools/one_frame.py 3840 2160 5 1 (round 1, after the
-# last kernel change); per frame / per octave-0 level launch
-NCU_SOURCE = "profiles/r02_ncu_full_frame_4k.csv"
-NCU_PYRAMID_DRAM_BYTES = 2222500352
-NCU_LEVEL_DRAM_BYTES = 368350822
-
-
 def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
+
+
+DUMP_DESC_ROWS = 32768      # descriptors kept by --dump-outputs (16 MB); the keypoints are all kept
+
+
+def dump_outputs(out_dir, results):
+    """results: per frame of the last timed step (features, descriptors, address of the descriptor buffer they were
+    downloaded into: Feature::desc[] points into it)"""
+    os.makedirs(out_dir, exist_ok=True)
+    rows, descs, counts = [], [], []
+    for i, (feat, desc, base) in enumerate(results):
+        counts.append((len(feat), len(desc)))
+        if not len(feat):
+            continue
+        k = np.arange(4)
+        fi, ki = np.nonzero(feat["num_ori"][:, None] > k[None, :])
+        didx = (feat["desc_ptr"][fi, ki].astype(np.int64) - base) // 512
+        kp = np.stack([np.full(len(fi), i, np.float32), feat["octave"][fi].astype(np.float32), feat["x"][fi], feat["y"][fi],
+                       feat["sigma"][fi], feat["ori"][fi, ki]], axis=1).astype(np.float32)
+        order = np.lexsort(kp.T[::-1])          # the extrema's arrival order varies from run to run; sorted rows do not
+        rows.append(kp[order])
+        descs.append(desc[didx[order]])
+    kp = np.concatenate(rows) if rows else np.zeros((0, 6), np.float32)
+    desc = np.concatenate(descs) if descs else np.zeros((0, 128), np.float32)
+    pick = np.sort(np.random.default_rng(0).choice(len(desc), min(len(desc), DUMP_DESC_ROWS), replace=False))
+    np.save(os.path.join(out_dir, "keypoints.npy"), kp)
+    np.save(os.path.join(out_dir, "descriptors.npy"), desc[pick].astype(np.float32))
+    np.save(os.path.join(out_dir, "descriptor_rows.npy"), pick.astype(np.float64))
+    np.save(os.path.join(out_dir, "counts.npy"), np.array(counts, np.float64).reshape(-1, 2))
 
 
 def run_ours(args, rank, world, local_rank):
@@ -242,30 +268,39 @@ def run_ours(args, rank, world, local_rank):
     dev_frames = [torch.from_numpy(f).cuda() for f in frames]
     # page-locked result buffers (ps_host_alloc): ps_download DMA-copies straight into them
     res = api._PinnedBlock(L, 200000, 200000)
-    feat_buf, desc_buf = res.feat, res.desc
     nf, nd = C.c_int32(), C.c_int32()
 
     def chk(rc):
         if rc != 0:
             raise SystemExit("popsift_b200 error %d: %s" % (rc, L.ps_last_error(ctx).decode()))
 
-    def step_dev():
-        """FRAMES_PER_STEP frames, SLOTS in flight; every job's features + descriptors land on the host."""
+    def step_dev(dest=None, counts_out=None):
+        """FRAMES_PER_STEP frames, SLOTS in flight; every job's features + descriptors land on the host: in the shared
+        page-locked block, or in dest[i] (one page-locked block per frame) when given.  counts_out receives the
+        (features, descriptors) of every frame."""
         tot_f = tot_d = 0
         inflight = []
+
+        def collect(s0, i):
+            chk(L.ps_counts(ctx, s0, C.byref(nf), C.byref(nd)))
+            blk = dest[i] if dest is not None else res
+            if nf.value > blk.n_feat or nd.value > blk.n_desc:
+                raise SystemExit("bench.py: frame %d returned more results than its result block holds" % i)
+            chk(L.ps_download(ctx, s0, blk.feat.ctypes.data, blk.desc.ctypes.data))
+            if counts_out is not None:
+                counts_out.append((nf.value, nd.value))
+            return nf.value, nd.value
+
         for i, df in enumerate(dev_frames):
             s = i % SLOTS
             if len(inflight) == SLOTS:
-                s0 = inflight.pop(0)
-                chk(L.ps_counts(ctx, s0, C.byref(nf), C.byref(nd)))
-                chk(L.ps_download(ctx, s0, feat_buf.ctypes.data, desc_buf.ctypes.data))
-                tot_f += nf.value; tot_d += nd.value
+                f, d = collect(*inflight.pop(0))
+                tot_f += f; tot_d += d
             chk(L.ps_submit_dev_u8(ctx, s, df.data_ptr(), W, W, H))
-            inflight.append(s)
-        for s0 in inflight:
-            chk(L.ps_counts(ctx, s0, C.byref(nf), C.byref(nd)))
-            chk(L.ps_download(ctx, s0, feat_buf.ctypes.data, desc_buf.ctypes.data))
-            tot_f += nf.value; tot_d += nd.value
+            inflight.append((s, i))
+        for s0, i in inflight:
+            f, d = collect(s0, i)
+            tot_f += f; tot_d += d
         return tot_f, tot_d
 
     def barrier():
@@ -277,8 +312,13 @@ def run_ours(args, rank, world, local_rank):
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    for _ in range(args.warmup):
-        step_dev()
+    warm_counts = []
+    for k in range(args.warmup):
+        step_dev(counts_out=warm_counts if k == args.warmup - 1 else None)
+    # --dump-outputs: the last timed step downloads every frame into a page-locked block of its own (sized by the
+    # warm-up, which ran the same frames), so that nothing is copied inside the timed region
+    dump = args.dump_outputs and rank == 0
+    dest = [api._PinnedBlock(L, f, d) for f, d in warm_counts] if dump else None
     barrier()
     launches0 = L.ps_launch_count(ctx)
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -291,8 +331,10 @@ def run_ours(args, rank, world, local_rank):
     t0 = time.perf_counter()
     wall0 = time.time()
     counts = (0, 0)
-    for _ in range(args.steps):
-        counts = step_dev()
+    last_counts = []
+    for k in range(args.steps):
+        last = k == args.steps - 1
+        counts = step_dev(dest if last else None, last_counts if last else None)
     for st in slot_streams:        # ev1 after everything the slots did
         e = torch.cuda.Event()
         e.record(st)
@@ -303,12 +345,16 @@ def run_ours(args, rank, world, local_rank):
     dev_ms = ev0.elapsed_time(ev1)
     launches = L.ps_launch_count(ctx) - launches0
     clocks = sampler.stop(wall0, time.time()) if rank == 0 else None
+    if dump:
+        dump_outputs(args.dump_outputs, [(b.feat[:f], b.desc[:d], b.desc.ctypes.data) for b, (f, d) in zip(dest, last_counts)])
+        for b in dest:
+            b.free()
 
     # ---------------- roofline of the pyramid stage (same context, slot 0 holds the last frame) ----
     chk(L.ps_submit_dev_u8(ctx, 0, dev_frames[0].data_ptr(), W, W, H))
     chk(L.ps_counts(ctx, 0, C.byref(nf), C.byref(nd)))
     s0 = slot_streams[0]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")      # > L2 (126 MB)
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")      # > L2 (50 MB)
     pyr_ms, dom_ms = [], []
     geo = octave_pixels()
     for it in range(3 + 10):
@@ -355,10 +401,10 @@ def run_ours(args, rank, world, local_rank):
         step_e2e()
     barrier()
     t0 = time.perf_counter()
-    for _ in range(max(2, args.steps // 2)):
+    for _ in range(args.steps):
         step_e2e()
     barrier()
-    pinned_wall_ms = (time.perf_counter() - t0) * 1e3 / max(2, args.steps // 2)
+    pinned_wall_ms = (time.perf_counter() - t0) * 1e3 / args.steps
     ps.uninit()
     del pinned
 
@@ -400,7 +446,7 @@ def run_ours(args, rank, world, local_rank):
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "frames_per_step_per_gpu": FRAMES_PER_STEP, "slots": SLOTS,
                    "sharding": "frames across ranks, no collective",
-                   "l2": "working set per frame 3.0 GB of planes >> 126 MB L2; L2 flushed (256 MB fill) before each roofline sample"},
+                   "l2": "working set per frame 3.0 GB of planes >> 50 MB L2; L2 flushed (256 MB fill) before each roofline sample"},
         "wall_ms_per_step": wall_ms / args.steps,
         "features_per_step": counts[0], "descriptors_per_step": counts[1],
         "gpu_launches": int(launches),
@@ -414,14 +460,9 @@ def run_ours(args, rank, world, local_rank):
         "roofline": {"bound": "hbm", "stage": "pyramid (all launches of one frame)", "achieved": alg_bytes_frame / (pyr * 1e-3) / 1e9,
                      "peak": peak, "unit": "GB/s", "frac": alg_bytes_frame / (pyr * 1e-3) / 1e9 / peak, "peak_source": peak_src,
                      "algorithmic_bytes": alg_bytes_frame, "ms": pyr,
-                     # dram__bytes_read.sum + dram__bytes_write.sum of the 26 pyramid launches of one frame, one
-                     # `ncu --set full` capture (profiles/r02_ncu_full_frame_4k.csv); below the algorithmic bytes
-                     # because part of every plane is still dirty in the 126 MB L2 when its consumer starts
-                     "traffic": NCU_PYRAMID_DRAM_BYTES, "traffic_source": NCU_SOURCE,
                      "dominant_kernel": {"name": "march_level_kernel (octave 0, levels 1..5: blur + DoG, avg per launch)",
                                          "algorithmic_bytes": dom_bytes, "ms": dom,
-                                         "achieved": dom_bytes / (dom * 1e-3) / 1e9, "frac": dom_bytes / (dom * 1e-3) / 1e9 / peak,
-                                         "traffic": NCU_LEVEL_DRAM_BYTES}},
+                                         "achieved": dom_bytes / (dom * 1e-3) / 1e9, "frac": dom_bytes / (dom * 1e-3) / 1e9 / peak}},
         "clocks": clocks,
         "numa": NUMA_INFO,
     }
@@ -478,7 +519,7 @@ def run_reference(args, rank, world, local_rank):
         return None
     exe = os.path.join(ROOT, "oracle", "_ref", "ref_dump")
     if not os.path.exists(exe):
-        return {"impl": "reference", "unavailable": "oracle/_ref/ref_dump not built (needs /root/reference at build time)"}
+        return {"impl": "reference", "unavailable": "oracle/_ref/ref_dump not built (needs the reference's sources at build time)"}
     n = max(1, args.gpus)
     try:
         with tempfile.TemporaryDirectory() as td:
@@ -506,7 +547,7 @@ def run_reference(args, rank, world, local_rank):
             "features_per_step": sum(j["features_last_step"] for j in outs), "descriptors_per_step": sum(j["descriptors_last_step"] for j in outs),
             "per_gpu_mpix_per_s": [j["mpix_per_s"] for j in outs],
             "cpu_baseline": {"value": v, "unit": "Mpixels/s", "cores": 2 * n, "kind": "reference",
-                             "sample": "%d frames 3840x2160 per step per GPU, unmodified reference libpopsift (oracle/_ref) on %d B200, "
+                             "sample": "%d frames 3840x2160 per step per GPU, unmodified reference libpopsift (oracle/_ref) on %d H100, "
                                        "2 host threads per GPU" % (FRAMES_PER_STEP, n)},
             "e2e": {"value": v, "unit": "Mpixels/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
 
@@ -520,7 +561,11 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,4 +1,4 @@
-// PopSift / SiftJob for the Blackwell-native drop-in.
+// PopSift / SiftJob for the H100 (sm_90a) drop-in.
 //
 // Same public surface as the reference (reference src/popsift/popsift.h:44-317): construct with a
 // Config, enqueue(w, h, pixels) copies the image and returns a SiftJob the caller owns,

@@ -1,4 +1,4 @@
-// popsift::Config for the Blackwell-native drop-in.
+// popsift::Config for the H100 (sm_90a) drop-in.
 //
 // Same public surface as the reference's popsift::Config (reference src/popsift/sift_conf.h:29-419):
 // public fields octaves / levels / sigma / _edge_limit / verbose, every setter, getter and enum, and

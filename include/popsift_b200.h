@@ -1,5 +1,5 @@
 /*
- * popsift_b200 -- C ABI of the Blackwell-native SIFT extractor.
+ * popsift_b200 -- C ABI of the H100-native (sm_90a) SIFT extractor.
  *
  * This is the drop-in boundary for the hot path of alicevision/popsift:
  *     image -> Gaussian pyramid -> DoG extrema -> orientation -> descriptors.
@@ -194,7 +194,7 @@ int   ps_pointer_device(const void* dev_ptr);
  * DEVICE arrays (e.g. the descriptor arrays filled by ps_download_dev); d_out receives n_left x {best index, second
  * index, accept} with accept = (best / second < 0.8f), also in DEVICE memory.  The call returns when the result is
  * complete.  flags: PS_MATCH_AUTO, or force one implementation (PS_MATCH_EXACT: CUDA cores in the reference's
- * evaluation order; PS_MATCH_TENSOR: tcgen05 tf32x3 candidate pass + exact re-rank). */
+ * evaluation order; PS_MATCH_TENSOR: wgmma tf32x3 candidate pass + exact re-rank). */
 enum { PS_MATCH_AUTO = 0, PS_MATCH_EXACT = 1, PS_MATCH_TENSOR = 2 };
 int ps_match(int device, const ps_descriptor* d_left, int n_left, const ps_descriptor* d_right, int n_right,
              int32_t* d_out, int flags);

@@ -1,9 +1,9 @@
 #!/usr/bin/env bash
 # TEST INFRASTRUCTURE ONLY -- builds the UNMODIFIED reference PopSift, from the
-# sources where they lie under /root/reference, into oracle/_ref/ (git-ignored,
-# but shipped to the GPU box by gpurun).  Nothing of the product links to it.
+# sources where they lie ($POPSIFT_REFERENCE, default /root/reference), into
+# oracle/_ref/ (git-ignored).  Nothing of the product links to it.
 #
-#   oracle/_ref/libpopsift_ref.so   reference library, SASS for sm_100 (+PTX)
+#   oracle/_ref/libpopsift_ref.so   reference library, SASS for sm_90 (+PTX)
 #   oracle/_ref/ref_dump            our driver (oracle/ref_driver.cpp) over the
 #                                   reference's public API (PopSift/enqueue/get)
 #
@@ -46,12 +46,16 @@ SRCS="$S/popsift.cpp $S/features.cu $S/sift_constants.cu $S/sift_conf.cu $S/gaus
  $S/s_desc_iloop.cu $S/s_desc_grid.cu $S/s_desc_igrid.cu $S/s_desc_notile.cu
  $S/common/assist.cu $S/common/plane_2d.cu $S/common/write_plane_2d.cu
  $S/common/debug_macros.cu $S/common/device_prop.cu"
-ARCH="-gencode arch=compute_100,code=sm_100 -gencode arch=compute_100,code=compute_100"
+ARCH="-gencode arch=compute_90,code=sm_90 -gencode arch=compute_90,code=compute_90"
 FLAGS="-std=c++17 -O3 -rdc=true --default-stream legacy -DCCCL_DISABLE_NVTX -DNVTX_DISABLE -w"
 INC="-I$REF/src -I$GEN -I$GEN/popsift"
-if [ ! -f "$OUT/libpopsift_ref.so" ] || [ "${FORCE:-0}" = 1 ]; then
+# a library built with other flags (another architecture) is rebuilt: the stamp records the flags it was built with
+STAMP="$OUT/libpopsift_ref.flags"
+if [ ! -f "$OUT/libpopsift_ref.so" ] || [ "${FORCE:-0}" = 1 ] || [ "$(cat "$STAMP" 2>/dev/null)" != "$FLAGS $ARCH" ]; then
     echo "build_ref: compiling reference library (about 1-2 min)" >&2
+    rm -f "$STAMP"
     nvcc $FLAGS -x cu $ARCH -Xcompiler -fPIC -shared $INC -o "$OUT/libpopsift_ref.so" $SRCS -lcudadevrt
+    printf '%s' "$FLAGS $ARCH" > "$STAMP"
 fi
 nvcc -std=c++17 -O2 $ARCH $INC -o "$OUT/ref_dump" "$HERE/ref_driver.cpp" \
      -L"$OUT" -lpopsift_ref -Xlinker -rpath -Xlinker '$ORIGIN' -lpthread

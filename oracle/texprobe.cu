@@ -1,4 +1,4 @@
-// TEST INFRASTRUCTURE ONLY.  Probes what the B200 texture unit returns for the
+// TEST INFRASTRUCTURE ONLY.  Probes what the GPU texture unit returns for the
 // input-image texture configuration the reference uses (normalized coordinates,
 // bilinear filter, clamp, u8 -> normalized float; /root/reference/src/popsift/s_image.cu:138-167)
 // when addressed the way normalizedSource::horiz does (s_pyramid_build_ra.cu:36-53).

@@ -1,8 +1,8 @@
-"""Builds the product's native code IN-TREE with nvcc for sm_100a (no JIT cache).
+"""Builds the product's native code IN-TREE with nvcc for sm_90a (H100; no JIT cache).
 
     python -m popsift_b200.build            # libpopsift_b200.so + popsift-demo
 
-Outputs (git-ignored, shipped to the GPU box by gpurun):
+Outputs (git-ignored):
     popsift_b200/lib/libpopsift_b200.so     C-ABI (include/popsift_b200.h) + C++ API (include/popsift/*.h)
     popsift_b200/bin/popsift-demo           CLI mirroring the reference's popsift-demo
 """
@@ -21,7 +21,7 @@ OBJ_DIR = os.path.join(PKG, "build")
 LIB = os.path.join(LIB_DIR, "libpopsift_b200.so")
 DEMO = os.path.join(BIN_DIR, "popsift-demo")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "--fmad=false",   # no implicit contraction anywhere; every fma in the kernels is explicit
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
@@ -59,6 +59,11 @@ def _headers():
 def build(verbose: bool = False, force: bool = False) -> str:
     for d in (LIB_DIR, BIN_DIR, OBJ_DIR):
         os.makedirs(d, exist_ok=True)
+    # products of other compiler flags (another architecture) are rebuilt, whatever their timestamps
+    stamp = os.path.join(OBJ_DIR, "flags")
+    flags = " ".join(ARCH + NVCC_FLAGS)
+    if not os.path.exists(stamp) or open(stamp).read() != flags:
+        force = True
     hdrs = _headers()
     objs = []
     procs = []
@@ -107,6 +112,8 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):
         # host-only check of popsift-demo's image reader
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(CSRC, "app"), PGM_CHECK_SRC, pgm_src, "-o", PGM_CHECK])
+    with open(stamp, "w") as f:
+        f.write(flags)
     return LIB
 
 

@@ -92,7 +92,7 @@ float warp_order_sq_dist(const Descriptor& l, const Descriptor& r)
 
 // reference features.cu:282-304: 2-nearest-neighbour search of every descriptor of *this among `other`'s, then one
 // line per descriptor on stdout (show_distance, features.cu:229-277: a device printf there, a host printf here).
-// The search runs on the device (ps_match: tcgen05 tensor-core pass + exact re-rank, or the CUDA-core kernel for small sets).
+// The search runs on the device (ps_match: wgmma tensor-core pass + exact re-rank, or the CUDA-core kernel for small sets).
 void FeaturesDev::match(FeaturesDev* other)
 {
     if (!other) throw std::runtime_error("FeaturesDev::match: null argument");

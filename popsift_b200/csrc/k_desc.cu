@@ -1,4 +1,4 @@
-// Stage 3b -- 128-D descriptors + normalisation + Feature records, hand-written for sm_100a.
+// Stage 3b -- 128-D descriptors + normalisation + Feature records, hand-written for sm_90a.
 //
 // Replaces ext_desc_loop / ext_desc_loop_sub, normalize_histogram<RootSift|L2> and prep_features
 // (reference src/popsift/s_desc_loop.cu:11-158, s_desc_norm_rs.h:41-77, s_desc_norm_l2.h:46-135,

@@ -1,4 +1,4 @@
-// The reference's alternative descriptor extraction modes (Config::DescMode, --desc-mode), for sm_100a:
+// The reference's alternative descriptor extraction modes (Config::DescMode, --desc-mode), for sm_90a:
 //   grid    16 x 16 sample points per cell on the rotated grid, each rounded to the nearest pixel, point-sampled gradient
 //           (reference src/popsift/s_desc_grid.cu:18-122)
 //   igrid   the same grid, unrounded; gradient from four bilinearly interpolated samples one pixel along / across the

@@ -1,4 +1,4 @@
-// Stage 2 -- DoG extrema scan + sub-pixel refinement, hand-written for sm_100a.
+// Stage 2 -- DoG extrema scan + sub-pixel refinement, hand-written for sm_90a.
 //
 // Replaces find_extrema_in_dog / is_extremum / ModeFunctions / solve
 // (reference src/popsift/s_extrema.cu:22-558, s_solve.h:25-86).  One launch covers every
@@ -514,8 +514,8 @@ template <int MODE>
 int launch_scan(const PyramidView& pyr, const Consts& k, InitialExtremum* iext, Counters* ct, cudaStream_t st)
 {
     if (pyr.cands_filled && !dense_choice()) {
-        // resident CTAs per SM: 3 (80 registers: 77.7 us per 4K frame) or 4 (64 registers, spills in the candidate loop:
-        // 84.4 us); POPSIFT_B200_EXTREMA_CTAS=4 for A/B timing
+        // resident CTAs per SM: 3 (80 registers) or 4 (64 registers, spills in the candidate loop);
+        // POPSIFT_B200_EXTREMA_CTAS=4 for A/B timing
         static const int ctas = [] { const char* e = getenv("POPSIFT_B200_EXTREMA_CTAS"); return e && atoi(e) == 4 ? 4 : 3; }();
         if (ctas == 3) cand_extrema_kernel<MODE, 3><<<sm_count() * 3, kScanThreads, 0, st>>>(pyr, k, iext, ct);
         else           cand_extrema_kernel<MODE, 4><<<sm_count() * 4, kScanThreads, 0, st>>>(pyr, k, iext, ct);

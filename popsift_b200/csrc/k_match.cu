@@ -1,4 +1,4 @@
-// Brute-force 2-nearest-neighbour descriptor matcher, hand-written for sm_100a (tcgen05 + TMEM + TMA).
+// Brute-force 2-nearest-neighbour descriptor matcher, hand-written for sm_90a (wgmma + TMA + mbarrier).
 //
 // Replaces FeaturesDev::match -> compute_distance (reference src/popsift/features.cu:165-227,282-304): for every
 // left descriptor the best and second-best right descriptor by squared L2 distance and the ratio test
@@ -10,15 +10,14 @@
 // Pipeline (ps_match):
 //   1. match_split_kernel     a = hi + lo with hi = tf32(a) (round to nearest), lo = a - hi; |b|^2 per right
 //                             descriptor.  Three tf32 products hi.hi + hi.lo + lo.hi give a.b to ~2^-21 relative.
-//   2. match_tc_kernel        one CTA per 128 left descriptors.  The A tile (hi and lo, 128 x 128 floats each) is
-//                             loaded once with TMA (SWIZZLE_128B, K-major) and stays in shared memory; the right
-//                             descriptors stream through a 4-stage TMA ring of [64 descriptors x 32 floats] tiles (hi and lo),
-//                             every CTA starting at a different tile of the right set; ONE thread
-//                             issues tcgen05.mma.kind::tf32 (M = 128, N = 64, K = 8) into a double-buffered fp32
-//                             accumulator in TMEM; four epilogue warps read the accumulator with tcgen05.ld
-//                             (thread = one left descriptor = one TMEM lane) and keep that descriptor's four best
-//                             candidates |b|^2 - 2 a.b in registers.  The n_left x n_right distance matrix never
-//                             touches HBM.  Warp roles: 0 = TMA producer, 1 = MMA issuer + TMEM owner, 2..5 = epilogue.
+//   2. match_tc_kernel        one CTA (three warpgroups) per 128 left descriptors.  The A tile (hi and lo, 128 x 128
+//                             floats each) is loaded once with TMA (SWIZZLE_128B, K-major) and stays in shared memory;
+//                             the right descriptors stream through a 3-stage TMA ring of [128 descriptors x 32 floats]
+//                             tiles (hi and lo).  Warpgroup 0 is the TMA producer (one thread); warpgroups 1 and 2 each
+//                             own 64 left descriptors and issue wgmma.mma_async m64n128k8 tf32 into a register
+//                             accumulator, then keep each of their rows' four best candidates |b|^2 - 2 a.b (a row's
+//                             128 columns are spread over the four lanes of a quad, merged at the end).  The
+//                             n_left x n_right distance matrix never touches HBM.
 //   3. match_rerank_kernel    one warp per left descriptor recomputes the exact float32 distance of its four
 //                             candidates in the reference's own evaluation order (per lane x*x, fma, fma, fma over its
 //                             float4, shuffle-down tree 16, 8, 4, 2, 1) and applies the reference's scan rule
@@ -119,15 +118,16 @@ match_split_kernel(const ps_descriptor* __restrict__ d, int n, int n_pad, float*
 
 // ------------------------------------------------------------------------------------------------ tensor-core pass
 
-constexpr int BM = 128, BN = 128;            // left descriptors per CTA, right descriptors per accumulator tile
+constexpr int BM = 128, BN = 128;            // left descriptors per CTA, right descriptors per tile (= N of one wgmma)
 constexpr int KB = 32;                       // floats per K-block = one 128-byte swizzle span
 constexpr int NKB = 128 / KB;                // K-blocks per descriptor
-constexpr int UMMA_K = 8;                    // tf32: 32 bytes per instruction
-constexpr int TILE_BYTES = BM * KB * 4;      // 16 KB: one [128 rows x 128 bytes] operand tile of the left set
-constexpr int TC_THREADS = 192;              // 6 warps
+constexpr int MMA_K = 8;                     // tf32: 32 bytes per instruction
+constexpr int TILE_BYTES = 128 * KB * 4;     // 16 KB: one [128 rows x 128 bytes] operand tile
+constexpr int STAGES = 3;                    // B ring: one K-block of a right tile (hi and lo) per stage
+constexpr int TC_THREADS = 384;              // warpgroup 0 = TMA producer, warpgroups 1 and 2 = MMA + epilogue
 constexpr int kCand = 4;                     // candidates kept per left descriptor
-constexpr size_t TC_SMEM = (size_t)2 * NKB * TILE_BYTES + 64 * 1024;    // A hi/lo resident + 64 KB B ring = 192 KB
-constexpr int TMEM_COLS = 2 * BN;            // two fp32 accumulators of 128 columns
+// A hi/lo resident (128 KB) + the ring (96 KB) + slack to align the dynamic buffer to 1024 bytes
+constexpr size_t TC_SMEM = (size_t)2 * NKB * TILE_BYTES + (size_t)STAGES * 2 * TILE_BYTES + 1024;
 
 __device__ __forceinline__ unsigned s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mb_init(uint64_t* b, unsigned n) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(s32(b)), "r"(n) : "memory"); }
@@ -148,45 +148,32 @@ __device__ __forceinline__ void tma_tile(void* dst, const CUtensorMap* map, int 
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  :: "r"(s32(dst)), "l"(reinterpret_cast<unsigned long long>(map)), "r"(k0), "r"(row0), "r"(s32(bar)) : "memory");
 }
-// K-major operand tile, SWIZZLE_128B, rows 128 bytes wide, 8-row groups 1024 bytes apart (cute::UMMA::SmemDescriptor:
-// start >> 4 in [0,14), LBO = 1 in [16,30), SBO = 1024 >> 4 in [32,46), version 1 in [46,48), layout SWIZZLE_128B = 2 in [61,64))
-__device__ __forceinline__ uint64_t umma_desc(const void* tile)
+// wgmma shared-memory descriptor of a K-major operand tile, SWIZZLE_128B, rows 128 bytes wide, 8-row groups 1024 bytes
+// apart: start >> 4 in [0,14), LBO = 1 in [16,30) (unused by swizzled K-major layouts), SBO = 1024 >> 4 in [32,46),
+// layout SWIZZLE_128B = 1 in [62,64)
+__device__ __forceinline__ uint64_t gmma_desc(const void* tile)
 {
-    return (uint64_t)((s32(tile) >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((s32(tile) >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// cute::UMMA::InstrDescriptor: D = F32 (1 << 4), A = B = TF32 (2 << 7, 2 << 10), both K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-__host__ __device__ constexpr unsigned idesc_for(int n) { return (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(n >> 3) << 17) | ((unsigned)(BM >> 4) << 24); }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
 
-__device__ __forceinline__ void umma_tf32(unsigned d_tmem, uint64_t a_desc, uint64_t b_desc, unsigned accumulate, unsigned kIdesc)
+// D[64 x 128] (+)= A[64 x 8] . B[128 x 8]^T, tf32 in, fp32 accumulate, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc, int accumulate)
 {
-    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}"
-                 :: "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(kIdesc), "r"(accumulate) : "memory");
+    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %66, 0;\n"
+                 " wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(s32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// 32 consecutive fp32 columns of this thread's TMEM lane: issue (the registers are valid after tmem_ld_wait)
-__device__ __forceinline__ void tmem_ld32_issue(unsigned taddr, unsigned (&r)[32])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Candidate bookkeeping of one left descriptor (one epilogue thread): the four smallest keys seen so far and where they
-// came from.  A key is the approximate distance |b|^2 - 2 a.b with its 5 low mantissa bits replaced by the column's index
-// inside its group of 32 (relative 2^-18: far below what separates candidates that matter, the exact re-rank follows), so
-// that the group's minimum -- a branch-free FMNMX tree -- carries its own position.
+// Candidate bookkeeping of one left descriptor: the four smallest keys seen so far and where they came from.  A key is
+// the approximate distance |b|^2 - 2 a.b with its 5 low mantissa bits replaced by the column's position e (0..31) among
+// the 32 columns of the tile this thread holds for the row (relative 2^-18: far below what separates candidates that
+// matter, the exact re-rank follows), so that the minimum -- a branch-free FMNMX tree -- carries its own position.
 struct Top4 {
     float t0 = INFINITY, t1 = INFINITY, t2 = INFINITY, t3 = INFINITY;
     int i0 = -1, i1 = -1, i2 = -1, i3 = -1;
@@ -197,25 +184,31 @@ struct Top4 {
             if (t2 < t1) { tf = t1; t1 = t2; t2 = tf; ti = i1; i1 = i2; i2 = ti;
                 if (t1 < t0) { tf = t0; t0 = t1; t1 = tf; ti = i0; i0 = i1; i1 = ti; } } }
     }
+    // the four best of this list and lane (lane ^ x)'s, whose columns are disjoint from ours
+    __device__ __forceinline__ void merge_xor(int x)
+    {
+        const float pt[4] = {__shfl_xor_sync(0xffffffffu, t0, x), __shfl_xor_sync(0xffffffffu, t1, x),
+                             __shfl_xor_sync(0xffffffffu, t2, x), __shfl_xor_sync(0xffffffffu, t3, x)};
+        const int pi[4] = {__shfl_xor_sync(0xffffffffu, i0, x), __shfl_xor_sync(0xffffffffu, i1, x),
+                           __shfl_xor_sync(0xffffffffu, i2, x), __shfl_xor_sync(0xffffffffu, i3, x)};
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (pt[k] < t3) insert(pt[k], pi[k]);
+    }
 };
 
-// one group of 32 columns: r = raw accumulator bits (a.b), rn = |b|^2 of the 32 columns, nb = index of the group's first column
-__device__ __forceinline__ void top4_group(Top4& T, const unsigned (&r)[32], const float4 (&rn)[8], int nb)
+// One row of the accumulator fragment: in the m64nNk8 layout a thread holds, for its row, the columns
+// 8b + 2q + u (b = 0..15, u = 0..1, q = lane % 4) in d[4b + 2h + u] (h = 0: row lane / 4, h = 1: that row + 8).  The keys
+// are formed in place; e = 2b + u is the column's position among the thread's 32.
+template <int HALF>
+__device__ __forceinline__ void top4_row(Top4& T, float (&d)[64], int nb, int q)
 {
-    float k[32];
-#pragma unroll
-    for (int i4 = 0; i4 < 8; ++i4) {
-        const float rr[4] = {rn[i4].x, rn[i4].y, rn[i4].z, rn[i4].w};
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const int i = i4 * 4 + u;
-            const float val = fmaf(-2.0f, __uint_as_float(r[i]), rr[u]);          // |b|^2 - 2 a.b  (+inf for padding)
-            k[i] = __uint_as_float((__float_as_uint(val) & 0xffffffe0u) | (unsigned)i);   // padding: inf -> inf (i = 0) or NaN
-        }
-    }
     float m[16];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) m[i] = fminf(k[i], k[i + 16]);                  // fminf drops NaNs
+    for (int i = 0; i < 16; ++i) {
+        const float a = d[4 * (i >> 1) + 2 * HALF + (i & 1)], b = d[4 * ((i + 16) >> 1) + 2 * HALF + (i & 1)];
+        m[i] = fminf(a, b);                                                        // fminf drops NaNs
+    }
 #pragma unroll
     for (int w = 8; w >= 1; w >>= 1)
 #pragma unroll
@@ -223,37 +216,27 @@ __device__ __forceinline__ void top4_group(Top4& T, const unsigned (&r)[32], con
     float best = m[0];
     // rare after the first tiles: the k-th best of n random items improves about 4 / n of the time
     while (best < T.t3) {
-        T.insert(best, nb + (int)(__float_as_uint(best) & 31u));
-        float nxt = INFINITY;                                                  // the group's next key above `best`
+        const int e = (int)(__float_as_uint(best) & 31u);
+        T.insert(best, nb + 8 * (e >> 1) + 2 * q + (e & 1));
+        float nxt = INFINITY;                                                  // the next key above `best`
 #pragma unroll
-        for (int i = 0; i < 32; ++i) nxt = (k[i] > best) ? fminf(nxt, k[i]) : nxt;
+        for (int i = 0; i < 32; ++i) {
+            const float k = d[4 * (i >> 1) + 2 * HALF + (i & 1)];
+            nxt = (k > best) ? fminf(nxt, k) : nxt;
+        }
         best = nxt;
     }
 }
 
-// Every CTA walks the right set from a different tile, so that the CTAs do not all pull the same lines out of the same L2
-// slices at the same moment (the candidate selection does not depend on the order of the tiles)
-template <bool ROT>
-__device__ __forceinline__ int tile_of(int j, int n_tiles)
-{
-    if (!ROT) return j;
-    const int t = j + (int)((blockIdx.x * 37u) % (unsigned)n_tiles);
-    return t >= n_tiles ? t - n_tiles : t;
-}
-
-// BNS = right descriptors per stage of the B ring and N of one MMA (128: two 32 KB stages; 64: four 16 KB stages)
-template <int BNS, bool ROT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 match_tc_kernel(const __grid_constant__ CUtensorMap tm_lhi, const __grid_constant__ CUtensorMap tm_llo,
                 const __grid_constant__ CUtensorMap tm_rhi, const __grid_constant__ CUtensorMap tm_rlo,
                 const float* __restrict__ rnorm, int nl, int n_tiles, int32_t* __restrict__ cand)
 {
-    constexpr int BTILE_BYTES = BNS * KB * 4;                   // one [BNS rows x 128 bytes] operand tile of the right set
-    constexpr int STAGES = 64 * 1024 / (2 * BTILE_BYTES);
-    constexpr unsigned kIdesc = idesc_for(BNS);
-    extern __shared__ __align__(1024) uint8_t smem[];          // SWIZZLE_128B tiles: 1024-byte aligned
-    __shared__ __align__(8) uint64_t a_full, b_full[4], b_empty[4], acc_full[2], acc_empty[2];
-    __shared__ unsigned tmem_base_s;
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t a_full, b_full[STAGES], b_empty[STAGES];
+    // SWIZZLE_128B tiles: 1024-byte aligned
+    uint8_t* smem = smem_raw + ((1024u - (s32(smem_raw) & 1023u)) & 1023u);
     uint8_t* A_hi = smem;                                       // NKB tiles
     uint8_t* A_lo = smem + NKB * TILE_BYTES;
     uint8_t* B_st = smem + 2 * NKB * TILE_BYTES;                // [STAGES][hi, lo]
@@ -262,118 +245,94 @@ match_tc_kernel(const __grid_constant__ CUtensorMap tm_lhi, const __grid_constan
 
     if (threadIdx.x == 0) {
         mb_init(&a_full, 1);
-        for (int s = 0; s < STAGES; ++s) { mb_init(&b_full[s], 1); mb_init(&b_empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { mb_init(&acc_full[b], 1); mb_init(&acc_empty[b], 4); }
+        for (int s = 0; s < STAGES; ++s) { mb_init(&b_full[s], 1); mb_init(&b_empty[s], 8); }   // 8 consumer warps
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {                                            // TMEM: allocated and freed by the same warp
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(s32(&tmem_base_s)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const unsigned tmem_base = tmem_base_s;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ===== TMA producer (one thread) =====
-        if (lane == 0) {
+        if (threadIdx.x == 0) {
             mb_expect(&a_full, 2 * NKB * TILE_BYTES);
             for (int kb = 0; kb < NKB; ++kb) {
                 tma_tile(A_hi + kb * TILE_BYTES, &tm_lhi, kb * KB, m0, &a_full);
                 tma_tile(A_lo + kb * TILE_BYTES, &tm_llo, kb * KB, m0, &a_full);
             }
             int s = 0; unsigned ph = 0;
-            for (int j = 0; j < n_tiles; ++j) {
-                const int jt = tile_of<ROT>(j, n_tiles);
-                for (int half = 0; half < BN / BNS; ++half)
-                    for (int kb = 0; kb < NKB; ++kb) {
-                        mb_wait(&b_empty[s], ph ^ 1u);           // the MMAs that read this slot have completed
-                        mb_expect(&b_full[s], 2 * BTILE_BYTES);
-                        tma_tile(B_st + (s * 2 + 0) * BTILE_BYTES, &tm_rhi, kb * KB, jt * BN + half * BNS, &b_full[s]);
-                        tma_tile(B_st + (s * 2 + 1) * BTILE_BYTES, &tm_rlo, kb * KB, jt * BN + half * BNS, &b_full[s]);
-                        if (++s == STAGES) { s = 0; ph ^= 1u; }
-                    }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one thread issues; the warp stays converged on the barriers) =====
-        mb_wait(&a_full, 0);
-        tc_fence_after();
-        int s = 0; unsigned ph = 0;
-        for (int j = 0; j < n_tiles; ++j) {
-            const int buf = j & 1;
-            mb_wait(&acc_empty[buf], ((unsigned)(j >> 1) & 1u) ^ 1u);   // the epilogue has drained this accumulator
-            tc_fence_after();
-            for (int half = 0; half < BN / BNS; ++half) {
-                const unsigned d_tmem = tmem_base + (unsigned)(buf * BN + half * BNS);
+            for (int j = 0; j < n_tiles; ++j)
                 for (int kb = 0; kb < NKB; ++kb) {
-                    mb_wait(&b_full[s], ph);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint64_t a_hi = umma_desc(A_hi + kb * TILE_BYTES), a_lo = umma_desc(A_lo + kb * TILE_BYTES);
-                        const uint64_t b_hi = umma_desc(B_st + (s * 2 + 0) * BTILE_BYTES), b_lo = umma_desc(B_st + (s * 2 + 1) * BTILE_BYTES);
-#pragma unroll
-                        for (int k8 = 0; k8 < KB / UMMA_K; ++k8) {
-                            const uint64_t adv = (uint64_t)(k8 * UMMA_K * 4 / 16);      // +32 bytes inside the swizzle span
-                            umma_tf32(d_tmem, a_hi + adv, b_hi + adv, (kb | k8) != 0 ? 1u : 0u, kIdesc);
-                            umma_tf32(d_tmem, a_hi + adv, b_lo + adv, 1u, kIdesc);
-                            umma_tf32(d_tmem, a_lo + adv, b_hi + adv, 1u, kIdesc);
-                        }
-                        umma_commit(&b_empty[s]);                // slot free once these MMAs have read it
-                        if (half == BN / BNS - 1 && kb == NKB - 1) umma_commit(&acc_full[buf]);
-                    }
-                    __syncwarp();
+                    mb_wait(&b_empty[s], ph ^ 1u);               // the MMAs that read this slot have completed
+                    mb_expect(&b_full[s], 2 * TILE_BYTES);
+                    tma_tile(B_st + (s * 2 + 0) * TILE_BYTES, &tm_rhi, kb * KB, j * BN, &b_full[s]);
+                    tma_tile(B_st + (s * 2 + 1) * TILE_BYTES, &tm_rlo, kb * KB, j * BN, &b_full[s]);
                     if (++s == STAGES) { s = 0; ph ^= 1u; }
                 }
-            }
         }
-    } else {
-        // ===== epilogue: thread = one left descriptor = one TMEM lane =====
-        const int q = warp & 3;                                  // TMEM lanes 32q .. 32q+31 belong to warps with warp % 4 == q
-        const int row = m0 + q * 32 + lane;
-        Top4 T;
-        const unsigned lane_base = tmem_base + ((unsigned)(q * 32) << 16);
-        for (int j = 0; j < n_tiles; ++j) {
-            const int buf = j & 1;
-            const int nb0 = tile_of<ROT>(j, n_tiles) * BN;
-            const float4* rn4 = reinterpret_cast<const float4*>(rnorm + nb0);
-            // |b|^2 of the first group is on its way while the accumulator is still being written
-            float4 rnA[8], rnB[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) rnA[i] = __ldg(rn4 + i);
-            mb_wait(&acc_full[buf], (unsigned)(j >> 1) & 1u);
-            tc_fence_after();
-            // four groups of 32 columns, two register sets: group g+1 is loaded from TMEM while group g is processed
-            unsigned ra[32], rb[32];
-            tmem_ld32_issue(lane_base + (unsigned)(buf * BN), ra);
-            tmem_ld_wait();
-            tmem_ld32_issue(lane_base + (unsigned)(buf * BN + 32), rb);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) rnB[i] = __ldg(rn4 + 8 + i);
-            top4_group(T, ra, rnA, nb0);
-            tmem_ld_wait();
-            tmem_ld32_issue(lane_base + (unsigned)(buf * BN + 64), ra);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) rnA[i] = __ldg(rn4 + 16 + i);
-            top4_group(T, rb, rnB, nb0 + 32);
-            tmem_ld_wait();
-            tmem_ld32_issue(lane_base + (unsigned)(buf * BN + 96), rb);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) rnB[i] = __ldg(rn4 + 24 + i);
-            top4_group(T, ra, rnA, nb0 + 64);
-            tmem_ld_wait();
-            // the accumulator has been read completely: hand it back before the last group is processed
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mb_arrive(&acc_empty[buf]);
-            top4_group(T, rb, rnB, nb0 + 96);
-        }
-        if (row < nl) *reinterpret_cast<int4*>(cand + (size_t)row * kCand) = make_int4(T.i0, T.i1, T.i2, T.i3);
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "n"(TMEM_COLS) : "memory");
+    // ===== consumers: warpgroup c owns left rows 64c .. 64c+63 of the CTA's 128 =====
+    const int c = (warp >> 2) - 1;
+    const int q = lane & 3;
+    const int row0 = m0 + 64 * c + 16 * (warp & 3) + (lane >> 2);      // fragment rows: row0 (h = 0) and row0 + 8 (h = 1)
+    const unsigned a_off = (unsigned)(64 * c * 128);                   // 64 rows x 128 bytes into every A tile
+    Top4 T0, T1;
+    float d[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) d[i] = 0.0f;
+    mb_wait(&a_full, 0);
+    int s = 0; unsigned ph = 0;
+    for (int j = 0; j < n_tiles; ++j) {
+        const int nb0 = j * BN;
+        // |b|^2 of the thread's 32 columns is on its way while the MMAs run
+        float2 rn[16];
+#pragma unroll
+        for (int b = 0; b < 16; ++b) rn[b] = __ldg(reinterpret_cast<const float2*>(rnorm + nb0 + 8 * b + 2 * q));
+        int prev = -1;
+        for (int kb = 0; kb < NKB; ++kb) {
+            mb_wait(&b_full[s], ph);
+            wg_fence();
+            const uint64_t a_hi = gmma_desc(A_hi + kb * TILE_BYTES + a_off), a_lo = gmma_desc(A_lo + kb * TILE_BYTES + a_off);
+            const uint64_t b_hi = gmma_desc(B_st + (s * 2 + 0) * TILE_BYTES), b_lo = gmma_desc(B_st + (s * 2 + 1) * TILE_BYTES);
+#pragma unroll
+            for (int k8 = 0; k8 < KB / MMA_K; ++k8) {
+                const uint64_t adv = (uint64_t)(k8 * MMA_K * 4 / 16);          // +32 bytes inside the swizzle span
+                wgmma_tf32(d, a_hi + adv, b_hi + adv, (kb | k8) != 0);
+                wgmma_tf32(d, a_hi + adv, b_lo + adv, 1);
+                wgmma_tf32(d, a_lo + adv, b_hi + adv, 1);
+            }
+            wg_commit();
+            if (prev >= 0) {                                   // the previous K-block's MMAs have read their slot
+                wg_wait<1>();
+                __syncwarp();
+                if (lane == 0) mb_arrive(&b_empty[prev]);
+            }
+            prev = s;
+            if (++s == STAGES) { s = 0; ph ^= 1u; }
+        }
+        wg_wait<0>();
+        __syncwarp();
+        if (lane == 0) mb_arrive(&b_empty[prev]);
+        // keys |b|^2 - 2 a.b (+inf for padding columns, whose |b|^2 is +inf) with the column position in the low bits
+#pragma unroll
+        for (int b = 0; b < 16; ++b)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                    const int i = 4 * b + 2 * h + u;
+                    const float val = fmaf(-2.0f, d[i], u ? rn[b].y : rn[b].x);
+                    d[i] = __uint_as_float((__float_as_uint(val) & 0xffffffe0u) | (unsigned)(2 * b + u));   // padding: inf or NaN
+                }
+        top4_row<0>(T0, d, nb0, q);
+        top4_row<1>(T1, d, nb0, q);
+    }
+    // the four lanes of a quad hold disjoint columns of the same two rows
+    T0.merge_xor(1); T1.merge_xor(1);
+    T0.merge_xor(2); T1.merge_xor(2);
+    if (q == 0) {
+        if (row0 < nl) *reinterpret_cast<int4*>(cand + (size_t)row0 * kCand) = make_int4(T0.i0, T0.i1, T0.i2, T0.i3);
+        if (row0 + 8 < nl) *reinterpret_cast<int4*>(cand + (size_t)(row0 + 8) * kCand) = make_int4(T1.i0, T1.i1, T1.i2, T1.i3);
+    }
 }
 
 // exact distances of the candidates, in increasing index order, through the reference's scan
@@ -463,30 +422,15 @@ int run_match(const ps_descriptor* l, int nl, const ps_descriptor* r, int nr, in
     rhi = reinterpret_cast<float*>(ws + 2 * lb); rlo = reinterpret_cast<float*>(ws + 2 * lb + rb);
     rnorm = reinterpret_cast<float*>(ws + 2 * lb + 2 * rb);
     cand = reinterpret_cast<int32_t*>(ws + 2 * lb + 2 * rb + (size_t)nr_pad * 4);
-    // POPSIFT_B200_MATCH_RING = 128 | 64 | 128r | 64r: rows per B stage, r = every CTA starts at a different tile (A/B timing)
-    static const int ring_cfg = [] {
-        const char* e = getenv("POPSIFT_B200_MATCH_RING");
-        if (!e) return 0;
-        return (atoi(e) == 64 ? 1 : 0) | (strchr(e, 'r') ? 2 : 0);
-    }();
-    const int bns = (ring_cfg & 1) ? 64 : 128;
     CUtensorMap m_lhi, m_llo, m_rhi, m_rlo;
     const bool ok = make_tmap_2d(&m_lhi, lhi, 128, nl_pad, 512, KB, BM, true) && make_tmap_2d(&m_llo, llo, 128, nl_pad, 512, KB, BM, true) &&
-                    make_tmap_2d(&m_rhi, rhi, 128, nr_pad, 512, KB, bns, true) && make_tmap_2d(&m_rlo, rlo, 128, nr_pad, 512, KB, bns, true);
+                    make_tmap_2d(&m_rhi, rhi, 128, nr_pad, 512, KB, BN, true) && make_tmap_2d(&m_rlo, rlo, 128, nr_pad, 512, KB, BN, true);
     if (!ok) { cudaFreeAsync(ws, st); *err = "cuTensorMapEncodeTiled failed (matcher)"; return -1; }
-    static_assert(TC_SMEM + 2048 <= 227 * 1024, "matcher shared memory");
+    static_assert(TC_SMEM + 1024 <= 227 * 1024, "matcher shared memory");
     match_split_kernel<<<(nl_pad + 3) / 4, 128, 0, st>>>(l, nl, nl_pad, lhi, llo, nullptr);
     match_split_kernel<<<(nr_pad + 3) / 4, 128, 0, st>>>(r, nr, nr_pad, rhi, rlo, rnorm);
-    auto launch = [&](auto kern) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
-        kern<<<nl_pad / BM, TC_THREADS, TC_SMEM, st>>>(m_lhi, m_llo, m_rhi, m_rlo, rnorm, nl, n_tiles, cand);
-    };
-    switch (ring_cfg) {
-        case 1:  launch(match_tc_kernel<64, false>); break;
-        case 2:  launch(match_tc_kernel<128, true>); break;
-        case 3:  launch(match_tc_kernel<64, true>); break;
-        default: launch(match_tc_kernel<128, false>); break;
-    }
+    cudaFuncSetAttribute(match_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
+    match_tc_kernel<<<nl_pad / BM, TC_THREADS, TC_SMEM, st>>>(m_lhi, m_llo, m_rhi, m_rlo, rnorm, nl, n_tiles, cand);
     match_rerank_kernel<<<(nl + 3) / 4, 128, 0, st>>>(l, nl, r, nr, cand, out);
     cudaFreeAsync(ws, st);
     return 4;

@@ -1,4 +1,4 @@
-// Stage 3a -- dominant orientations, hand-written for sm_100a.
+// Stage 3a -- dominant orientations, hand-written for sm_90a.
 //
 // Replaces ori_par + ori_prefix_sum (reference src/popsift/s_orientation.cu:75-362,
 // s_gradiant.h:55-69, common/warp_bitonic_sort.h, common/excl_blk_prefix_sum.h).

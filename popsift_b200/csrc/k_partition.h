@@ -10,11 +10,11 @@
 namespace psb {
 
 // Work partition: strips of TW columns x segments of whole chunk-rows (Q rows), ONE wave of CTAs
-// (148 SMs x 4 resident CTAs).  CTAs of one segment index handle neighbouring strips, so CTAs that run
+// (SMs x 4 resident CTAs).  CTAs of one segment index handle neighbouring strips, so CTAs that run
 // side by side touch the same image rows and every DRAM page of a row is streamed by neighbouring CTAs
-// at about the same time (a strip-major split of the same work measured ~30 % slower).
+// at about the same time.
 //
-// S strips seldom divide the 592 slots: with nh segments of uh chunk-rows per strip, S*nh CTAs leave
+// S strips seldom divide the slots (4 per SM: 528 on an H100 SXM): with nh segments of uh chunk-rows per strip, S*nh CTAs leave
 // slots (and whole SMs' worth of issue bandwidth) idle.  The spare slots go to `light` strips, spread
 // evenly over the image, that are cut into nl > nh shorter segments (ul chunk-rows).  Block b < S*nh is
 // (strip b % S, segment b / S); the remaining blocks are the extra segments of the light strips.

@@ -1,4 +1,4 @@
-// Stage 1 -- Gaussian scale-space pyramid + DoG, hand-written for sm_100a.
+// Stage 1 -- Gaussian scale-space pyramid + DoG, hand-written for sm_90a.
 //
 // What the reference does with 13 launches per octave through textures and surfaces
 // (normalizedSource::horiz, absoluteSource::horiz/vert, get_by_2_pick_every_second, make_dog;

@@ -1,4 +1,4 @@
-// Stage 1, fast path -- "column-marching" fused Gaussian level kernel for sm_100a.
+// Stage 1, fast path -- "column-marching" fused Gaussian level kernel for sm_90a.
 //
 // One CTA (128 threads) owns a strip of TW=128 output columns and marches down a segment of rows in
 // chunks of Q=16 rows.  Per chunk:
@@ -12,8 +12,8 @@
 //   2. row pass: thread = (row, 16-column group); a 16+2R wide register window is loaded with
 //      conflict-free LDS.128 (row stride with an odd number of float4 -- the TMA box is that wide) and
 //      produces 16 outputs -> ring buffer HB of row-filtered lines (Q+2R lines);
-//   3. column pass: thread = (pair of adjacent columns, 8 rows); the 8+2R ring lines are loaded once and every
-//      tap is one packed FFMA2; the outputs lag the input by R rows: level l, DoG[l-1] (= out - centre
+//   3. column pass: thread = (pair of adjacent columns, 8 rows); the 8+2R ring lines are loaded once (one
+//      64-bit load per line) and every tap is two FFMAs; the outputs lag the input by R rows: level l, DoG[l-1] (= out - centre
 //      source, still in the staging buffers) and, for level L, the 2:1 decimated level 0 of the next octave.
 // Every source row is read from HBM once (+2R warm-up rows per segment), every output written once;
 // the row-filtered intermediate never leaves shared memory.
@@ -195,14 +195,12 @@ __device__ __forceinline__ void row_pass(const float* __restrict__ S, float* __r
 
 // ---- column pass: ring -> outputs ------------------------------------------------------------
 //
-// Thread = (pair of adjacent columns, half of the chunk's rows).  Both columns ride in one 64-bit
-// register pair, so every tap is ONE packed FFMA2 (fma.rn.f32x2; the tap weight is a scalar
-// uniform-register operand): half the FP32 issue slots of the scalar form, identical IEEE results.
+// Thread = (pair of adjacent columns, half of the chunk's rows).  Both columns ride in one float2: one
+// 64-bit shared-memory load per ring line and one 64-bit store per output row; every tap is two FFMAs
+// with the same scalar weight.
 
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pack2(float lo, float hi) { f32x2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void unpack2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 fma2(f32x2 a, float g, f32x2 c) { return make_float2(__fmaf_rn(a.x, g, c.x), __fmaf_rn(a.y, g, c.y)); }
 
 constexpr int QH = Q / 2;   // output rows per thread in the column pass
 
@@ -222,20 +220,18 @@ __device__ __forceinline__ void col_emit(const f32x2 (&win)[QH + 2 * R], const f
     unsigned pm = 0;
 #pragma unroll
     for (int jj = 0; jj < QH; ++jj) {
-        f32x2 acc = pack2(0.0f, 0.0f);
+        f32x2 acc = make_float2(0.0f, 0.0f);
 #pragma unroll
         for (int off = R; off > 0; --off) {
-            const f32x2 g2 = pack2(t.g[off], t.g[off]);
-            acc = fma2(win[jj + R - off], g2, acc);
-            acc = fma2(win[jj + R + off], g2, acc);
+            acc = fma2(win[jj + R - off], t.g[off], acc);
+            acc = fma2(win[jj + R + off], t.g[off], acc);
         }
-        acc = fma2(win[jj + R], pack2(t.g[0], t.g[0]), acc);
+        acc = fma2(win[jj + R], t.g[0], acc);
         const int j = jbase + jj;                       // row of the chunk's output block (0..Q-1)
         const bool ok = !GUARD || (col_in && y_first + j >= ys && y_first + j < ye);
         if (ok) {
             *reinterpret_cast<f32x2*>(pd) = acc;
-            float a0, a1;
-            unpack2(acc, a0, a1);
+            const float a0 = acc.x, a1 = acc.y;
             if (WRITE_DOG) {
                 // centre source row: chunk-relative row j-R lives in the current (j >= R) or previous buffer
                 const float* cp = (j >= R) ? Scur + (j - R) * G::SWP : Sprev + (j - R + Q) * G::SWP;
@@ -604,7 +600,7 @@ bool uniform_choice()
     return v;
 }
 
-Partition make_partition(int W, int H, int slots = 0)     // one wave: SMs x 4 resident CTAs (592 on B200)
+Partition make_partition(int W, int H, int slots = 0)     // one wave: SMs x 4 resident CTAs (528 on H100 SXM)
 {
     return psb::make_partition(W, H, TW, Q, slots > 0 ? slots : 4 * sm_count(), uniform_choice());
 }
@@ -616,9 +612,9 @@ int level0_slots()
     return v > 0 ? v : 6 * sm_count();
 }
 
-// POPSIFT_B200_PDL=1 launches the level kernels with programmatic dependent launch.  Off by default: measured
-// 0.794 ms (on) vs 0.777 ms (off) for the 4K pyramid -- the early-launched CTAs of the next level take the slots the
-// side stream's ready kernels (levels L+1, L+2 of the previous octave) would otherwise run in.
+// POPSIFT_B200_PDL=1 launches the level kernels with programmatic dependent launch.  Off by default: the
+// early-launched CTAs of the next level take the slots the side stream's ready kernels (levels L+1, L+2 of the
+// previous octave) would otherwise run in.
 bool pdl_choice()
 {
     static const bool v = [] { const char* e = getenv("POPSIFT_B200_PDL"); return e && e[0] == '1'; }();

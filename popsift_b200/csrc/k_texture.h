@@ -1,4 +1,4 @@
-// What the B200 texture unit returns for the reference's input textures, as device functions.
+// What the texture unit returns for the reference's input textures, as device functions.
 // Measured with oracle/texprobe.cu, restated in oracle/sift_oracle.c (orc_tex_u8 / orc_tex_f32) and pinned
 // by tests/golden/texture_pairs.npz, tests/golden/texture_float.npz.
 #pragma once

@@ -350,11 +350,11 @@ int psb::sm_count()
     static std::mutex mu;
     static int cached[64] = {};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); return 148; }
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); return 132; }
     std::lock_guard<std::mutex> g(mu);
     if (cached[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) { cudaGetLastError(); n = 148; }
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) { cudaGetLastError(); n = 132; }
         cached[dev] = n;
     }
     return cached[dev];

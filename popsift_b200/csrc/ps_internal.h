@@ -106,7 +106,7 @@ inline float extrema_threshold(const Consts& k)
     return k.sift_mode == PS_MODE_OPENCV ? floorf(k.threshold) : 1.6f * k.threshold;
 }
 
-// multiprocessors of the CURRENT device (cudaDeviceProp::multiProcessorCount, cached per device; 148 on B200):
+// multiprocessors of the CURRENT device (cudaDeviceProp::multiProcessorCount, cached per device; 132 on H100 SXM):
 // every fixed grid and the one-wave partition of the pyramid kernels are sized from it
 int sm_count();
 

@@ -11,7 +11,7 @@ for p in (HERE, ROOT):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
 
 
 def _have_gpu() -> bool:

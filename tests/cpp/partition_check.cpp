@@ -1,14 +1,16 @@
 // Host check of the marching kernels' work partition (popsift_b200/csrc/k_partition.h): for a sweep of
 // plane sizes every (strip, row) must be covered by exactly one block, no block may be empty beyond
-// the ones `locate` rejects, and the grid must fit the slots whenever a single wave is possible.
+// the ones `locate` rejects, and the grid must fit the slots whenever a single wave is possible.  Slot counts: 4 resident
+// CTAs x 132 SMs (H100 SXM) and x 148 SMs (a larger part), so that both light / heavy strip splits are exercised.
 #include "k_partition.h"
 #include <cstdio>
 #include <vector>
 
 int main()
 {
-    const int TW = 128, Q = 16, slots = 592;
+    const int TW = 128, Q = 16;
     long checked = 0;
+    for (int slots : {528, 592})
     for (int uniform = 0; uniform < 2; ++uniform)
         for (int W = 1; W <= 16384; W += (W < 300 ? 7 : 97))
             for (int H = 1; H <= 9000; H += (H < 200 ? 5 : 131)) {
@@ -44,8 +46,11 @@ int main()
                     }
                 ++checked;
             }
-    const psb::Partition p4k = psb::make_partition(7680, 4320, TW, Q, slots, false);
-    std::printf("OK %ld partitions; 7680x4320: S=%d nh=%d uh=%d nl=%d ul=%d heavy=%d B=%d\n", checked, p4k.strips, p4k.nh,
-                p4k.uh, p4k.nl, p4k.ul, p4k.heavy, p4k.B);
+    std::printf("OK %ld partitions\n", checked);
+    for (int slots : {528, 592}) {
+        const psb::Partition p4k = psb::make_partition(7680, 4320, TW, Q, slots, false);
+        std::printf("7680x4320 slots=%d: S=%d nh=%d uh=%d nl=%d ul=%d heavy=%d B=%d\n", slots, p4k.strips, p4k.nh, p4k.uh, p4k.nl,
+                    p4k.ul, p4k.heavy, p4k.B);
+    }
     return 0;
 }

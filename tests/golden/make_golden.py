@@ -1,9 +1,9 @@
 """Turns the raw outputs of the UNMODIFIED reference (run on a B200 by
 tools/gpu_ref_golden.sh through oracle/_ref/ref_dump and oracle/_ref/texprobe,
-results in gpurun_out/ref1/) into the small committed fixtures in tests/golden/.
+results in ref_out/ref1/) into the small committed fixtures in tests/golden/.
 
-    /usr/local/graft/bin/gpurun --timeout 900 -- 'bash tools/gpu_ref_golden.sh'
-    python tests/golden/make_golden.py gpurun_out/ref1
+    bash tools/gpu_ref_golden.sh                       (on a GPU machine)
+    python tests/golden/make_golden.py ref_out/ref1
 
 Fixtures:
   planes_f256.npz     sha256 of every Gaussian / DoG plane of the 256x192 frame (seed 3), full
@@ -11,9 +11,7 @@ Fixtures:
   feat_*.npz          reference features (+descriptors) for the named frame / config
   texture_pairs.npz   what the B200 texture unit returns for the reference's input texture
                       configuration: fraction-0 for 256 values, fraction-0.5 for all (a,b) pairs
-  ref_timings.json    reference wall-clock numbers measured in the same call (context only)
 """
-import glob
 import hashlib
 import json
 import os
@@ -64,13 +62,7 @@ def main(src):
     y = np.frombuffer(data, np.float32, n2, 8 + 4 * n)
     np.savez_compressed(os.path.join(HERE, "texture_pairs.npz"), x_half=x[:65536].reshape(256, 256),
                         frac0=x[65536:], y_half=y.reshape(256, 256))
-    tim = {}
-    for fn in glob.glob(os.path.join(src, "bench_ref_*.json")):
-        tim[os.path.basename(fn)[:-5]] = json.loads(open(fn).read())
-    tim["gpu"] = open(os.path.join(src, "gpu.txt")).read().strip().splitlines()[-1]
-    tim["host_cores"] = int(open(os.path.join(src, "nproc.txt")).read())
-    json.dump(tim, open(os.path.join(HERE, "ref_timings.json"), "w"), indent=1)
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else "gpurun_out/ref1")
+    main(sys.argv[1] if len(sys.argv) > 1 else "ref_out/ref1")

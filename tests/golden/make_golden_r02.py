@@ -1,9 +1,9 @@
 """Round-2 fixtures: turns the raw outputs of the UNMODIFIED reference (run on a B200 by
 tools/gpu_ref_golden_r02.sh through oracle/_ref/ref_dump and oracle/_ref/texprobe, results in
-gpurun_out/ref2/) into the small committed files in tests/golden/.
+ref_out/ref2/) into the small committed files in tests/golden/.
 
-    /usr/local/graft/bin/gpurun --timeout 1200 -- 'bash tools/gpu_ref_golden_r02.sh'
-    python tests/golden/make_golden_r02.py gpurun_out/ref2
+    bash tools/gpu_ref_golden_r02.sh                   (on a GPU machine)
+    python tests/golden/make_golden_r02.py ref_out/ref2
 
 Fixtures:
   texture_float.npz            what the B200 texture unit returns for the reference's FLOAT input texture
@@ -143,11 +143,11 @@ def main(src):
             out[tag + "_r16"] = r16[sel][:, xs, :].astype(np.uint16)
             out[tag + "_meta"], out[tag + "_up"] = np.array([w, h, W0, H0, maxoff], np.int32), np.float32(up)
         np.savez_compressed(os.path.join(HERE, "texture_coords.npz"), **out)
-    # ---- Config::ScaleDirect (tools/gpu_round2_p.sh: ref_dump --direct-scaling --log on the 256x192 frame; the 640x480
-    # output is saved by tests/test_gpu_parity.py::test_direct_scaling_vs_oracle_and_live_reference)
+    # ---- Config::ScaleDirect (ref_dump --direct-scaling --log on the 256x192 frame and on the 640x480 frame of
+    # tests/test_gpu_parity.py::test_direct_scaling_vs_oracle_and_live_reference)
     save_feat(src, "ref_direct_f256.bin", "f256_direct")
     save_feat(os.path.dirname(src.rstrip("/")), "ref_direct_640.bin", "f640_direct")
-    # --gauss-mode relative (tools/gpu_round2_t.sh), the unnormalized linear float texture probe (tools/gpu_round2_s.sh)
+    # --gauss-mode relative, the unnormalized linear float texture probe (`texprobe lcoords`)
     save_feat(src, "ref_relative_f256.bin", "f256_relative")
     save_feat(os.path.dirname(src.rstrip("/")), "ref_vlfeat_direct_640.bin", "f640_vlfeat_direct")
     fn = os.path.join(src, "ref_relative_f256_planes.json")
@@ -162,13 +162,13 @@ def main(src):
         o = np.frombuffer(data, np.float32, n, 16 + 8 * n)
         sel = np.r_[np.arange(0, 17 * 8192, 5), np.arange(17 * 8192, n, 3)]
         np.savez_compressed(os.path.join(HERE, "texture_lcoords.npz"), W=np.int32(W), H=np.int32(H), xy=q[sel], out=o[sel])
-    # --gauss-mode fixed9 / fixed15 (tools/gpu_round2_u.sh)
+    # --gauss-mode fixed9 / fixed15
     for m in ("fixed9", "fixed15"):
         save_feat(src, "ref_%s_f256.bin" % m, "f256_%s" % m)
         fn = os.path.join(src, "ref_%s_f256_planes.json" % m)
         if os.path.exists(fn):
             json.dump(json.load(open(fn)), open(os.path.join(HERE, "planes_f256_%s.json" % m), "w"), indent=0)
-    # --gauss-mode vlfeat-direct (tools/gpu_round2_r.sh)
+    # --gauss-mode vlfeat-direct
     save_feat(src, "ref_vlfeat_direct_f256.bin", "f256_vlfeat_direct")
     fn = os.path.join(src, "ref_vlfeat_direct_f256_planes.json")
     if os.path.exists(fn):
@@ -179,4 +179,4 @@ def main(src):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else "gpurun_out/ref2")
+    main(sys.argv[1] if len(sys.argv) > 1 else "ref_out/ref2")

@@ -5,6 +5,8 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may import 
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
+import json
 import os
 import struct
 import subprocess
@@ -200,6 +202,22 @@ def read_ref_features(path: str, with_rev: bool = False):
     assert data[off:off + 4] == b"PSR1"
     rev = np.frombuffer(data, dtype="<i4", count=nd, offset=off + 4).copy()
     return feat, desc, rev
+
+
+def ref_golden(name: str):
+    """A stored run of the reference (tests/golden/live/<name>.npz, written by tests/golden/make_golden_live.py) ->
+    (feat[REF_FEATURE_DTYPE], desc[n_desc, 128] with NaN rows where the descriptor was not kept, planes
+    {"octave_level": (rows, cols, sha256)} of the run's --log plane dumps)."""
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live", name + ".npz"))
+    desc = np.full((int(z["n_desc"][0]), 128), np.nan, np.float32)
+    desc[z["desc_rows"]] = z["desc"]
+    planes = {k: tuple(v) for k, v in json.loads(bytes(z["planes"]).decode()).items()}
+    return z["feat"], desc, planes
+
+
+def plane_id(p: np.ndarray):
+    """(rows, cols, sha256) of a plane, as ref_golden stores them"""
+    return (p.shape[0], p.shape[1], hashlib.sha256(np.ascontiguousarray(p, dtype="<f4").tobytes()).hexdigest())
 
 
 def flatten(feat, desc):

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Parity of the BENCHMARK workload itself (runs on the B200 box): the 32 synthetic 3840x2160 frames of
+"""Parity of the BENCHMARK workload itself (runs on a GPU machine): the 32 synthetic 3840x2160 frames of
 bench.py, default Config (PopSift mode, RootSift, octaves=5, levels=3), through
   * the unmodified reference (oracle/_ref/ref_dump), TWICE  -> its own run-to-run jitter,
   * this library.

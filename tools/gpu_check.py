@@ -1,5 +1,5 @@
-"""Verbose parity + timing report for the GPU box (diagnostics, not a test):
-    gpurun -- 'python tools/gpu_check.py > gpurun_out/check.txt 2>&1'
+"""Verbose parity + timing report (diagnostics, not a test; needs a GPU):
+    python tools/gpu_check.py > check.txt 2>&1
 Compares the CUDA path with the CPU oracle plane by plane, extremum by extremum, and with the
 reference library itself (oracle/_ref/ref_dump) when present."""
 import os

@@ -1,8 +1,8 @@
 #!/usr/bin/env bash
-# Runs on the GPU box (via gpurun): reference outputs + texture probe -> gpurun_out/ref1/
+# Runs on a GPU machine: reference outputs + texture probe -> ref_out/ref1/
 set -uo pipefail
 cd "$(dirname "$0")/.."
-O=gpurun_out/ref1; mkdir -p $O
+O=ref_out/ref1; mkdir -p $O
 nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm,memory.total --format=csv > $O/gpu.txt 2>&1
 nproc > $O/nproc.txt
 R=$PWD/oracle/_ref

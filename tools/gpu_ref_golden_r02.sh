@@ -1,12 +1,12 @@
 #!/usr/bin/env bash
-# Runs on the GPU box (via gpurun): round-2 reference outputs -> gpurun_out/ref2/
+# Runs on a GPU machine: round-2 reference outputs -> ref_out/ref2/
 #   OpenCV SiftMode, float images (+ float texture probe), grid filter, descriptor modes, the brute-force
 #   matcher (FeaturesDev::match) and device-resident results, the synthetic affine set (BASELINE configs[4]
 #   stand-in), and the parity of the benchmark workload itself (tools/bench_parity.py).
 # tests/golden/make_golden_r02.py turns the small files into committed fixtures.
 set -uo pipefail
 cd "$(dirname "$0")/.."
-O=gpurun_out/ref2; mkdir -p $O
+O=ref_out/ref2; mkdir -p $O
 R=$PWD/oracle/_ref
 nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm --format=csv > $O/gpu.txt 2>&1
 python -m popsift_b200.synth 256 192 3 $O/f256.pgm

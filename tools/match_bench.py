@@ -68,7 +68,7 @@ def main():
     res["roofline"] = {"bound": "tensor", "achieved": res["tensor_tflops"], "peak": bf16 / 2, "unit": "TFLOP/s",
                        "frac": res["tensor_tflops"] / (bf16 / 2),
                        "peak_source": "MEASURED_PEAKS.json bf16_tflops / 2 (tf32 issues at half the bf16 rate)",
-                       "note": "whole ps_match call (split + tcgen05 pass + re-rank, one CTA per 128 left descriptors: %d CTAs on 148 SMs)" % ((nl + 127) // 128)}
+                       "note": "whole ps_match call (split + wgmma pass + re-rank, one CTA per 128 left descriptors: %d CTAs)" % ((nl + 127) // 128)}
     L.ps_dev_free(d_out)
     pm.uninit()
     print(json.dumps(res))

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """The columns of an `ncu --set full ... --page raw --csv` export that the roofline discussion uses, one line per launch.
 
-    python tools/ncu_summary.py full_frame_raw.csv > profiles/rNN_ncu_full_summary.tsv
+    python tools/ncu_summary.py full_frame_raw.csv > ncu_full_summary.tsv
 """
 import csv
 import re

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Where do the last-bit differences of orientation angles come from?  (runs on the B200 box)
+"""Where do the last-bit differences of orientation angles come from?  (runs on a GPU machine)
 
 Four 4K benchmark frames through the reference (5 octaves, twice; and 2 octaves: the same octave-0/1 data in a different
 launch context) and through this library with the orientation kernel in several launch shapes (environment toggles of

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-kernel SASS opcode histogram of the product library (evidence for profiles/rNN_sass_summary.txt).
+"""Per-kernel SASS opcode histogram of the product library.
 
     python tools/sass_hist.py [lib.so] [--filter SUBSTR] [--top N] [--all]
 
@@ -7,7 +7,7 @@ Runs `cuobjdump -sass` on the library, demangles nothing (the mangled names carr
 arguments), and prints for every kernel: instruction count, registers are NOT in SASS (see
 `cuobjdump -res-usage`), and the opcode histogram collapsed to the mnemonic before the first '.'.
 The lines that matter for the north_star claims are marked: UTMALDG / UBLKCP (TMA), SYNCS (mbarrier),
-LDGSTS (cp.async), FFMA2 (packed FP32), UTCHMMA / UTCQMMA / LDTM (tcgen05 + TMEM), ATOMS / ATOMG / RED.
+LDGSTS (cp.async), HGMMA (warpgroup MMA), ATOMS / ATOMG / RED.
 """
 from __future__ import annotations
 
@@ -18,8 +18,7 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-MARK = ("UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "LDGSTS", "FFMA2", "FADD2", "FMUL2", "UTCHMMA", "UTCQMMA", "UTCIMMA",
-        "UTCMMA", "LDTM", "STTM", "UTCBAR", "ATOMS", "ATOMG", "RED", "HMMA", "ELECT", "UTCATOMSWS", "UTCCP")
+MARK = ("UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "LDGSTS", "HGMMA", "WARPGROUP", "ATOMS", "ATOMG", "RED", "HMMA", "ELECT")
 
 
 def histogram(lib):
