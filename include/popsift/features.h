@@ -4,6 +4,7 @@
 #pragma once
 
 #include <iostream>
+#include <utility>
 #include <vector>
 
 #define ORIENTATION_MAX_COUNT 4
@@ -105,5 +106,11 @@ public:
     Descriptor* getDescriptors() { return _ori; }
     int*        getReverseMap() { return _rev; }
 };
+
+/// 2-nearest-neighbour matching of many pairs in one call (an addition to the reference's interface; C ABI
+/// ps_match_batch): entry p equals sets[pairs[p].first]->matchIndices(sets[pairs[p].second], flags).  Every set is
+/// prepared once per group of pairs and all pairs share one tensor-core launch; flags as for ps_match.
+std::vector<std::vector<int>> matchPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                         int flags = 0);
 
 } // namespace popsift

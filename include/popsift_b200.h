@@ -198,6 +198,17 @@ int   ps_pointer_device(const void* dev_ptr);
 enum { PS_MATCH_AUTO = 0, PS_MATCH_EXACT = 1, PS_MATCH_TENSOR = 2 };
 int ps_match(int device, const ps_descriptor* d_left, int n_left, const ps_descriptor* d_right, int n_right,
              int32_t* d_out, int flags);
+/* 2-NN matching of many pairs of descriptor sets in one call (an addition to the reference's interface).  d_sets[i]
+ * (DEVICE, on `device`, n_desc[i] descriptors) for i < n_sets; pairs = n_pairs x {left set, right set} (i == j allowed).
+ * d_sets, n_desc and pairs are host arrays.  d_out (DEVICE) receives, for pair p, n_desc[pairs[2p]] rows {best, second,
+ * accept} starting at row sum_{q<p} n_desc[pairs[2q]]: row by row what ps_match(device, d_sets[l], n_desc[l], d_sets[r],
+ * n_desc[r], ..., flags) gives.  Empty left sets contribute no rows; an empty right set gives rows (0, 0, 0).
+ * PS_MATCH_EXACT runs the CUDA-core kernel pair by pair; PS_MATCH_AUTO / PS_MATCH_TENSOR split every set once per group
+ * of pairs and run all pairs' tensor-core work in one persistent launch, then one re-rank launch.  Returns when the
+ * result is complete; PS_ERR_ARG for negative counts, a set index out of range, a null pointer with a count > 0, or a
+ * set that is not device memory on `device`. */
+int ps_match_batch(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc,
+                   int n_pairs, const int32_t* pairs, int32_t* d_out, int flags);
 /* page-locked host memory for images and results (thin wrappers of cudaHostAlloc / cudaFreeHost).
  * ps_submit_* and ps_download detect page-locked buffers and copy straight from / into them; pageable
  * buffers are staged through the slot's own pinned buffers (one extra host memcpy). */

@@ -57,7 +57,7 @@ EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps
            "ps_last_error", "ps_submit_u8", "ps_submit_f32", "ps_submit_dev_u8", "ps_counts", "ps_download",
            "ps_sync", "ps_debug_plane", "ps_debug_extrema", "ps_slot_geometry", "ps_set_timing", "ps_stage_ms",
            "ps_launch_count", "ps_slot_stream", "ps_run_pyramid_only", "ps_run_level_only", "ps_host_alloc", "ps_host_free",
-           "ps_download_dev", "ps_dev_alloc", "ps_dev_free", "ps_dev_to_host", "ps_wait_input", "ps_match", "ps_pointer_device", "ps_host_to_dev",
+           "ps_download_dev", "ps_dev_alloc", "ps_dev_free", "ps_dev_to_host", "ps_wait_input", "ps_match", "ps_match_batch", "ps_pointer_device", "ps_host_to_dev",
            "ps_debug_level0_plan", "ps_format_gauss_tables"]
 
 _lib = None
@@ -89,6 +89,8 @@ def load_library():
     L.ps_sync.argtypes = [C.c_void_p, C.c_int]
     L.ps_wait_input.argtypes = [C.c_void_p, C.c_int]
     L.ps_match.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+    if hasattr(L, "ps_match_batch"):    # absent from builds that predate it (POPSIFT_B200_LIB A/B runs)
+        L.ps_match_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -437,6 +439,51 @@ def match_descriptors(left: np.ndarray, right: np.ndarray, flags=0, device=0) ->
     finally:
         for p in bufs:
             lib.ps_dev_free(p)
+
+
+def match_pairs(sets, pairs, flags=0, device=None) -> list:
+    """2-NN matching of many pairs in one call (C ABI ps_match_batch; an addition to the reference's interface).
+    `sets` holds FeaturesDev objects or host (n, 128) float32 arrays (copied through device memory); `pairs` is a list of
+    (left, right) indices into `sets`.  Entry p is the (n_left, 3) int32 array (best, second, accept) that
+    match_descriptors(sets[l], sets[r], flags) gives."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    owned, ptrs, counts = [], [], []
+    try:
+        for s in sets:
+            if isinstance(s, FeaturesDev):
+                ptrs.append(s.getDescriptors()); counts.append(s.getDescriptorCount())
+                continue
+            a = np.ascontiguousarray(s, np.float32).reshape(-1, 128)
+            p = lib.ps_dev_alloc(max(a.nbytes, 4))
+            if not p:
+                raise PopSiftError("ps_dev_alloc failed")
+            owned.append(p)
+            if a.nbytes and lib.ps_host_to_dev(p, a.ctypes.data, a.nbytes) != 0:
+                raise PopSiftError("host -> device copy failed")
+            ptrs.append(p); counts.append(len(a))
+        if device is None:
+            device = next((lib.ps_pointer_device(p) for p, n in zip(ptrs, counts) if n > 0), 0)
+            device = max(0, device)
+        rows = [counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs]
+        out = np.zeros((sum(rows), 3), np.int32)
+        d_out = lib.ps_dev_alloc(max(out.nbytes, 4))
+        if not d_out:
+            raise PopSiftError("ps_dev_alloc failed")
+        owned.append(d_out)
+        c_sets = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
+        c_n = (C.c_int32 * max(len(counts), 1))(*counts)
+        c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
+        rc = lib.ps_match_batch(device, len(ptrs), c_sets, c_n, len(pairs), c_pairs, d_out, flags)
+        if rc != 0:
+            raise PopSiftError("ps_match_batch error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        if out.nbytes and lib.ps_dev_to_host(out.ctypes.data, d_out, out.nbytes) != 0:
+            raise PopSiftError("device -> host copy failed")
+    finally:
+        for p in owned:
+            lib.ps_dev_free(p)
+    starts = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
+    return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
 
 
 class SiftJob:

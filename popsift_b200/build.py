@@ -38,6 +38,10 @@ API_BENCH_SRC = os.path.join(ROOT, "tests", "cpp", "api_bench.cpp")
 PART_CHECK = os.path.join(BIN_DIR, "partition_check")
 PART_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "partition_check.cpp")
 PGM_CHECK = os.path.join(BIN_DIR, "pgmread_check")
+MATCH_PLAN_CHECK = os.path.join(BIN_DIR, "match_plan_check")
+MATCH_PLAN_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_plan_check.cpp")
+MATCH_PAIRS_CHECK = os.path.join(BIN_DIR, "match_pairs_check")
+MATCH_PAIRS_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_pairs_check.cpp")
 PGM_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "pgmread_check.cpp")
 
 
@@ -108,6 +112,14 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if os.path.exists(PART_CHECK_SRC) and (force or _newer(PART_CHECK, [PART_CHECK_SRC, part_hdr])):
         # host-only sweep of the marching kernels' work partition (no CUDA, no library)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + CSRC, PART_CHECK_SRC, "-o", PART_CHECK])
+    plan_hdr = os.path.join(CSRC, "k_match_plan.h")
+    if os.path.exists(MATCH_PLAN_CHECK_SRC) and (force or _newer(MATCH_PLAN_CHECK, [MATCH_PLAN_CHECK_SRC, plan_hdr])):
+        # host-only sweep of the batched matcher's planner (no CUDA, no library)
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + CSRC, MATCH_PLAN_CHECK_SRC, "-o", MATCH_PLAN_CHECK])
+    if os.path.exists(MATCH_PAIRS_CHECK_SRC) and (force or _newer(MATCH_PAIRS_CHECK, [MATCH_PAIRS_CHECK_SRC, LIB] + hdrs)):
+        # popsift::matchPairs against FeaturesDev::matchIndices through the C++ API
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), MATCH_PAIRS_CHECK_SRC, "-o", MATCH_PAIRS_CHECK,
+                               "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
     pgm_src = os.path.join(CSRC, "app", "pgmread.cpp")
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):
         # host-only check of popsift-demo's image reader

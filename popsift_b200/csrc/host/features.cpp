@@ -133,6 +133,42 @@ std::vector<int> FeaturesDev::matchIndices(FeaturesDev* other, int flags)
     return m;
 }
 
+std::vector<std::vector<int>> matchPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs, int flags)
+{
+    std::vector<const ps_descriptor*> d_sets(sets.size());
+    std::vector<int32_t> n_desc(sets.size());
+    for (size_t i = 0; i < sets.size(); ++i) {
+        if (!sets[i]) throw std::runtime_error("popsift::matchPairs: null set");
+        d_sets[i] = reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors());
+        n_desc[i] = sets[i]->getDescriptorCount();
+    }
+    std::vector<int32_t> flat(2 * pairs.size());
+    std::vector<std::vector<int>> out(pairs.size());
+    size_t rows = 0;
+    for (size_t p = 0; p < pairs.size(); ++p) {
+        const int l = pairs[p].first, r = pairs[p].second;
+        if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error("popsift::matchPairs: set index out of range");
+        flat[2 * p] = l; flat[2 * p + 1] = r;
+        out[p].assign((size_t)std::max(n_desc[l], 0) * 3, 0);
+        rows += out[p].size() / 3;
+    }
+    if (rows == 0) return out;
+    int32_t* d_out = static_cast<int32_t*>(ps_dev_alloc(rows * 3 * sizeof(int32_t)));
+    if (!d_out) throw std::runtime_error("popsift::matchPairs: failed to allocate device memory");
+    int dev = 0;
+    for (size_t i = 0; i < sets.size(); ++i)
+        if (n_desc[i] > 0) { dev = std::max(0, ps_pointer_device(d_sets[i])); break; }
+    int rc = ps_match_batch(dev, (int)sets.size(), d_sets.data(), n_desc.data(), (int)pairs.size(), flat.data(), d_out, flags);
+    size_t row = 0;
+    for (size_t p = 0; p < pairs.size() && rc == PS_OK; ++p) {
+        rc = ps_dev_to_host(out[p].data(), d_out + 3 * row, out[p].size() * sizeof(int32_t));
+        row += out[p].size() / 3;
+    }
+    ps_dev_free(d_out);
+    if (rc != PS_OK) throw std::runtime_error(std::string("popsift::matchPairs failed: ") + ps_last_error(nullptr));
+    return out;
+}
+
 void FeaturesHost::pin() {}
 void FeaturesHost::unpin() {}
 

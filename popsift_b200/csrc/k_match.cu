@@ -7,32 +7,40 @@
 // n_left times).  This is the one dense contraction of the library:
 //     |a - b|^2 = |a|^2 + |b|^2 - 2 a.b        ->   S = A . B^T  on the tensor cores.
 //
-// Pipeline (ps_match):
-//   1. match_split_kernel     a = hi + lo with hi = tf32(a) (round to nearest), lo = a - hi; |b|^2 per right
-//                             descriptor.  Three tf32 products hi.hi + hi.lo + lo.hi give a.b to ~2^-21 relative.
-//   2. match_tc_kernel        one CTA (three warpgroups) per 128 left descriptors.  The A tile (hi and lo, 128 x 128
-//                             floats each) is loaded once with TMA (SWIZZLE_128B, K-major) and stays in shared memory;
-//                             the right descriptors stream through a 3-stage TMA ring of [128 descriptors x 32 floats]
-//                             tiles (hi and lo).  Warpgroup 0 is the TMA producer (one thread); warpgroups 1 and 2 each
-//                             own 64 left descriptors and issue wgmma.mma_async m64n128k8 tf32 into a register
-//                             accumulator, then keep each of their rows' four best candidates |b|^2 - 2 a.b (a row's
-//                             128 columns are spread over the four lanes of a quad, merged at the end).  The
-//                             n_left x n_right distance matrix never touches HBM.
-//   3. match_rerank_kernel    one warp per left descriptor recomputes the exact float32 distance of its four
-//                             candidates in the reference's own evaluation order (per lane x*x, fma, fma, fma over its
-//                             float4, shuffle-down tree 16, 8, 4, 2, 1) and applies the reference's scan rule
-//                             (strict <, ties keep the lower index) and ratio test.
-// The result equals the reference's except when three or more right descriptors lie within ~4e-6 (relative) of the second
-// best (the candidate pass could then miss the reference's pick among exact near-ties).
+// Pipeline (ps_match = a batch of one pair, ps_match_batch = many; per group of pairs planned by k_match_plan.h):
+//   1. match_split_kernel     a = hi + lo with hi = tf32(a) (round to nearest), lo = a - hi, and |a|^2, for every set of
+//                             the group once, into one pooled hi plane, lo plane and norm array (each set's rows padded
+//                             to a multiple of 128; padding rows have norm +inf).  Three tf32 products hi.hi + hi.lo +
+//                             lo.hi give a.b to ~2^-21 relative.
+//   2. match_tc_kernel        persistent, one CTA (three warpgroups) per SM drawing work items (pair, 128-row left
+//                             tile, contiguous chunk of right tiles).  The A tile (hi and lo, 128 x 128 floats each) is
+//                             loaded with TMA (SWIZZLE_128B, K-major) and stays in shared memory while consecutive items
+//                             share it; the right tiles stream through a 3-stage TMA ring of [128 descriptors x 32
+//                             floats] tiles (hi and lo).  Both are row offsets into the same two tensor maps.  Warpgroup
+//                             0 is the TMA producer (one thread); warpgroups 1 and 2 each own 64 left descriptors and
+//                             issue wgmma.mma_async m64n128k8 tf32 into a register accumulator, then keep each of their
+//                             rows' four best candidates |b|^2 - 2 a.b per item (a row's 128 columns are spread over the
+//                             four lanes of a quad, merged at the end).  The n_left x n_right distance matrix never
+//                             touches HBM.
+//   3. match_rerank_kernel    one warp per (pair, left row) gathers the four candidates of each of the row's chunks and
+//                             recomputes their exact float32 distances in the reference's own evaluation order (per lane
+//                             x*x, fma, fma, fma over its float4, shuffle-down tree 16, 8, 4, 2, 1), in increasing index
+//                             order, with the reference's scan rule (strict <, ties keep the lower index) and ratio test.
+// The result equals the reference's except when three or more right descriptors of one chunk lie within ~4e-6 (relative)
+// of the second best (the candidate pass could then miss the reference's pick among exact near-ties); more chunks keep
+// more candidates and can only bring the result closer.
 // match_exact_kernel is the same computation on CUDA cores (one warp per left descriptor over all right ones): used
 // for small problems and as the in-library cross-check (PS_MATCH_EXACT).
 #include "ps_internal.h"
+#include "k_match_plan.h"
 #include "tma_util.h"
 
+#include <algorithm>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <vector>
 
 namespace psb {
 
@@ -94,26 +102,33 @@ __device__ __forceinline__ float to_tf32(float v)
     return __uint_as_float(u);
 }
 
-// one warp per descriptor: hi / lo planes (rows padded with zero descriptors up to n_pad) and, for the right set,
-// |b|^2 (+inf for the padding rows so that they never become candidates)
+// one set of a group: its descriptors and its first row in the pooled planes (its padded rows run up to the next set's)
+struct SplitSet { const ps_descriptor* d; int32_t n; int32_t row; };
+
+// one warp per pooled row: hi / lo planes (each set's rows padded with zero descriptors to a multiple of 128) and |b|^2
+// (+inf for the padding rows so that they never become candidates)
 __global__ void __launch_bounds__(128)
-match_split_kernel(const ps_descriptor* __restrict__ d, int n, int n_pad, float* __restrict__ hi, float* __restrict__ lo, float* __restrict__ norm)
+match_split_kernel(const SplitSet* __restrict__ sets, int n_sets, int rows, float* __restrict__ hi, float* __restrict__ lo, float* __restrict__ norm)
 {
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
-    if (row >= n_pad) return;
+    if (row >= rows) return;
+    int a = 0, b = n_sets - 1;                                    // the last set that starts at or before `row`
+    while (a < b) { const int m = (a + b + 1) >> 1; if (sets[m].row <= row) a = m; else b = m - 1; }
+    const SplitSet ss = sets[a];
+    const int n = ss.n;
+    const ps_descriptor* d = ss.d;
+    const int local = row - ss.row;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (row < n) v = __ldg(reinterpret_cast<const float4*>(d + row) + lane);
+    if (local < n) v = __ldg(reinterpret_cast<const float4*>(d + local) + lane);
     const float4 h = make_float4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w));
     const float4 lw = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
     reinterpret_cast<float4*>(hi + (size_t)row * 128)[lane] = h;
     reinterpret_cast<float4*>(lo + (size_t)row * 128)[lane] = lw;
-    if (norm) {
-        float s = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, v.w * v.w)));
+    float s = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, v.w * v.w)));
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (lane == 0) norm[row] = row < n ? s : INFINITY;
-    }
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) norm[row] = local < n ? s : INFINITY;
 }
 
 // ------------------------------------------------------------------------------------------------ tensor-core pass
@@ -228,24 +243,27 @@ __device__ __forceinline__ void top4_row(Top4& T, float (&d)[64], int nb, int q)
     }
 }
 
+// Persistent: CTA b runs the work items b, b + gridDim.x, ... (k_match_plan.h), each one 128-row left tile (A) against
+// a contiguous run of right tiles (B), both addressed as rows of the same pooled hi / lo planes.  The producer and the
+// consumers walk the same item sequence; the B ring's stage / phase carries across items, and A is reloaded only when
+// the next item's left tile differs (a_empty: both consumer warpgroups' MMAs on the old A have completed).
 __global__ void __launch_bounds__(TC_THREADS, 1)
-match_tc_kernel(const __grid_constant__ CUtensorMap tm_lhi, const __grid_constant__ CUtensorMap tm_llo,
-                const __grid_constant__ CUtensorMap tm_rhi, const __grid_constant__ CUtensorMap tm_rlo,
-                const float* __restrict__ rnorm, int nl, int n_tiles, int32_t* __restrict__ cand)
+match_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
+                const float* __restrict__ norm, const MatchItem* __restrict__ items, int n_items, int32_t* __restrict__ cand)
 {
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t a_full, b_full[STAGES], b_empty[STAGES];
+    __shared__ __align__(8) uint64_t a_full, a_empty, b_full[STAGES], b_empty[STAGES];
     // SWIZZLE_128B tiles: 1024-byte aligned
     uint8_t* smem = smem_raw + ((1024u - (s32(smem_raw) & 1023u)) & 1023u);
     uint8_t* A_hi = smem;                                       // NKB tiles
     uint8_t* A_lo = smem + NKB * TILE_BYTES;
     uint8_t* B_st = smem + 2 * NKB * TILE_BYTES;                // [STAGES][hi, lo]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.x * BM;
 
     if (threadIdx.x == 0) {
         mb_init(&a_full, 1);
-        for (int s = 0; s < STAGES; ++s) { mb_init(&b_full[s], 1); mb_init(&b_empty[s], 8); }   // 8 consumer warps
+        mb_init(&a_empty, 8);                                                                    // 8 consumer warps
+        for (int s = 0; s < STAGES; ++s) { mb_init(&b_full[s], 1); mb_init(&b_empty[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -253,114 +271,160 @@ match_tc_kernel(const __grid_constant__ CUtensorMap tm_lhi, const __grid_constan
     if (warp < 4) {
         // ===== TMA producer (one thread) =====
         if (threadIdx.x == 0) {
-            mb_expect(&a_full, 2 * NKB * TILE_BYTES);
-            for (int kb = 0; kb < NKB; ++kb) {
-                tma_tile(A_hi + kb * TILE_BYTES, &tm_lhi, kb * KB, m0, &a_full);
-                tma_tile(A_lo + kb * TILE_BYTES, &tm_llo, kb * KB, m0, &a_full);
-            }
             int s = 0; unsigned ph = 0;
-            for (int j = 0; j < n_tiles; ++j)
-                for (int kb = 0; kb < NKB; ++kb) {
-                    mb_wait(&b_empty[s], ph ^ 1u);               // the MMAs that read this slot have completed
-                    mb_expect(&b_full[s], 2 * TILE_BYTES);
-                    tma_tile(B_st + (s * 2 + 0) * TILE_BYTES, &tm_rhi, kb * KB, j * BN, &b_full[s]);
-                    tma_tile(B_st + (s * 2 + 1) * TILE_BYTES, &tm_rlo, kb * KB, j * BN, &b_full[s]);
-                    if (++s == STAGES) { s = 0; ph ^= 1u; }
+            int a_cur = -1; unsigned a_ph = 0;
+            for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+                const MatchItem w = items[it];
+                if (w.a_row != a_cur) {
+                    if (a_cur >= 0) { mb_wait(&a_empty, a_ph); a_ph ^= 1u; }   // the consumers are done with the old A
+                    a_cur = w.a_row;
+                    mb_expect(&a_full, 2 * NKB * TILE_BYTES);
+                    for (int kb = 0; kb < NKB; ++kb) {
+                        tma_tile(A_hi + kb * TILE_BYTES, &tm_hi, kb * KB, w.a_row, &a_full);
+                        tma_tile(A_lo + kb * TILE_BYTES, &tm_lo, kb * KB, w.a_row, &a_full);
+                    }
                 }
+                for (int j = 0; j < w.b_tiles; ++j)
+                    for (int kb = 0; kb < NKB; ++kb) {
+                        mb_wait(&b_empty[s], ph ^ 1u);               // the MMAs that read this slot have completed
+                        mb_expect(&b_full[s], 2 * TILE_BYTES);
+                        tma_tile(B_st + (s * 2 + 0) * TILE_BYTES, &tm_hi, kb * KB, w.b_row + j * BN, &b_full[s]);
+                        tma_tile(B_st + (s * 2 + 1) * TILE_BYTES, &tm_lo, kb * KB, w.b_row + j * BN, &b_full[s]);
+                        if (++s == STAGES) { s = 0; ph ^= 1u; }
+                    }
+            }
         }
         return;
     }
-    // ===== consumers: warpgroup c owns left rows 64c .. 64c+63 of the CTA's 128 =====
+    // ===== consumers: warpgroup c owns rows 64c .. 64c+63 of each item's 128 =====
     const int c = (warp >> 2) - 1;
     const int q = lane & 3;
-    const int row0 = m0 + 64 * c + 16 * (warp & 3) + (lane >> 2);      // fragment rows: row0 (h = 0) and row0 + 8 (h = 1)
+    const int r0 = 64 * c + 16 * (warp & 3) + (lane >> 2);             // fragment rows: r0 (h = 0) and r0 + 8 (h = 1)
     const unsigned a_off = (unsigned)(64 * c * 128);                   // 64 rows x 128 bytes into every A tile
-    Top4 T0, T1;
     float d[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) d[i] = 0.0f;
-    mb_wait(&a_full, 0);
     int s = 0; unsigned ph = 0;
-    for (int j = 0; j < n_tiles; ++j) {
-        const int nb0 = j * BN;
-        // |b|^2 of the thread's 32 columns is on its way while the MMAs run
-        float2 rn[16];
+    int a_cur = -1; unsigned a_ph = 0;
+    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+        const MatchItem w = items[it];
+        if (w.a_row != a_cur) { mb_wait(&a_full, a_ph); a_ph ^= 1u; a_cur = w.a_row; }
+        const float* __restrict__ rnorm = norm + w.b_row;
+        Top4 T0, T1;
+        for (int j = 0; j < w.b_tiles; ++j) {
+            const int nb0 = j * BN;
+            // |b|^2 of the thread's 32 columns is on its way while the MMAs run
+            float2 rn[16];
 #pragma unroll
-        for (int b = 0; b < 16; ++b) rn[b] = __ldg(reinterpret_cast<const float2*>(rnorm + nb0 + 8 * b + 2 * q));
-        int prev = -1;
-        for (int kb = 0; kb < NKB; ++kb) {
-            mb_wait(&b_full[s], ph);
-            wg_fence();
-            const uint64_t a_hi = gmma_desc(A_hi + kb * TILE_BYTES + a_off), a_lo = gmma_desc(A_lo + kb * TILE_BYTES + a_off);
-            const uint64_t b_hi = gmma_desc(B_st + (s * 2 + 0) * TILE_BYTES), b_lo = gmma_desc(B_st + (s * 2 + 1) * TILE_BYTES);
+            for (int b = 0; b < 16; ++b) rn[b] = __ldg(reinterpret_cast<const float2*>(rnorm + nb0 + 8 * b + 2 * q));
+            int prev = -1;
+            for (int kb = 0; kb < NKB; ++kb) {
+                mb_wait(&b_full[s], ph);
+                wg_fence();
+                const uint64_t a_hi = gmma_desc(A_hi + kb * TILE_BYTES + a_off), a_lo = gmma_desc(A_lo + kb * TILE_BYTES + a_off);
+                const uint64_t b_hi = gmma_desc(B_st + (s * 2 + 0) * TILE_BYTES), b_lo = gmma_desc(B_st + (s * 2 + 1) * TILE_BYTES);
 #pragma unroll
-            for (int k8 = 0; k8 < KB / MMA_K; ++k8) {
-                const uint64_t adv = (uint64_t)(k8 * MMA_K * 4 / 16);          // +32 bytes inside the swizzle span
-                wgmma_tf32(d, a_hi + adv, b_hi + adv, (kb | k8) != 0);
-                wgmma_tf32(d, a_hi + adv, b_lo + adv, 1);
-                wgmma_tf32(d, a_lo + adv, b_hi + adv, 1);
-            }
-            wg_commit();
-            if (prev >= 0) {                                   // the previous K-block's MMAs have read their slot
-                wg_wait<1>();
-                __syncwarp();
-                if (lane == 0) mb_arrive(&b_empty[prev]);
-            }
-            prev = s;
-            if (++s == STAGES) { s = 0; ph ^= 1u; }
-        }
-        wg_wait<0>();
-        __syncwarp();
-        if (lane == 0) mb_arrive(&b_empty[prev]);
-        // keys |b|^2 - 2 a.b (+inf for padding columns, whose |b|^2 is +inf) with the column position in the low bits
-#pragma unroll
-        for (int b = 0; b < 16; ++b)
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int u = 0; u < 2; ++u) {
-                    const int i = 4 * b + 2 * h + u;
-                    const float val = fmaf(-2.0f, d[i], u ? rn[b].y : rn[b].x);
-                    d[i] = __uint_as_float((__float_as_uint(val) & 0xffffffe0u) | (unsigned)(2 * b + u));   // padding: inf or NaN
+                for (int k8 = 0; k8 < KB / MMA_K; ++k8) {
+                    const uint64_t adv = (uint64_t)(k8 * MMA_K * 4 / 16);          // +32 bytes inside the swizzle span
+                    wgmma_tf32(d, a_hi + adv, b_hi + adv, (kb | k8) != 0);
+                    wgmma_tf32(d, a_hi + adv, b_lo + adv, 1);
+                    wgmma_tf32(d, a_lo + adv, b_hi + adv, 1);
                 }
-        top4_row<0>(T0, d, nb0, q);
-        top4_row<1>(T1, d, nb0, q);
-    }
-    // the four lanes of a quad hold disjoint columns of the same two rows
-    T0.merge_xor(1); T1.merge_xor(1);
-    T0.merge_xor(2); T1.merge_xor(2);
-    if (q == 0) {
-        if (row0 < nl) *reinterpret_cast<int4*>(cand + (size_t)row0 * kCand) = make_int4(T0.i0, T0.i1, T0.i2, T0.i3);
-        if (row0 + 8 < nl) *reinterpret_cast<int4*>(cand + (size_t)(row0 + 8) * kCand) = make_int4(T1.i0, T1.i1, T1.i2, T1.i3);
+                wg_commit();
+                if (prev >= 0) {                                   // the previous K-block's MMAs have read their slot
+                    wg_wait<1>();
+                    __syncwarp();
+                    if (lane == 0) mb_arrive(&b_empty[prev]);
+                }
+                prev = s;
+                if (++s == STAGES) { s = 0; ph ^= 1u; }
+            }
+            wg_wait<0>();
+            __syncwarp();
+            if (lane == 0) mb_arrive(&b_empty[prev]);
+            // keys |b|^2 - 2 a.b (+inf for padding columns, whose |b|^2 is +inf) with the column position in the low bits
+#pragma unroll
+            for (int b = 0; b < 16; ++b)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int u = 0; u < 2; ++u) {
+                        const int i = 4 * b + 2 * h + u;
+                        const float val = fmaf(-2.0f, d[i], u ? rn[b].y : rn[b].x);
+                        d[i] = __uint_as_float((__float_as_uint(val) & 0xffffffe0u) | (unsigned)(2 * b + u));   // padding: inf or NaN
+                    }
+            // candidate indices relative to the right set
+            top4_row<0>(T0, d, w.b_col0 + nb0, q);
+            top4_row<1>(T1, d, w.b_col0 + nb0, q);
+        }
+        // the four lanes of a quad hold disjoint columns of the same two rows
+        T0.merge_xor(1); T1.merge_xor(1);
+        T0.merge_xor(2); T1.merge_xor(2);
+        if (q == 0) {
+            int32_t* cw = cand + (size_t)(w.cand + (int64_t)r0 * w.stride) * kCand;
+            if (w.l_row0 + r0 < w.nl) *reinterpret_cast<int4*>(cw) = make_int4(T0.i0, T0.i1, T0.i2, T0.i3);
+            if (w.l_row0 + r0 + 8 < w.nl) *reinterpret_cast<int4*>(cw + (size_t)8 * w.stride * kCand) = make_int4(T1.i0, T1.i1, T1.i2, T1.i3);
+        }
+        // every MMA of this warp on the current A has completed (wg_wait<0> of the last tile): release it if the next item
+        // needs another left tile
+        const int nx = it + gridDim.x;
+        if (nx < n_items && items[nx].a_row != a_cur) {
+            __syncwarp();
+            if (lane == 0) mb_arrive(&a_empty);
+        }
     }
 }
 
-// exact distances of the candidates, in increasing index order, through the reference's scan
+// the re-rank's view of one pair of a group
+struct RerankPair {
+    const ps_descriptor* l;
+    const ps_descriptor* r;
+    int64_t out_row;      // first output row of the pair
+    int64_t row;          // first row of the pair among the group's rows (ascending over the group's pairs)
+    int64_t cand;         // first candidate slot; row i, chunk c: cand + i * chunks + c
+    int32_t nr, chunks;
+};
+
+// One warp per (pair, left row): the 4 x chunks candidates (one lane each), sorted ascending by a warp bitonic sort,
+// duplicates and empty slots dropped, then their exact distances in increasing index order through the reference's scan.
+// With one chunk this is the four-candidate re-rank of the single-pair matcher, step for step.
 __global__ void __launch_bounds__(128)
-match_rerank_kernel(const ps_descriptor* __restrict__ l, int nl, const ps_descriptor* __restrict__ r, int nr,
-                    const int32_t* __restrict__ cand, int32_t* __restrict__ out)
+match_rerank_kernel(const RerankPair* __restrict__ pairs, int n_pairs, int64_t rows, const int32_t* __restrict__ cand,
+                    int32_t* __restrict__ out)
 {
     const int lane = threadIdx.x & 31;
-    const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
-    if (row >= nl) return;
-    const float4 l4 = __ldg(reinterpret_cast<const float4*>(l + row) + lane);
-    int c[kCand];
-#pragma unroll
-    for (int k = 0; k < kCand; ++k) { c[k] = cand[(size_t)row * kCand + k]; if (c[k] < 0 || c[k] >= nr) c[k] = 0x7fffffff; }
-    // sort the four indices ascending (the scan rule depends on arrival order)
-#pragma unroll
-    for (int a = 0; a < kCand; ++a)
-#pragma unroll
-        for (int b = a + 1; b < kCand; ++b)
-            if (c[b] < c[a]) { const int t = c[a]; c[a] = c[b]; c[b] = t; }
-    Best2 best; best.init();
-#pragma unroll
-    for (int k = 0; k < kCand; ++k) {
-        if (c[k] == 0x7fffffff) continue;                         // warp-uniform
-        if (k > 0 && c[k] == c[k - 1]) continue;
-        best.step(warp_sq_dist(l4, reinterpret_cast<const float4*>(r + c[k]), lane), c[k]);
+    const int64_t g = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (g >= rows) return;
+    int a = 0, b = n_pairs - 1;                                   // the last pair that starts at or before row g
+    while (a < b) { const int m = (a + b + 1) >> 1; if (pairs[m].row <= g) a = m; else b = m - 1; }
+    const RerankPair P = pairs[a];
+    const int64_t row = g - P.row;
+    int v = 0x7fffffff;
+    if (lane < kCand * P.chunks) {
+        v = cand[(size_t)(P.cand + row * P.chunks) * kCand + lane];
+        if (v < 0 || v >= P.nr) v = 0x7fffffff;
     }
-    if (lane == 0) best.store(out + 3 * (size_t)row);
+    // ascending across the first K lanes, K = 4 x chunks rounded up to a power of two (the scan rule depends on arrival
+    // order; the lanes beyond 4 x chunks hold 0x7fffffff)
+    const int K = P.chunks <= 1 ? 4 : P.chunks <= 2 ? 8 : P.chunks <= 4 ? 16 : 32;
+    for (int k = 2; k <= K; k <<= 1)
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            const int o = __shfl_xor_sync(0xffffffffu, v, j);
+            v = (((lane & j) == 0) == ((lane & k) == 0)) ? min(v, o) : max(v, o);
+        }
+    Best2 best; best.init();
+    if (P.chunks > 0) {
+        const float4 l4 = __ldg(reinterpret_cast<const float4*>(P.l + row) + lane);
+        int prev = -1;
+        for (int k = 0; k < K; ++k) {
+            const int ck = __shfl_sync(0xffffffffu, v, k);        // warp-uniform
+            if (ck == 0x7fffffff) break;
+            if (ck == prev) continue;
+            prev = ck;
+            best.step(warp_sq_dist(l4, reinterpret_cast<const float4*>(P.r + ck), lane), ck);
+        }
+    }
+    if (lane == 0) best.store(out + 3 * (size_t)(P.out_row + row));
 }
 
 } // namespace
@@ -376,6 +440,157 @@ int match_choice(int flags)
     return flags ? flags : env;
 }
 
+namespace {
+
+// the library's own memory pool of the current device: a pool gives freed memory back to the OS at the next
+// synchronisation unless told to keep it, and mapping the workspace again on every call costs more than the matching
+// itself (the application's default pool is left alone)
+cudaMemPool_t match_pool(const char** err)
+{
+    static std::mutex mu;
+    static cudaMemPool_t pools[64] = {};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); *err = "cudaGetDevice failed (matcher)"; return nullptr; }
+    std::lock_guard<std::mutex> g(mu);
+    if (!pools[dev]) {
+        cudaMemPoolProps props = {};
+        props.allocType = cudaMemAllocationTypePinned;
+        props.handleTypes = cudaMemHandleTypeNone;
+        props.location.type = cudaMemLocationTypeDevice;
+        props.location.id = dev;
+        if (cudaMemPoolCreate(&pools[dev], &props) != cudaSuccess) { cudaGetLastError(); pools[dev] = nullptr; *err = "cudaMemPoolCreate failed (matcher)"; return nullptr; }
+        unsigned long long keep = kMatchPoolKeep;                              // freed workspace that stays mapped
+        cudaMemPoolSetAttribute(pools[dev], cudaMemPoolAttrReleaseThreshold, &keep);
+    }
+    return pools[dev];
+}
+
+size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Copies the plan's metadata to `dst` on `st` from a page-locked staging buffer of the current device, so that the copy
+// is queued without waiting (a pageable source would hold the host until the transfer is done).  The buffer is reused
+// by the next call once the event recorded after this copy has completed.
+bool upload_plan(void* dst, const std::vector<uint8_t>& host, cudaStream_t st)
+{
+    struct Stage { uint8_t* buf = nullptr; size_t cap = 0; cudaEvent_t done = nullptr; };
+    static std::mutex mu;
+    static Stage stages[64];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); return false; }
+    std::lock_guard<std::mutex> g(mu);
+    Stage& s = stages[dev];
+    if (!s.done && cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); s.done = nullptr; return false; }
+    if (cudaEventSynchronize(s.done) != cudaSuccess) { cudaGetLastError(); return false; }     // the previous copy has left the buffer
+    if (s.cap < host.size()) {
+        if (s.buf) cudaFreeHost(s.buf);
+        s.buf = nullptr; s.cap = 0;
+        const size_t cap = std::max<size_t>(align_up(host.size(), 1 << 16), 1 << 16);
+        if (cudaHostAlloc(reinterpret_cast<void**>(&s.buf), cap, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); s.buf = nullptr; return false; }
+        s.cap = cap;
+    }
+    std::memcpy(s.buf, host.data(), host.size());
+    if (cudaMemcpyAsync(dst, s.buf, host.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) { cudaGetLastError(); return false; }
+    if (cudaEventRecord(s.done, st) != cudaSuccess) { cudaGetLastError(); return false; }
+    return true;
+}
+
+} // namespace
+
+size_t match_workspace_cap()
+{
+    static const size_t cap = [] {
+        const char* e = getenv("POPSIFT_B200_MATCH_WS");
+        const unsigned long long v = e ? strtoull(e, nullptr, 10) : 0ull;
+        return v > 0 ? (size_t)v : kMatchPoolKeep;
+    }();
+    return cap;
+}
+
+int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs,
+                    int32_t* out, int flags, cudaStream_t st, const char** err)
+{
+    *err = nullptr;
+    if (n_pairs <= 0) return 0;
+    flags = match_choice(flags);
+    const MatchPlan plan = plan_match(n_sets, n_desc, n_pairs, pairs, sm_count(), match_workspace_cap());
+    int launches = 0;
+    if (flags == PS_MATCH_EXACT) {
+        // the CUDA-core kernel, pair by pair: the in-library reference
+        for (int p = 0; p < n_pairs; ++p) {
+            const int l = pairs[2 * p], r = pairs[2 * p + 1];
+            if (n_desc[l] <= 0) continue;
+            match_exact_kernel<<<(n_desc[l] + 3) / 4, 128, 0, st>>>(sets[l], n_desc[l], sets[r], n_desc[r], out + 3 * (size_t)plan.out_row[p]);
+            ++launches;
+        }
+        return launches;
+    }
+    if (plan.groups.empty()) return 0;
+    // every group's sets, pairs and items, uploaded once; one workspace for the largest group's planes, reused in turn
+    struct Meta { size_t sets, pairs, items; };
+    std::vector<Meta> meta;
+    size_t meta_bytes = 0, planes = 0;
+    for (const MatchGroup& g : plan.groups) {
+        if (g.rows > 0x7fffff80) { *err = "matcher: a group of pairs has more than 2^31 rows"; return -1; }
+        Meta m;
+        m.sets = meta_bytes;  meta_bytes = align_up(meta_bytes + g.sets.size() * sizeof(SplitSet), 16);
+        m.pairs = meta_bytes; meta_bytes = align_up(meta_bytes + g.pairs.size() * sizeof(RerankPair), 16);
+        m.items = meta_bytes; meta_bytes = align_up(meta_bytes + g.items.size() * sizeof(MatchItem), 16);
+        meta.push_back(m);
+        planes = std::max(planes, g.bytes());
+    }
+    meta_bytes = align_up(meta_bytes, 1024);
+    std::vector<uint8_t> host(meta_bytes);
+    for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
+        const MatchGroup& g = plan.groups[gi];
+        SplitSet* hs = reinterpret_cast<SplitSet*>(host.data() + meta[gi].sets);
+        for (size_t k = 0; k < g.sets.size(); ++k) hs[k] = {sets[g.sets[k].set], n_desc[g.sets[k].set], (int32_t)g.sets[k].row};
+        RerankPair* hp = reinterpret_cast<RerankPair*>(host.data() + meta[gi].pairs);
+        for (size_t k = 0; k < g.pairs.size(); ++k) {
+            const MatchGroupPair& gp = g.pairs[k];
+            const int l = pairs[2 * gp.pair], r = pairs[2 * gp.pair + 1];
+            hp[k] = {sets[l], sets[r], plan.out_row[gp.pair], gp.row, gp.cand, n_desc[r], gp.chunks};
+        }
+        if (!g.items.empty()) std::memcpy(host.data() + meta[gi].items, g.items.data(), g.items.size() * sizeof(MatchItem));
+    }
+    cudaMemPool_t pool = match_pool(err);
+    if (!pool) return -1;
+    uint8_t* ws = nullptr;
+    // stream-ordered, so nothing blocks
+    if (cudaMallocFromPoolAsync(&ws, meta_bytes + planes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (matcher workspace)"; cudaGetLastError(); return -1; }
+    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "matcher: plan upload failed"; return -1; }
+    static_assert(TC_SMEM + 1024 <= 227 * 1024, "matcher shared memory");
+    static_assert(BM == kMatchTile && BN == kMatchTile && kCand == kMatchCand, "planner and kernel tile sizes");
+    cudaFuncSetAttribute(match_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
+    const int sms = sm_count();
+    for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
+        const MatchGroup& g = plan.groups[gi];
+        const RerankPair* d_pairs = reinterpret_cast<const RerankPair*>(ws + meta[gi].pairs);
+        int32_t* cand = nullptr;
+        if (!g.items.empty()) {
+            const int rows = (int)g.rows;
+            float* hi = reinterpret_cast<float*>(ws + meta_bytes);
+            float* lo = reinterpret_cast<float*>(ws + meta_bytes + (size_t)rows * 512);
+            float* norm = reinterpret_cast<float*>(ws + meta_bytes + (size_t)rows * 1024);
+            cand = reinterpret_cast<int32_t*>(ws + meta_bytes + (size_t)rows * 1028);
+            // one tensor map per plane: a left tile and a right tile are both row offsets into it
+            CUtensorMap m_hi, m_lo;
+            if (!make_tmap_2d(&m_hi, hi, 128, rows, 512, KB, BM, true) || !make_tmap_2d(&m_lo, lo, 128, rows, 512, KB, BM, true)) {
+                cudaFreeAsync(ws, st); *err = "cuTensorMapEncodeTiled failed (matcher)"; return -1;
+            }
+            match_split_kernel<<<(rows + 3) / 4, 128, 0, st>>>(reinterpret_cast<const SplitSet*>(ws + meta[gi].sets), (int)g.sets.size(),
+                                                               rows, hi, lo, norm);
+            const int n_items = (int)g.items.size();
+            match_tc_kernel<<<std::min(sms, n_items), TC_THREADS, TC_SMEM, st>>>(m_hi, m_lo, norm,
+                                                                                reinterpret_cast<const MatchItem*>(ws + meta[gi].items), n_items, cand);
+            launches += 2;
+        }
+        match_rerank_kernel<<<(unsigned)((g.left_rows + 3) / 4), 128, 0, st>>>(d_pairs, (int)g.pairs.size(), g.left_rows, cand, out);
+        ++launches;
+    }
+    cudaFreeAsync(ws, st);
+    return launches;
+}
+
 int run_match(const ps_descriptor* l, int nl, const ps_descriptor* r, int nr, int32_t* out, int flags, cudaStream_t st,
               const char** err)
 {
@@ -389,51 +604,12 @@ int run_match(const ps_descriptor* l, int nl, const ps_descriptor* r, int nr, in
         match_exact_kernel<<<(nl + 3) / 4, 128, 0, st>>>(l, nl, r, nr, out);
         return 1;
     }
-    const int nl_pad = (nl + BM - 1) / BM * BM, n_tiles = (nr + BN - 1) / BN, nr_pad = n_tiles * BN;
-    float *lhi = nullptr, *llo = nullptr, *rhi = nullptr, *rlo = nullptr, *rnorm = nullptr;
-    int32_t* cand = nullptr;
-    const size_t lb = (size_t)nl_pad * 512, rb = (size_t)nr_pad * 512;
-    // one workspace allocation per call, stream-ordered so nothing blocks, from the library's own pool per device: a pool
-    // gives freed memory back to the OS at the next synchronisation unless told to keep it, and mapping 50 MB again on
-    // every call costs more than the matching itself (the application's default pool is left alone)
-    cudaMemPool_t pool = nullptr;
-    {
-        static std::mutex mu;
-        static cudaMemPool_t pools[64] = {};
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); *err = "cudaGetDevice failed (matcher)"; return -1; }
-        std::lock_guard<std::mutex> g(mu);
-        if (!pools[dev]) {
-            cudaMemPoolProps props = {};
-            props.allocType = cudaMemAllocationTypePinned;
-            props.handleTypes = cudaMemHandleTypeNone;
-            props.location.type = cudaMemLocationTypeDevice;
-            props.location.id = dev;
-            if (cudaMemPoolCreate(&pools[dev], &props) != cudaSuccess) { cudaGetLastError(); pools[dev] = nullptr; *err = "cudaMemPoolCreate failed (matcher)"; return -1; }
-            unsigned long long keep = 1ull << 30;                          // up to 1 GB of freed workspace stays mapped
-            cudaMemPoolSetAttribute(pools[dev], cudaMemPoolAttrReleaseThreshold, &keep);
-        }
-        pool = pools[dev];
-    }
-    uint8_t* ws = nullptr;
-    const size_t total = 2 * lb + 2 * rb + (size_t)nr_pad * 4 + (size_t)nl_pad * kCand * 4;
-    if (cudaMallocFromPoolAsync(&ws, total, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (matcher workspace)"; cudaGetLastError(); return -1; }
-    lhi = reinterpret_cast<float*>(ws); llo = reinterpret_cast<float*>(ws + lb);
-    rhi = reinterpret_cast<float*>(ws + 2 * lb); rlo = reinterpret_cast<float*>(ws + 2 * lb + rb);
-    rnorm = reinterpret_cast<float*>(ws + 2 * lb + 2 * rb);
-    cand = reinterpret_cast<int32_t*>(ws + 2 * lb + 2 * rb + (size_t)nr_pad * 4);
-    CUtensorMap m_lhi, m_llo, m_rhi, m_rlo;
-    const bool ok = make_tmap_2d(&m_lhi, lhi, 128, nl_pad, 512, KB, BM, true) && make_tmap_2d(&m_llo, llo, 128, nl_pad, 512, KB, BM, true) &&
-                    make_tmap_2d(&m_rhi, rhi, 128, nr_pad, 512, KB, BN, true) && make_tmap_2d(&m_rlo, rlo, 128, nr_pad, 512, KB, BN, true);
-    if (!ok) { cudaFreeAsync(ws, st); *err = "cuTensorMapEncodeTiled failed (matcher)"; return -1; }
-    static_assert(TC_SMEM + 1024 <= 227 * 1024, "matcher shared memory");
-    match_split_kernel<<<(nl_pad + 3) / 4, 128, 0, st>>>(l, nl, nl_pad, lhi, llo, nullptr);
-    match_split_kernel<<<(nr_pad + 3) / 4, 128, 0, st>>>(r, nr, nr_pad, rhi, rlo, rnorm);
-    cudaFuncSetAttribute(match_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
-    match_tc_kernel<<<nl_pad / BM, TC_THREADS, TC_SMEM, st>>>(m_lhi, m_llo, m_rhi, m_rlo, rnorm, nl, n_tiles, cand);
-    match_rerank_kernel<<<(nl + 3) / 4, 128, 0, st>>>(l, nl, r, nr, cand, out);
-    cudaFreeAsync(ws, st);
-    return 4;
+    // a batch of one pair (one set when both sides are the same array)
+    const ps_descriptor* sets[2] = {l, r};
+    const int32_t n_desc[2] = {nl, nr};
+    const bool same = l == r && nl == nr;
+    const int32_t pair[2] = {0, same ? 0 : 1};
+    return run_match_batch(sets, n_desc, same ? 1 : 2, pair, 1, out, PS_MATCH_TENSOR, st, err);
 }
 
 } // namespace psb

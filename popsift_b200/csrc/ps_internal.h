@@ -178,5 +178,12 @@ int launch_fix_feature_pointers(ps_feature* feat, ps_descriptor* desc, int n, cu
 // brute-force 2-NN matcher (k_match.cu; reference features.cu:165-304): out = n_left x (best, second, accept), device
 // memory; asynchronous on `st`; returns the number of kernels launched or -1 (*err set)
 int run_match(const ps_descriptor* l, int nl, const ps_descriptor* r, int nr, int32_t* out, int flags, cudaStream_t st, const char** err);
+// many pairs (indices into sets / n_desc, already validated): pair p's rows start at row sum_{q<p} n_desc[pairs[2q]] of out.
+// EXACT runs match_exact_kernel pair by pair; AUTO / TENSOR plan groups of pairs (k_match_plan.h) and run one split, one
+// tensor-core and one re-rank launch per group
+int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs,
+                    int32_t* out, int flags, cudaStream_t st, const char** err);
+// bytes one group of the batched matcher may use (POPSIFT_B200_MATCH_WS, default 1 GB)
+size_t match_workspace_cap();
 
 } // namespace psb

@@ -53,3 +53,15 @@ if only in ("all", "match"):
     a = api.match_descriptors(l, r, api.FeaturesDev.MATCH_TENSOR)
     b = api.match_descriptors(l, r, api.FeaturesDev.MATCH_EXACT)
     print("match rows differing", int((a != b).any(1).sum()), flush=True)
+if only in ("all", "match-batch"):
+    # ragged sets, self pairs, an empty left and an empty right set; 1 x 20 left tiles take S > 1, and a 3 MB group cap
+    # (set in the environment by the caller: POPSIFT_B200_MATCH_WS=3000000) makes several groups
+    rng = np.random.default_rng(1)
+    def unit(n):
+        d = rng.random((n, 128), dtype=np.float32)
+        return d / np.maximum(np.linalg.norm(d, axis=1, keepdims=True), 1e-12)
+    sets = [unit(n) for n in (100, 2500, 129, 0, 1800, 700)]
+    pairs = [(0, 1), (1, 0), (2, 2), (3, 1), (1, 3), (4, 5), (5, 4), (0, 4), (2, 1), (1, 1)]
+    got = api.match_pairs(sets, pairs, api.FeaturesDev.MATCH_TENSOR)
+    bad = sum(int((g != api.match_descriptors(sets[i], sets[j], api.FeaturesDev.MATCH_EXACT)).any(1).sum()) for g, (i, j) in zip(got, pairs))
+    print("match-batch rows differing", bad, flush=True)
