@@ -113,4 +113,11 @@ public:
 std::vector<std::vector<int>> matchPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
                                          int flags = 0);
 
+/// matchPairs on 8-bit descriptors (an addition to the reference's interface; C ABI ps_descriptors_to_u8 +
+/// ps_match_u8_batch): entry p equals matchPairs(...) on the descriptors rounded as --write-as-uchar prints them
+/// (saturated to [0, 255]; scale them with Config::setNormalizationMultiplier, e.g. 9).  Each set is quantised on the
+/// device and matched with exact integer distances; flags as for ps_match.
+std::vector<std::vector<int>> matchPairsU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                           int flags = 0);
+
 } // namespace popsift

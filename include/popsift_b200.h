@@ -209,6 +209,22 @@ int ps_match(int device, const ps_descriptor* d_left, int n_left, const ps_descr
  * set that is not device memory on `device`. */
 int ps_match_batch(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc,
                    int n_pairs, const int32_t* pairs, int32_t* d_out, int flags);
+/* Device-side quantisation of float descriptors to 8 bits (an addition to the reference's interface):
+ * d_out[128 i + k] = roundf(min(max(d_in[i].features[k], 0), 255)), NaN -> 0.  For components in [0, 255] this is the
+ * value the reference prints under --write-as-uchar (features.cu:317-320); larger values saturate.  Scaling is the
+ * caller's, e.g. ps_config::norm_multi = 9 as the reference's help text suggests.  d_in (n descriptors) and d_out
+ * (n x 128 bytes) are DEVICE memory on `device`.  Returns when the result is complete; PS_ERR_ARG for n < 0, a null
+ * pointer with n > 0, or a pointer that is not device memory on `device`. */
+int ps_descriptors_to_u8(int device, const ps_descriptor* d_in, int n, uint8_t* d_out);
+/* ps_match_batch for 8-bit descriptors: d_sets[i] = n_desc[i] rows of 128 uint8_t (DEVICE, on `device`, 16-byte
+ * aligned).  Same pair list, output layout and argument checks as ps_match_batch, and a set pointer that is not 16-byte
+ * aligned is refused with PS_ERR_ARG.  Distances are exact integers: pair p's rows are bit for bit what
+ * ps_match_batch(..., PS_MATCH_EXACT) gives on float32 copies of the same sets -- best = the smallest (distance, index),
+ * second = the next, accept = float(d1) / float(d2) < 0.8f (equal distances give 0); an empty right set gives (0, 0, 0),
+ * a single right descriptor (0, 0, 1).  PS_MATCH_AUTO / PS_MATCH_TENSOR run the integer tensor-core path (wgmma u8 x u8
+ * -> s32), PS_MATCH_EXACT a CUDA-core kernel pair by pair. */
+int ps_match_u8_batch(int device, int n_sets, const uint8_t* const* d_sets, const int32_t* n_desc,
+                      int n_pairs, const int32_t* pairs, int32_t* d_out, int flags);
 /* page-locked host memory for images and results (thin wrappers of cudaHostAlloc / cudaFreeHost).
  * ps_submit_* and ps_download detect page-locked buffers and copy straight from / into them; pageable
  * buffers are staged through the slot's own pinned buffers (one extra host memcpy). */

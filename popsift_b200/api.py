@@ -58,6 +58,7 @@ EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps
            "ps_sync", "ps_debug_plane", "ps_debug_extrema", "ps_slot_geometry", "ps_set_timing", "ps_stage_ms",
            "ps_launch_count", "ps_slot_stream", "ps_run_pyramid_only", "ps_run_level_only", "ps_host_alloc", "ps_host_free",
            "ps_download_dev", "ps_dev_alloc", "ps_dev_free", "ps_dev_to_host", "ps_wait_input", "ps_match", "ps_match_batch", "ps_pointer_device", "ps_host_to_dev",
+           "ps_descriptors_to_u8", "ps_match_u8_batch",
            "ps_debug_level0_plan", "ps_format_gauss_tables"]
 
 _lib = None
@@ -91,6 +92,9 @@ def load_library():
     L.ps_match.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
     if hasattr(L, "ps_match_batch"):    # absent from builds that predate it (POPSIFT_B200_LIB A/B runs)
         L.ps_match_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+    if hasattr(L, "ps_match_u8_batch"):
+        L.ps_descriptors_to_u8.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p]
+        L.ps_match_u8_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -477,6 +481,97 @@ def match_pairs(sets, pairs, flags=0, device=None) -> list:
         rc = lib.ps_match_batch(device, len(ptrs), c_sets, c_n, len(pairs), c_pairs, d_out, flags)
         if rc != 0:
             raise PopSiftError("ps_match_batch error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        if out.nbytes and lib.ps_dev_to_host(out.ctypes.data, d_out, out.nbytes) != 0:
+            raise PopSiftError("device -> host copy failed")
+    finally:
+        for p in owned:
+            lib.ps_dev_free(p)
+    starts = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
+    return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
+
+
+def _to_u8_dev(lib, d_in, n, device) -> int:
+    """device copy of n float descriptors at d_in quantised to 8 bits (ps_descriptors_to_u8); the caller frees it"""
+    q = lib.ps_dev_alloc(max(n * 128, 16))
+    if not q:
+        raise PopSiftError("ps_dev_alloc failed")
+    rc = lib.ps_descriptors_to_u8(device, d_in, n, q) if n else 0
+    if rc != 0:
+        lib.ps_dev_free(q)
+        raise PopSiftError("ps_descriptors_to_u8 error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+    return q
+
+
+def descriptors_to_u8(x, device=None) -> np.ndarray:
+    """8-bit descriptors computed on the device (C ABI ps_descriptors_to_u8): roundf(min(max(v, 0), 255)) per component,
+    NaN -> 0 -- what the reference prints under --write-as-uchar, saturated.  `x` is a FeaturesDev or a host (n, 128)
+    float32 array; returns a host (n, 128) uint8 array."""
+    lib = load_library()
+    owned = []
+    try:
+        if isinstance(x, FeaturesDev):
+            d_in, n = x.getDescriptors(), x.getDescriptorCount()
+        else:
+            a = np.ascontiguousarray(x, np.float32).reshape(-1, 128)
+            n = len(a)
+            d_in = lib.ps_dev_alloc(max(a.nbytes, 4))
+            if not d_in:
+                raise PopSiftError("ps_dev_alloc failed")
+            owned.append(d_in)
+            if a.nbytes and lib.ps_host_to_dev(d_in, a.ctypes.data, a.nbytes) != 0:
+                raise PopSiftError("host -> device copy failed")
+        if device is None:
+            device = max(0, lib.ps_pointer_device(d_in)) if n else 0
+        q = _to_u8_dev(lib, d_in, n, device)
+        owned.append(q)
+        out = np.zeros((n, 128), np.uint8)
+        if out.nbytes and lib.ps_dev_to_host(out.ctypes.data, q, out.nbytes) != 0:
+            raise PopSiftError("device -> host copy failed")
+        return out
+    finally:
+        for p in owned:
+            lib.ps_dev_free(p)
+
+
+def match_pairs_u8(sets, pairs, flags=0, device=None) -> list:
+    """match_pairs for 8-bit descriptors with exact integer distances (C ABI ps_match_u8_batch).  `sets` holds host (n, 128)
+    uint8 arrays (copied through device memory) or FeaturesDev objects (quantised on the device by ps_descriptors_to_u8;
+    the descriptors never leave it).  Entry p is the (n_left, 3) int32 array (best, second, accept), row for row what
+    match_pairs gives on float32 copies of the 8-bit sets under FeaturesDev.MATCH_EXACT."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    owned, ptrs, counts = [], [], []
+    try:
+        if device is None:
+            dev_sets = [s for s in sets if isinstance(s, FeaturesDev) and s.getDescriptorCount() > 0]
+            device = max(0, lib.ps_pointer_device(dev_sets[0].getDescriptors())) if dev_sets else 0
+        for s in sets:
+            if isinstance(s, FeaturesDev):
+                n = s.getDescriptorCount()
+                p = _to_u8_dev(lib, s.getDescriptors(), n, device)
+                owned.append(p)
+                ptrs.append(p); counts.append(n)
+                continue
+            a = np.ascontiguousarray(s, np.uint8).reshape(-1, 128)
+            p = lib.ps_dev_alloc(max(a.nbytes, 16))
+            if not p:
+                raise PopSiftError("ps_dev_alloc failed")
+            owned.append(p)
+            if a.nbytes and lib.ps_host_to_dev(p, a.ctypes.data, a.nbytes) != 0:
+                raise PopSiftError("host -> device copy failed")
+            ptrs.append(p); counts.append(len(a))
+        rows = [counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs]
+        out = np.zeros((sum(rows), 3), np.int32)
+        d_out = lib.ps_dev_alloc(max(out.nbytes, 4))
+        if not d_out:
+            raise PopSiftError("ps_dev_alloc failed")
+        owned.append(d_out)
+        c_sets = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
+        c_n = (C.c_int32 * max(len(counts), 1))(*counts)
+        c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
+        rc = lib.ps_match_u8_batch(device, len(ptrs), c_sets, c_n, len(pairs), c_pairs, d_out, flags)
+        if rc != 0:
+            raise PopSiftError("ps_match_u8_batch error %d: %s" % (rc, lib.ps_last_error(None).decode()))
         if out.nbytes and lib.ps_dev_to_host(out.ctypes.data, d_out, out.nbytes) != 0:
             raise PopSiftError("device -> host copy failed")
     finally:

@@ -26,7 +26,7 @@ NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "--fmad=false",   # no implicit contraction anywhere; every fma in the kernels is explicit
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu",
+LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu",
                "host/sift_conf.cpp", "host/features.cpp", "host/popsift.cpp", "host/device_prop.cpp", "host/log_dump.cpp"]
 DEMO_SOURCES = ["app/popsift_demo.cpp", "app/pgmread.cpp"]
 MATCH_SOURCES = ["app/popsift_match.cpp"]            # + app/pgmread.cpp
@@ -40,8 +40,12 @@ PART_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "partition_check.cpp")
 PGM_CHECK = os.path.join(BIN_DIR, "pgmread_check")
 MATCH_PLAN_CHECK = os.path.join(BIN_DIR, "match_plan_check")
 MATCH_PLAN_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_plan_check.cpp")
+MATCH_PLAN_U8_CHECK = os.path.join(BIN_DIR, "match_plan_u8_check")
+MATCH_PLAN_U8_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_plan_u8_check.cpp")
 MATCH_PAIRS_CHECK = os.path.join(BIN_DIR, "match_pairs_check")
 MATCH_PAIRS_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_pairs_check.cpp")
+MATCH_U8_CHECK = os.path.join(BIN_DIR, "match_u8_check")
+MATCH_U8_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_u8_check.cpp")
 PGM_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "pgmread_check.cpp")
 
 
@@ -116,9 +120,16 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if os.path.exists(MATCH_PLAN_CHECK_SRC) and (force or _newer(MATCH_PLAN_CHECK, [MATCH_PLAN_CHECK_SRC, plan_hdr])):
         # host-only sweep of the batched matcher's planner (no CUDA, no library)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + CSRC, MATCH_PLAN_CHECK_SRC, "-o", MATCH_PLAN_CHECK])
+    if os.path.exists(MATCH_PLAN_U8_CHECK_SRC) and (force or _newer(MATCH_PLAN_U8_CHECK, [MATCH_PLAN_U8_CHECK_SRC, plan_hdr])):
+        # the same planner at the 8-bit matcher's 132-byte rows (host only)
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + CSRC, MATCH_PLAN_U8_CHECK_SRC, "-o", MATCH_PLAN_U8_CHECK])
     if os.path.exists(MATCH_PAIRS_CHECK_SRC) and (force or _newer(MATCH_PAIRS_CHECK, [MATCH_PAIRS_CHECK_SRC, LIB] + hdrs)):
         # popsift::matchPairs against FeaturesDev::matchIndices through the C++ API
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), MATCH_PAIRS_CHECK_SRC, "-o", MATCH_PAIRS_CHECK,
+                               "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
+    if os.path.exists(MATCH_U8_CHECK_SRC) and (force or _newer(MATCH_U8_CHECK, [MATCH_U8_CHECK_SRC, LIB] + hdrs)):
+        # popsift::matchPairsU8 against the float matcher on the quantised descriptors, through the C++ and C APIs
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), MATCH_U8_CHECK_SRC, "-o", MATCH_U8_CHECK,
                                "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
     pgm_src = os.path.join(CSRC, "app", "pgmread.cpp")
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):

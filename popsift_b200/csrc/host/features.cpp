@@ -169,6 +169,54 @@ std::vector<std::vector<int>> matchPairs(const std::vector<FeaturesDev*>& sets, 
     return out;
 }
 
+std::vector<std::vector<int>> matchPairsU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs, int flags)
+{
+    std::vector<int32_t> n_desc(sets.size());
+    for (size_t i = 0; i < sets.size(); ++i) {
+        if (!sets[i]) throw std::runtime_error("popsift::matchPairsU8: null set");
+        n_desc[i] = std::max(sets[i]->getDescriptorCount(), 0);
+    }
+    std::vector<int32_t> flat(2 * pairs.size());
+    std::vector<std::vector<int>> out(pairs.size());
+    size_t rows = 0;
+    for (size_t p = 0; p < pairs.size(); ++p) {
+        const int l = pairs[p].first, r = pairs[p].second;
+        if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error("popsift::matchPairsU8: set index out of range");
+        flat[2 * p] = l; flat[2 * p + 1] = r;
+        out[p].assign((size_t)n_desc[l] * 3, 0);
+        rows += out[p].size() / 3;
+    }
+    if (rows == 0) return out;
+    int dev = 0;
+    for (size_t i = 0; i < sets.size(); ++i)
+        if (n_desc[i] > 0) { dev = std::max(0, ps_pointer_device(sets[i]->getDescriptors())); break; }
+    // the 8-bit copies of every set (cudaMalloc: 256-byte aligned) and the result rows
+    std::vector<void*> owned;
+    auto release = [&]() { for (void* p : owned) ps_dev_free(p); };
+    std::vector<const uint8_t*> d_sets(sets.size(), nullptr);
+    int rc = PS_OK;
+    for (size_t i = 0; i < sets.size() && rc == PS_OK; ++i) {
+        if (n_desc[i] == 0) continue;
+        uint8_t* q = static_cast<uint8_t*>(ps_dev_alloc((size_t)n_desc[i] * 128));
+        if (!q) { release(); throw std::runtime_error("popsift::matchPairsU8: failed to allocate device memory"); }
+        owned.push_back(q);
+        d_sets[i] = q;
+        rc = ps_descriptors_to_u8(dev, reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors()), n_desc[i], q);
+    }
+    int32_t* d_out = rc == PS_OK ? static_cast<int32_t*>(ps_dev_alloc(rows * 3 * sizeof(int32_t))) : nullptr;
+    if (rc == PS_OK && !d_out) { release(); throw std::runtime_error("popsift::matchPairsU8: failed to allocate device memory"); }
+    if (d_out) owned.push_back(d_out);
+    if (rc == PS_OK) rc = ps_match_u8_batch(dev, (int)sets.size(), d_sets.data(), n_desc.data(), (int)pairs.size(), flat.data(), d_out, flags);
+    size_t row = 0;
+    for (size_t p = 0; p < pairs.size() && rc == PS_OK; ++p) {
+        rc = ps_dev_to_host(out[p].data(), d_out + 3 * row, out[p].size() * sizeof(int32_t));
+        row += out[p].size() / 3;
+    }
+    release();
+    if (rc != PS_OK) throw std::runtime_error(std::string("popsift::matchPairsU8 failed: ") + ps_last_error(nullptr));
+    return out;
+}
+
 void FeaturesHost::pin() {}
 void FeaturesHost::unpin() {}
 

@@ -32,6 +32,7 @@
 // match_exact_kernel is the same computation on CUDA cores (one warp per left descriptor over all right ones): used
 // for small problems and as the in-library cross-check (PS_MATCH_EXACT).
 #include "ps_internal.h"
+#include "k_match_common.h"
 #include "k_match_plan.h"
 #include "tma_util.h"
 
@@ -143,37 +144,6 @@ constexpr int TC_THREADS = 384;              // warpgroup 0 = TMA producer, warp
 constexpr int kCand = 4;                     // candidates kept per left descriptor
 // A hi/lo resident (128 KB) + the ring (96 KB) + slack to align the dynamic buffer to 1024 bytes
 constexpr size_t TC_SMEM = (size_t)2 * NKB * TILE_BYTES + (size_t)STAGES * 2 * TILE_BYTES + 1024;
-
-__device__ __forceinline__ unsigned s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mb_init(uint64_t* b, unsigned n) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(s32(b)), "r"(n) : "memory"); }
-__device__ __forceinline__ void mb_expect(uint64_t* b, unsigned bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(s32(b)), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void mb_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(s32(b)) : "memory"); }
-__device__ __forceinline__ void mb_wait(uint64_t* b, unsigned parity)
-{
-    unsigned ok, spins = 0;
-    for (;;) {
-        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok) : "r"(s32(b)), "r"(parity) : "memory");
-        if (ok) break;
-        if (++spins > (1u << 24)) __trap();          // abort instead of hanging the device
-    }
-}
-__device__ __forceinline__ void tma_tile(void* dst, const CUtensorMap* map, int k0, int row0, uint64_t* bar)
-{
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 :: "r"(s32(dst)), "l"(reinterpret_cast<unsigned long long>(map)), "r"(k0), "r"(row0), "r"(s32(bar)) : "memory");
-}
-// wgmma shared-memory descriptor of a K-major operand tile, SWIZZLE_128B, rows 128 bytes wide, 8-row groups 1024 bytes
-// apart: start >> 4 in [0,14), LBO = 1 in [16,30) (unused by swizzled K-major layouts), SBO = 1024 >> 4 in [32,46),
-// layout SWIZZLE_128B = 1 in [62,64)
-__device__ __forceinline__ uint64_t gmma_desc(const void* tile)
-{
-    return (uint64_t)((s32(tile) >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
-}
-__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
 
 // D[64 x 128] (+)= A[64 x 8] . B[128 x 8]^T, tf32 in, fp32 accumulate, both operands K-major in shared memory
 __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc, int accumulate)
@@ -440,8 +410,6 @@ int match_choice(int flags)
     return flags ? flags : env;
 }
 
-namespace {
-
 // the library's own memory pool of the current device: a pool gives freed memory back to the OS at the next
 // synchronisation unless told to keep it, and mapping the workspace again on every call costs more than the matching
 // itself (the application's default pool is left alone)
@@ -464,8 +432,6 @@ cudaMemPool_t match_pool(const char** err)
     }
     return pools[dev];
 }
-
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // Copies the plan's metadata to `dst` on `st` from a page-locked staging buffer of the current device, so that the copy
 // is queued without waiting (a pageable source would hold the host until the transfer is done).  The buffer is reused
@@ -493,8 +459,6 @@ bool upload_plan(void* dst, const std::vector<uint8_t>& host, cudaStream_t st)
     if (cudaEventRecord(s.done, st) != cudaSuccess) { cudaGetLastError(); return false; }
     return true;
 }
-
-} // namespace
 
 size_t match_workspace_cap()
 {

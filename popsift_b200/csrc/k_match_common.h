@@ -1,0 +1,53 @@
+// What both brute-force matchers (k_match.cu: float32 descriptors, k_match_u8.cu: 8-bit descriptors) share: the
+// mbarrier / TMA / wgmma-descriptor helpers of their persistent tensor-core kernels, the matcher's memory pool and the
+// upload of a plan's metadata.
+#pragma once
+#include <cuda.h>
+#include <cuda_runtime.h>
+#include <cstddef>
+#include <cstdint>
+#include <vector>
+
+namespace psb {
+
+__device__ __forceinline__ unsigned s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mb_init(uint64_t* b, unsigned n) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(s32(b)), "r"(n) : "memory"); }
+__device__ __forceinline__ void mb_expect(uint64_t* b, unsigned bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(s32(b)), "r"(bytes) : "memory"); }
+__device__ __forceinline__ void mb_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(s32(b)) : "memory"); }
+__device__ __forceinline__ void mb_wait(uint64_t* b, unsigned parity)
+{
+    unsigned ok, spins = 0;
+    for (;;) {
+        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
+                     : "=r"(ok) : "r"(s32(b)), "r"(parity) : "memory");
+        if (ok) break;
+        if (++spins > (1u << 24)) __trap();          // abort instead of hanging the device
+    }
+}
+__device__ __forceinline__ void tma_tile(void* dst, const CUtensorMap* map, int k0, int row0, uint64_t* bar)
+{
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 :: "r"(s32(dst)), "l"(reinterpret_cast<unsigned long long>(map)), "r"(k0), "r"(row0), "r"(s32(bar)) : "memory");
+}
+// wgmma shared-memory descriptor of a K-major operand tile, SWIZZLE_128B, rows 128 bytes wide, 8-row groups 1024 bytes
+// apart: start >> 4 in [0,14), LBO = 1 in [16,30) (unused by swizzled K-major layouts), SBO = 1024 >> 4 in [32,46),
+// layout SWIZZLE_128B = 1 in [62,64)
+__device__ __forceinline__ uint64_t gmma_desc(const void* tile)
+{
+    return (uint64_t)((s32(tile) >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+
+inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// the library's own memory pool of the current device (k_match.cu): a pool gives freed memory back to the OS at the next
+// synchronisation unless told to keep it, and mapping the workspace again on every call costs more than the matching
+// itself (the application's default pool is left alone)
+cudaMemPool_t match_pool(const char** err);
+// Copies a plan's metadata to `dst` on `st` from a page-locked staging buffer of the current device (k_match.cu)
+bool upload_plan(void* dst, const std::vector<uint8_t>& host, cudaStream_t st);
+
+} // namespace psb

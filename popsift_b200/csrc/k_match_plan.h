@@ -22,7 +22,8 @@ namespace psb {
 constexpr int kMatchTile = 128;                 // rows of a left tile and of a right tile
 constexpr int kMatchMaxChunks = 8;              // bound of S
 constexpr int kMatchCand = 4;                   // candidates one item keeps per left row
-constexpr size_t kMatchRowBytes = 2 * 512 + 4;  // pooled hi + lo row and its norm
+constexpr size_t kMatchRowBytes = 2 * 512 + 4;  // pooled hi + lo row and its norm (float32 descriptors)
+constexpr size_t kMatchU8RowBytes = 128 + 4;    // pooled 8-bit row and its norm key (k_match_u8.cu)
 // freed workspace the matcher's memory pool keeps mapped, and the default cap of one group's workspace
 // (POPSIFT_B200_MATCH_WS=bytes overrides the cap)
 constexpr size_t kMatchPoolKeep = (size_t)1 << 30;
@@ -60,7 +61,8 @@ struct MatchGroup {
     int64_t cand_slots = 0;
     int64_t left_rows = 0;     // rows the re-rank writes
     int     chunks = 1;        // S of the group
-    size_t  bytes() const { return (size_t)rows * kMatchRowBytes + (size_t)cand_slots * kMatchCand * 4; }
+    size_t  row_bytes = kMatchRowBytes;   // workspace bytes of one pooled row
+    size_t  bytes() const { return (size_t)rows * row_bytes + (size_t)cand_slots * kMatchCand * 4; }
 };
 
 struct MatchPlan {
@@ -165,8 +167,10 @@ inline int64_t cand_slots(const MatchGroup& g, const int32_t* n_desc, const int3
 
 } // namespace plan_detail
 
-// n_desc: n_sets sizes; pairs: n_pairs x {left, right} (indices already validated); sms: persistent CTAs; cap: bytes
-inline MatchPlan plan_match(int n_sets, const int32_t* n_desc, int n_pairs, const int32_t* pairs, int sms, size_t cap)
+// n_desc: n_sets sizes; pairs: n_pairs x {left, right} (indices already validated); sms: persistent CTAs; cap: bytes;
+// row_bytes: workspace bytes of one pooled row (kMatchRowBytes for float32 descriptors, kMatchU8RowBytes for 8-bit ones)
+inline MatchPlan plan_match(int n_sets, const int32_t* n_desc, int n_pairs, const int32_t* pairs, int sms, size_t cap,
+                            size_t row_bytes = kMatchRowBytes)
 {
     MatchPlan plan;
     plan.out_row.resize((size_t)n_pairs);
@@ -177,9 +181,11 @@ inline MatchPlan plan_match(int n_sets, const int32_t* n_desc, int n_pairs, cons
     // groups, sized with one chunk per pair
     std::vector<int> member((size_t)std::max(n_sets, 0), -1);     // set -> group that holds it
     MatchGroup cur;
+    cur.row_bytes = row_bytes;
     auto close = [&]() {
         if (!cur.pairs.empty()) plan.groups.push_back(std::move(cur));
         cur = MatchGroup();
+        cur.row_bytes = row_bytes;
     };
     for (int p = 0; p < n_pairs; ++p) {
         const int l = pairs[2 * p], r = pairs[2 * p + 1];
@@ -192,7 +198,7 @@ inline MatchPlan plan_match(int n_sets, const int32_t* n_desc, int n_pairs, cons
             if (member[r] != gi && r != l) rows += match_tiles(nr) * kMatchTile;
             slots += nl;
         }
-        if (!cur.pairs.empty() && (size_t)rows * kMatchRowBytes + (size_t)slots * kMatchCand * 4 > cap) {
+        if (!cur.pairs.empty() && (size_t)rows * row_bytes + (size_t)slots * kMatchCand * 4 > cap) {
             close();
             p -= 1;                                     // the pair opens the next group
             continue;
@@ -220,7 +226,7 @@ inline MatchPlan plan_match(int n_sets, const int32_t* n_desc, int n_pairs, cons
             int64_t best_t = plan_detail::makespan(g, n_desc, pairs, 1, sms);
             for (int S = 2; S <= kMatchMaxChunks; ++S) {
                 // more chunks only cost more candidate slots
-                if (g.pairs.size() > 1 && (size_t)g.rows * kMatchRowBytes + (size_t)plan_detail::cand_slots(g, n_desc, pairs, S) * kMatchCand * 4 > cap) break;
+                if (g.pairs.size() > 1 && (size_t)g.rows * row_bytes + (size_t)plan_detail::cand_slots(g, n_desc, pairs, S) * kMatchCand * 4 > cap) break;
                 const int64_t t = plan_detail::makespan(g, n_desc, pairs, S, sms);
                 if (t < best_t) { best_t = t; best_s = S; }
             }

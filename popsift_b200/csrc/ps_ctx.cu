@@ -931,6 +931,43 @@ extern "C" int ps_match_batch(int device, int n_sets, const ps_descriptor* const
     return PS_OK;
 }
 
+extern "C" int ps_descriptors_to_u8(int device, const ps_descriptor* d_in, int n, uint8_t* d_out)
+{
+    if (n < 0 || (n > 0 && (!d_in || !d_out))) return PS_ERR_ARG;
+    if (n == 0) return PS_OK;
+    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (ps_pointer_device(d_in) != device || ps_pointer_device(d_out) != device) return PS_ERR_ARG;
+    run_descriptors_to_u8(d_in, n, d_out, nullptr);
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string("ps_descriptors_to_u8: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
+}
+
+extern "C" int ps_match_u8_batch(int device, int n_sets, const uint8_t* const* d_sets, const int32_t* n_desc,
+                                 int n_pairs, const int32_t* pairs, int32_t* d_out, int flags)
+{
+    if (n_sets < 0 || n_pairs < 0 || (n_sets > 0 && (!d_sets || !n_desc)) || (n_pairs > 0 && !pairs)) return PS_ERR_ARG;
+    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    for (int i = 0; i < n_sets; ++i) {
+        if (n_desc[i] < 0) return PS_ERR_ARG;
+        if (n_desc[i] > 0 && (!d_sets[i] || (reinterpret_cast<uintptr_t>(d_sets[i]) & 15u) || ps_pointer_device(d_sets[i]) != device)) return PS_ERR_ARG;
+    }
+    int64_t rows = 0;
+    for (int p = 0; p < n_pairs; ++p) {
+        const int l = pairs[2 * p], r = pairs[2 * p + 1];
+        if (l < 0 || l >= n_sets || r < 0 || r >= n_sets) return PS_ERR_ARG;
+        rows += n_desc[l];
+    }
+    if (rows == 0) return PS_OK;
+    if (!d_out) return PS_ERR_ARG;
+    const char* err = nullptr;
+    const int n = run_match_u8_batch(d_sets, n_desc, n_sets, pairs, n_pairs, d_out, flags, nullptr, &err);
+    if (n < 0) { g_create_error = err ? err : "ps_match_u8_batch failed"; return PS_ERR_CUDA; }
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string("ps_match_u8_batch: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
+}
+
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)
 {
     if (bytes == 0) return PS_OK;

@@ -185,5 +185,15 @@ int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int
                     int32_t* out, int flags, cudaStream_t st, const char** err);
 // bytes one group of the batched matcher may use (POPSIFT_B200_MATCH_WS, default 1 GB)
 size_t match_workspace_cap();
+// flags after the POPSIFT_B200_MATCH=exact|tc override (k_match.cu)
+int match_choice(int flags);
+
+// 8-bit descriptors (k_match_u8.cu): out[i] = roundf(min(max(in[i], 0), 255)) (NaN -> 0) for n x 128 components
+int run_descriptors_to_u8(const ps_descriptor* in, int n, uint8_t* out, cudaStream_t st);
+// run_match_batch for sets of n_desc[i] x 128 uint8_t (16-byte aligned): same pair list, same output rows, exact integer
+// distances.  EXACT runs match_u8_exact_kernel pair by pair; AUTO / TENSOR plan groups of pairs with 132-byte rows and run
+// one pack, one integer tensor-core and one finalize launch per group
+int run_match_u8_batch(const uint8_t* const* sets, const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs,
+                       int32_t* out, int flags, cudaStream_t st, const char** err);
 
 } // namespace psb

@@ -7,6 +7,14 @@ H100 SXM data sheet's 989 TFLOP/s dense BF16 / 2 = 495 TFLOP/s).
     python tools/match_bench.py --batch N [out.json]    N 1920x1080 frames, all N (N - 1) ordered pairs: a Python loop of
                                                         ps_match against one ps_match_batch call
 
+    python tools/match_bench.py --u8 [--batch N] [out.json]
+                                                        the same workloads extracted with norm_multi = 9 and quantised
+                                                        with ps_descriptors_to_u8: ps_match_u8_batch against the float
+                                                        ps_match_batch on the same frames, alternating.  Integer TOPS count
+                                                        2 x 128 x n_left x n_right per pair against dense INT8
+                                                        (MEASURED_PEAKS.json int8_tops when present, else the H100 SXM data
+                                                        sheet's 1979 TOPS)
+
 Every result records the card name, power limit and maximum SM clock (nvidia-smi).  Set POPSIFT_B200_LIB to time
 another build of the library (the 4K leg only needs ps_match).
 
@@ -30,6 +38,7 @@ from popsift_b200 import api  # noqa: E402
 from popsift_b200.synth import make_frame, write_pgm  # noqa: E402
 
 TF32_DENSE_SHEET = 989.0 / 2        # H100 SXM data sheet: 989 TFLOP/s dense BF16; tf32 issues at half that rate
+INT8_DENSE_SHEET = 1979.0           # H100 SXM data sheet: 1979 TOPS dense INT8
 
 
 def card():
@@ -47,6 +56,15 @@ def tf32_peak():
     if os.path.exists(peaks):
         return float(json.load(open(peaks))["bf16_tflops"]) / 2, "MEASURED_PEAKS.json bf16_tflops / 2 (tf32 issues at half the bf16 rate)"
     return TF32_DENSE_SHEET, "H100 SXM data sheet, 989 TFLOP/s dense BF16 / 2"
+
+
+def int8_peak():
+    peaks = os.path.join(ROOT, "MEASURED_PEAKS.json")
+    if os.path.exists(peaks):
+        v = json.load(open(peaks)).get("int8_tops")
+        if v:
+            return float(v), "MEASURED_PEAKS.json int8_tops"
+    return INT8_DENSE_SHEET, "H100 SXM data sheet, 1979 TOPS dense INT8"
 
 
 def timed(fn, reps):
@@ -145,15 +163,105 @@ def batch(n):
     return res
 
 
+def u8_vs_float(fds, pairs, reps):
+    """ps_match_u8_batch on the quantised sets against the float ps_match_batch on the same sets, timed alternately"""
+    L = api.load_library()
+    n = len(fds)
+    counts = [fd.getDescriptorCount() for fd in fds]
+    rows = sum(counts[i] for i, _ in pairs)
+    d_f, d_q = L.ps_dev_alloc(12 * max(rows, 1)), L.ps_dev_alloc(12 * max(rows, 1))
+    fptrs = [fd.getDescriptors() for fd in fds]
+    qptrs = [L.ps_dev_alloc(max(128 * c, 16)) for c in counts]
+    quant = lambda: [L.ps_descriptors_to_u8(0, fp, c, qp) for fp, c, qp in zip(fptrs, counts, qptrs)]  # noqa: E731
+    assert all(rc == 0 for rc in quant())
+    c_f, c_q = (C.c_void_p * n)(*fptrs), (C.c_void_p * n)(*qptrs)
+    c_n = (C.c_int32 * n)(*counts)
+    c_pairs = (C.c_int32 * (2 * len(pairs)))(*[v for pq in pairs for v in pq])
+    flag = api.FeaturesDev.MATCH_AUTO
+
+    def f32(flags=flag, out=d_f):
+        rc = L.ps_match_batch(0, n, c_f, c_n, len(pairs), c_pairs, out, flags)
+        assert rc == 0, L.ps_last_error(None)
+
+    def u8(flags=flag, out=d_q):
+        rc = L.ps_match_u8_batch(0, n, c_q, c_n, len(pairs), c_pairs, out, flags)
+        assert rc == 0, L.ps_last_error(None)
+
+    def fetch(d):
+        out = np.zeros((rows, 3), np.int32)
+        L.ps_dev_to_host(out.ctypes.data, d, out.nbytes)
+        return out
+    f32(); u8()                                 # warm-up of the same shapes
+    tf, tq = [], []
+    for _ in range(reps):                       # alternating, so that clock and thermal drift hit both alike
+        tf += timed(f32, 1)
+        tq += timed(u8, 1)
+    ops = 2.0 * 128 * sum(counts[i] * counts[j] for i, j in pairs)
+    peak, src = int8_peak()
+    res = {"pairs": len(pairs), "descriptors_per_set_min_max": [int(min(counts)), int(max(counts))]}
+    for name, ts in (("float_ps_match_batch", tf), ("u8_ps_match_u8_batch", tq)):
+        ms = float(np.median(ts))
+        res[name] = {"ms": ms, "ms_min_max": [float(min(ts)), float(max(ts))]}
+    res["u8_ps_match_u8_batch"]["int_tops"] = ops / (res["u8_ps_match_u8_batch"]["ms"] * 1e-3) / 1e12
+    res["u8_ps_match_u8_batch"]["frac_of_dense_int8"] = res["u8_ps_match_u8_batch"]["int_tops"] / peak
+    res["speedup_u8_vs_float"] = res["float_ps_match_batch"]["ms"] / res["u8_ps_match_u8_batch"]["ms"]
+    res["peak"] = {"int8_tops": peak, "source": src}
+    res["quantise_ms"] = float(np.median(timed(quant, 5)))
+    m_q = fetch(d_q)
+    f32(); m_f = fetch(d_f)
+    u8(api.FeaturesDev.MATCH_EXACT); m_e = fetch(d_q)
+    res["rows_differing_u8_vs_u8_exact"] = int((m_q != m_e).any(1).sum())
+    # informational: quantisation may change matches
+    res["rows_differing_u8_vs_float"] = int((m_q != m_f).any(1).sum())
+    res["accepted_u8"], res["accepted_float"] = int(m_q[:, 2].sum()), int(m_f[:, 2].sum())
+    res["accepted_differing_u8_vs_float"] = int(((m_q[:, 2] == 1) != (m_f[:, 2] == 1)).sum() +
+                                                ((m_q[:, 2] == 1) & (m_f[:, 2] == 1) & (m_q[:, 0] != m_f[:, 0])).sum())
+    for p in qptrs + [d_f, d_q]:
+        L.ps_dev_free(p)
+    return res
+
+
+def u8_four_k():
+    frames = bench.synth_frames(2, 0)
+    cfg = api.Config()
+    cfg.setOctaves(bench.OCTAVES); cfg.setLevels(bench.LEVELS); cfg.setNormalizationMultiplier(9)
+    pm = api.PopSift(cfg, mode=api.Config.MatchingMode, max_width=bench.W, max_height=bench.H, slots=2)
+    fds = [pm.enqueue(bench.W, bench.H, f).getDev() for f in frames]
+    res = {"workload": "one 4K pair (0, 1)", "norm_multi": 9}
+    res.update(u8_vs_float(fds, [(0, 1)], 10))
+    del fds
+    pm.uninit()
+    return res
+
+
+def u8_batch(n):
+    w, h = 1920, 1080
+    cfg = api.Config()
+    cfg.setNormalizationMultiplier(9)
+    pm = api.PopSift(cfg, mode=api.Config.MatchingMode, max_width=w, max_height=h, slots=2)
+    fds = [pm.enqueue(w, h, make_frame(w, h, 100 + k)).getDev() for k in range(n)]
+    res = {"workload": "%d 1920x1080 frames, all ordered pairs" % n, "norm_multi": 9}
+    res.update(u8_vs_float(fds, [(i, j) for i in range(n) for j in range(n) if i != j], 5))
+    del fds
+    pm.uninit()
+    return res
+
+
 def main():
     args = sys.argv[1:]
     pgm_dir, n_batch = None, 0
+    u8 = "--u8" in args
+    if u8:
+        args.remove("--u8")
     if "--pgm" in args:
         i = args.index("--pgm"); pgm_dir = args[i + 1]; del args[i:i + 2]
     if "--batch" in args:
         i = args.index("--batch"); n_batch = int(args[i + 1]); del args[i:i + 2]
     out = args[0] if args else None
-    res = batch(n_batch) if n_batch else four_k(pgm_dir)
+    if u8:
+        res = u8_batch(n_batch) if n_batch else u8_four_k()
+    else:
+        res = batch(n_batch) if n_batch else four_k(pgm_dir)
     res["card"] = card()
     res["library"] = api.LIB_PATH
     print(json.dumps(res))

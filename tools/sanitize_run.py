@@ -65,3 +65,13 @@ if only in ("all", "match-batch"):
     got = api.match_pairs(sets, pairs, api.FeaturesDev.MATCH_TENSOR)
     bad = sum(int((g != api.match_descriptors(sets[i], sets[j], api.FeaturesDev.MATCH_EXACT)).any(1).sum()) for g, (i, j) in zip(got, pairs))
     print("match-batch rows differing", bad, flush=True)
+if only in ("all", "match-u8"):
+    # the 8-bit matcher on ragged sets: self pairs, an empty left and an empty right set, a single-descriptor set, one
+    # left tile against 20 right tiles (S > 1); with POPSIFT_B200_MATCH_WS=300000 in the environment, several groups
+    rng = np.random.default_rng(2)
+    sets = [rng.integers(0, 64, size=(n, 128)).astype(np.uint8) for n in (100, 2500, 129, 0, 1800, 700, 1)]
+    pairs = [(0, 1), (1, 0), (2, 2), (3, 1), (1, 3), (4, 5), (5, 4), (0, 4), (2, 1), (1, 1), (6, 6), (0, 6)]
+    got = api.match_pairs_u8(sets, pairs, api.FeaturesDev.MATCH_TENSOR)
+    want = api.match_pairs_u8(sets, pairs, api.FeaturesDev.MATCH_EXACT)
+    q = api.descriptors_to_u8(rng.normal(scale=100.0, size=(37, 128)).astype(np.float32))
+    print("match-u8 rows differing", sum(int((g != w).any(1).sum()) for g, w in zip(got, want)), "quantised", q.shape, flush=True)
