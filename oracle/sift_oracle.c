@@ -761,7 +761,8 @@ static void orientation_one(const orc_ctx* c, const iext_t* ie, ext_t* e)
     for (int i = 0; i < 3; i++) { box3(hist, sm); box3(sm, hist); }
     memcpy(sm, hist, sizeof(sm));
 
-    float refined[ORI_NBINS], yval[ORI_NBINS];
+    float refined[64], yval[64];                 /* bins 36 .. 63: the sort's padding (no peak) */
+    for (int b = ORI_NBINS; b < 64; b++) { refined[b] = -1.0f; yval[b] = -INFINITY; }
     for (int b = 0; b < ORI_NBINS; b++) {
         const int prev = b == 0 ? ORI_NBINS - 1 : b - 1;
         const int next = b == ORI_NBINS - 1 ? 0 : b + 1;
@@ -774,13 +775,32 @@ static void orientation_one(const orc_ctx* c, const iext_t* ie, ext_t* e)
         refined[b] = pred ? (float)prev + newbin : -1.0f;
         yval[b] = pred ? -(num * num) / (4.0f * denB) + sm[prev] : -INFINITY;
     }
-    /* descending sort by yval (common/warp_bitonic_sort.h), top 4 with yval >= 0.8*best */
-    int idx[ORI_NBINS];
-    for (int b = 0; b < ORI_NBINS; b++) idx[b] = b;
-    for (int i = 1; i < ORI_NBINS; i++) {   /* stable insertion sort */
-        int k = idx[i], j = i - 1;
-        while (j >= 0 && yval[idx[j]] < yval[k]) { idx[j + 1] = idx[j]; j--; }
-        idx[j + 1] = k;
+    /* descending order of yval by the 64-wide warp bitonic network (s_orientation.cu:224-227, common/warp_bitonic_sort.h),
+     * top 4 with yval >= 0.8*best.  Lane l holds bins l (sequence 0) and l + 32 (sequence 1, yval -inf from bin 36 on);
+     * exact ties leave the network in its own order, which is the order of the orientations. */
+    int idx[ORIENTATION_MAX_COUNT];
+    {
+        const float* y64 = yval;
+        int seq[2][32];
+        for (int l = 0; l < 32; l++) { seq[0][l] = l; seq[1][l] = l + 32; }
+        for (int phase = 0; phase < 2; phase++) {
+            for (int k = 1; k <= 5; k++)
+                for (int j = k - 1; j >= 0; j--)
+                    for (int s = 0; s < 2; s++) {
+                        const int up = phase == 0 && s == 1;
+                        int nxt[32];
+                        for (int l = 0; l < 32; l++) {
+                            const float mine = y64[seq[s][l]], other = y64[seq[s][l ^ (1 << j)]];
+                            const int more = (l & (1 << j)) == 0 ? mine > other : mine < other;
+                            nxt[l] = more == (((l >> k) & 1) != up) ? seq[s][l ^ (1 << j)] : seq[s][l];
+                        }
+                        memcpy(seq[s], nxt, sizeof(nxt));
+                    }
+            if (phase == 0)
+                for (int l = 0; l < 32; l++)
+                    if (y64[seq[0][l]] < y64[seq[1][l]]) { const int t = seq[0][l]; seq[0][l] = seq[1][l]; seq[1][l] = t; }
+        }
+        for (int k = 0; k < ORIENTATION_MAX_COUNT; k++) idx[k] = seq[0][k];
     }
     const float best = yval[idx[0]];
     const float yref = 0.8f * best;
@@ -1021,4 +1041,24 @@ int orc_download(const orc_ctx* c, orc_feature* feat, float* desc128)
     }
     if (desc128 && c->desc) memcpy(desc128, c->desc, (size_t)c->n_desc * 128 * sizeof(float));
     return 0;
+}
+
+/* The descriptor stage alone, on the caller's keypoints and orientations (octave-local x, y, sigma, angle; octave and
+ * lpos): separates the descriptor arithmetic from the orientation stage, whose angles come from libm here and from
+ * the CUDA math library in the reference.  Needs the pyramid of a previous orc_run_*. */
+int orc_describe(const orc_ctx* c, int n, const float* kp4, const int32_t* oct_lpos, float* desc128)
+{
+    int bad = 0;
+    #pragma omp parallel for schedule(dynamic, 64) reduction(+:bad)
+    for (int i = 0; i < n; i++) {
+        float* f = desc128 + (size_t)128 * i;
+        ext_t e;
+        memset(&e, 0, sizeof(e));
+        e.x = kp4[4 * i]; e.y = kp4[4 * i + 1]; e.sigma = kp4[4 * i + 2];
+        e.octave = oct_lpos[2 * i]; e.lpos = oct_lpos[2 * i + 1];
+        if (e.octave < 0 || e.octave >= c->noct) { memset(f, 0, 128 * sizeof(float)); bad++; continue; }
+        descriptor_one(c, &e, kp4[4 * i + 3], f);
+        normalize_desc(c, f);
+    }
+    return bad ? -1 : 0;
 }

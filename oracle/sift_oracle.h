@@ -103,6 +103,8 @@ int      orc_num_extrema(const orc_ctx* ctx);
 int      orc_get_extrema(const orc_ctx* ctx, float* out5);
 int      orc_counts(const orc_ctx* ctx, int32_t* n_feat, int32_t* n_desc);
 int      orc_download(const orc_ctx* ctx, orc_feature* feat, float* desc128);
+/* descriptors of n caller-given keypoints: kp4 = n x {x, y, sigma, angle} (octave-local), oct_lpos = n x {octave, lpos} */
+int      orc_describe(const orc_ctx* ctx, int n, const float* kp4, const int32_t* oct_lpos, float* desc128);
 /* stand-alone: normalised value the input texture returns (pins the texture model) */
 float    orc_tex_u8(const uint8_t* img, int w, int h, float rx, float ry);
 float    orc_tex_f32(const float* img, int w, int h, float rx, float ry);

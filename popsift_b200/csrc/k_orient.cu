@@ -15,7 +15,8 @@
 //     orientations and the same angles.  (Round 1 summed lane-private bins in lane order: 925 of 453 753
 //     keypoints of the benchmark frames then differed in the last bits of an angle, and 7 in the NUMBER of
 //     orientations -- 522 535 vs 522 542 descriptors.);
-//   * top-4 selection by four warp arg-max rounds instead of a 64-wide bitonic sort.
+//   * the top 4 peaks come from the reference's 64-wide warp bitonic network with values carried instead of bin
+//     indices, so that exact ties leave it in the reference's order.
 // Per-sample math is the reference's: hypotf/atan2f gradients of the data plane lpos,
 // weight = grad*expf(int(sq_dist)*__fdividef(-0.5, sigw^2)), bin = round(36*(theta+pi)/2pi),
 // 3x(box3, box3) smoothing, parabola refinement, peaks >= 0.8*best, theta = fma(2pi*bin, 1/36, -pi).
@@ -201,24 +202,41 @@ orientation_kernel(PyramidView pyr, Consts k, const InitialExtremum* __restrict_
                 if (pred) { ra[s] = (float)pv + newbin; yv[s] = -(num * num) / (4.0f * den) + hp; }
             }
         }
-        // four arg-max rounds (descending yval; ties -> lower bin)
+        // Descending order of yval by the reference's 64-wide warp bitonic network (s_orientation.cu:224-227,
+        // common/warp_bitonic_sort.h): a lane holds bins `lane` (sequence 0) and `lane + 32` (sequence 1); both
+        // sequences are sorted, opposite ways, the lanes compare-exchange across them, and both are sorted again.  On
+        // exact ties in yval (symmetric content: checkerboards, plateaus) the order in which the network leaves them is
+        // the order of Feature::orientation[] and of the descriptors; a plain arg-max would order ties differently.
+        auto cmp_xchg = [&](float& y, float& r, int j, int k, bool up) {
+            const float oy = __shfl_xor_sync(0xffffffffu, y, 1 << j);
+            const float orr = __shfl_xor_sync(0xffffffffu, r, 1 << j);
+            const bool mine_more = (lane & (1 << j)) == 0 ? (y > oy) : (y < oy);
+            if (mine_more == (((lane >> k) & 1) != (up ? 1 : 0))) { y = oy; r = orr; }
+        };
+#pragma unroll
+        for (int k = 1; k <= 5; ++k)
+#pragma unroll
+            for (int j = k - 1; j >= 0; --j) {
+                cmp_xchg(yv[0], ra[0], j, k, false);
+                cmp_xchg(yv[1], ra[1], j, k, true);
+            }
+        if (yv[0] < yv[1]) {
+            const float ty = yv[0], tr = ra[0];
+            yv[0] = yv[1]; ra[0] = ra[1]; yv[1] = ty; ra[1] = tr;
+        }
+#pragma unroll
+        for (int k = 1; k <= 5; ++k)
+#pragma unroll
+            for (int j = k - 1; j >= 0; --j) {
+                cmp_xchg(yv[0], ra[0], j, k, false);
+                cmp_xchg(yv[1], ra[1], j, k, false);
+            }
+        // lanes 0 .. 3 of sequence 0 hold the four largest, in order
         float best_y[PS_MAX_ORI], best_r[PS_MAX_ORI];
 #pragma unroll
         for (int r = 0; r < PS_MAX_ORI; ++r) {
-            float cy; int cb;
-            if (yv[0] >= yv[1] || !(yv[1] == yv[1])) { cy = yv[0]; cb = lane; } else { cy = yv[1]; cb = lane + 32; }
-            float wy = cy; int wb = cb;
-#pragma unroll
-            for (int d = 16; d >= 1; d >>= 1) {
-                const float oy = __shfl_xor_sync(0xffffffffu, wy, d);
-                const int ob = __shfl_xor_sync(0xffffffffu, wb, d);
-                if (oy > wy || (oy == wy && ob < wb)) { wy = oy; wb = ob; }
-            }
-            // owner publishes its refined angle and retires the bin
-            const int owner = wb & 31, slot = wb >> 5;
-            const float rr = __shfl_sync(0xffffffffu, slot ? ra[1] : ra[0], owner);
-            best_y[r] = wy; best_r[r] = rr;
-            if (lane == owner) { if (slot) yv[1] = -INFINITY; else yv[0] = -INFINITY; }
+            best_y[r] = __shfl_sync(0xffffffffu, yv[0], r);
+            best_r[r] = __shfl_sync(0xffffffffu, ra[0], r);
         }
         const float yref = __fmul_rn(0.8f, best_y[0]);
         if (lane == 0) {

@@ -10,7 +10,10 @@ commit:
 bench32.npz holds the 32 benchmark frames (octaves=5, levels=3): per frame the counts and the sha256 of the sorted
 keypoint keys, orientation counts and angles, and a sample of 16 descriptors per frame.
 
-    python tests/golden/make_golden_live.py OUTDIR        (on a GPU machine, with oracle/_ref/ref_dump built)
+stress_*.npz / knob_*.npz are runs on the adversarial images of tests/stress_images.py (STRESS_RUNS), with the octave-0
+planes of their --log dumps.
+
+    python tests/golden/make_golden_live.py OUTDIR [--only 'stress_*']   (on a GPU machine, with oracle/_ref/ref_dump built)
 """
 import hashlib
 import json
@@ -77,6 +80,39 @@ RUNS = {
 }
 
 
+def ocv(*extra):
+    return ["--mode", "opencv", "--norm", "classic"] + list(extra)
+
+
+# name -> (tests/stress_images.py image, ref_dump arguments): test_stress_parity.py::test_stress_vs_reference_runs
+STRESS_RUNS = {
+    "stress_checker_p8_prs": ("checker_p8", prs()),
+    "stress_checker_p8_ocv": ("checker_p8", ocv()),
+    "stress_checker_rot30_p6_prs": ("checker_rot30_p6", prs()),
+    "stress_checker_rot30_p6_vlc": ("checker_rot30_p6", vlc()),
+    "stress_block_noise_4_prs": ("block_noise_4", prs()),
+    "stress_block_noise_4_ocv": ("block_noise_4", ocv()),
+    "stress_block_noise_4_vlc": ("block_noise_4", vlc()),
+    "stress_binary_noise_vlc": ("binary_noise", vlc()),
+    "stress_saturated_prs": ("saturated", prs()),
+    "stress_dark_prs": ("dark", prs("--threshold", "0.001")),
+    "stress_border_impulses_prs": ("border_impulses", prs()),
+    "stress_border_impulses_ocv": ("border_impulses", ocv()),
+    "stress_step_edges_vlc": ("step_edges", vlc()),
+    # the Config knobs structure-from-motion callers set
+    "knob_threshold_0.005": ("saturated", prs("--threshold", "0.005")),
+    "knob_threshold_0.1": ("saturated", prs("--threshold", "0.1")),
+    "knob_edge_2": ("saturated", prs("--edge-limit", "2")),
+    "knob_edge_50": ("saturated", prs("--edge-limit", "50")),
+    "knob_iblur_0": ("saturated", prs("--initial-blur", "0")),
+    "knob_iblur_1": ("saturated", prs("--initial-blur", "1")),
+    "knob_iblur_1_block_noise_4": ("block_noise_4", prs("--initial-blur", "1")),
+    "knob_nm9_rs": ("block_noise_4", prs("--norm-multi", "9")),
+    "knob_nm3_classic": ("block_noise_4", vlc("--norm-multi", "3")),
+    "knob_sigma2_l2": ("checker_rot30_p6", prs("--sigma", "2.0", "--levels", "2")),
+}
+
+
 def sample_rows(n, seed, keep_all=False):
     if keep_all or n <= MAX_DESC:
         return np.arange(n, dtype=np.int64)
@@ -98,7 +134,10 @@ def run_one(td, img, args, log_octaves):
     planes = {}
     for oc in range(log_octaves):
         for lv in range(6):
-            p = ol.read_ref_dump(os.path.join(td, "dir-octave-dump", "pyramid-o-%d-l-%d.dump" % (oc, lv)))
+            fn = os.path.join(td, "dir-octave-dump", "pyramid-o-%d-l-%d.dump" % (oc, lv))
+            if lv == 5 and not os.path.exists(fn):         # levels = 2: five Gaussian planes per octave
+                break
+            p = ol.read_ref_dump(fn)
             planes["%d_%d" % (oc, lv)] = [p.shape[0], p.shape[1], hashlib.sha256(p.tobytes()).hexdigest()]
     return feat, desc, planes
 
@@ -138,20 +177,42 @@ def bench32_keys(feat):
 
 
 def main():
-    out = sys.argv[1]
+    import argparse
+    import fnmatch
+    ap = argparse.ArgumentParser()
+    ap.add_argument("out")
+    ap.add_argument("--only", default="*", help="make only the runs whose name matches this shell pattern, e.g. 'stress_*'")
+    a = ap.parse_args()
+    out = a.out
     os.makedirs(out, exist_ok=True)
+    want = lambda name: fnmatch.fnmatchcase(name, a.only)   # noqa: E731
+    # the sample seed of a run is its index in the sorted table: the stress / knob runs are numbered separately so that
+    # adding them left the earlier fixtures unchanged
     for k, (name, (w, h, seed, args, log_oc)) in enumerate(sorted(RUNS.items())):
+        if not want(name):
+            continue
         with tempfile.TemporaryDirectory() as td:
             feat, desc, planes = run_one(td, make_frame(w, h, seed), args, log_oc)
         save_run(os.path.join(out, name + ".npz"), feat, desc, planes, k)
         print(name, len(feat), len(desc), flush=True)
+    import stress_images
+    for k, (name, (img_name, args)) in enumerate(sorted(STRESS_RUNS.items())):
+        if not want(name):
+            continue
+        with tempfile.TemporaryDirectory() as td:
+            feat, desc, planes = run_one(td, stress_images.image(img_name), args, 1)
+        save_run(os.path.join(out, name + ".npz"), feat, desc, planes, 500 + k)
+        print(name, len(feat), len(desc), flush=True)
     for k, (im, _A) in enumerate(affine_set(), 1):
+        if not want("aff%d" % k):
+            continue
         with tempfile.TemporaryDirectory() as td:
             feat, desc, planes = run_one(td, im, vlc(), 0)
         save_run(os.path.join(out, "aff%d.npz" % k), feat, desc, planes, 100 + k, keep_all=True)
         print("aff%d" % k, len(feat), len(desc), flush=True)
-    bench32(out)
-    print("bench32 done", flush=True)
+    if want("bench32"):
+        bench32(out)
+        print("bench32 done", flush=True)
 
 
 if __name__ == "__main__":

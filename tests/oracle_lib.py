@@ -79,6 +79,7 @@ def lib():
         L.orc_get_extrema.argtypes = [C.c_void_p, C.c_void_p]
         L.orc_counts.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
         L.orc_download.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.orc_describe.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.orc_compute_tables.argtypes = [C.POINTER(OrcConfig), C.POINTER(OrcTables)]
         L.orc_geometry.argtypes = [C.POINTER(OrcConfig), C.c_int, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
         L.orc_default_config.argtypes = [C.POINTER(OrcConfig)]
@@ -168,6 +169,16 @@ class Oracle:
         desc = np.zeros((nd.value, 128), dtype=np.float32)
         lib().orc_download(self.ctx, feat.ctypes.data, desc.ctypes.data)
         return feat, desc
+
+    def describe(self, x, y, sigma, angle, octave, lpos) -> np.ndarray:
+        """normalised descriptors [n, 128] of the given keypoints (octave-local x, y, sigma; orientation angle) on this
+        run's pyramid: the descriptor stage alone, at someone else's orientations"""
+        kp = np.ascontiguousarray(np.stack([x, y, sigma, angle], 1), dtype=np.float32)
+        ol_ = np.ascontiguousarray(np.stack([octave, lpos], 1), dtype=np.int32)
+        out = np.zeros((len(kp), 128), dtype=np.float32)
+        if len(kp):
+            assert lib().orc_describe(self.ctx, len(kp), kp.ctypes.data, ol_.ctypes.data, out.ctypes.data) == 0
+        return out
 
 
 # ---- readers for files written by the reference (oracle/ref_driver.cpp, write_plane_2d.cu:142-178)
