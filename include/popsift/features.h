@@ -31,6 +31,17 @@ struct Feature
 
 std::ostream& operator<<(std::ostream& ostr, const Feature& feature);
 
+/// A keypoint for PopSift::describe, in input-image units like Feature (same bytes as ps_keypoint, 24).
+struct Keypoint
+{
+    float xpos;
+    float ypos;
+    float sigma;
+    float orientation = 0.0f;   // radians; used unless describe() computes the orientations
+    int   octave = -1;          // -1: derived from sigma; else the octave, as Feature::debug_octave
+    int   level = -1;           // -1: derived from sigma; else the Gaussian level of the octave, 0 .. levels+2
+};
+
 class FeaturesBase
 {
     int _num_ext;

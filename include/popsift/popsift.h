@@ -18,6 +18,7 @@
 #include <future>
 #include <memory>
 #include <string>
+#include <vector>
 
 struct ps_ctx;
 
@@ -30,10 +31,15 @@ class SiftJob
     unsigned char* _imageData;
     bool           _isFloat;
     std::exception_ptr _err;
+    int            _describe = -1;                // -1: detection; else the ps_describe_* flags
+    std::vector<popsift::Keypoint> _keypoints;    // describe jobs: the caller's keypoints
 
 public:
     SiftJob(int w, int h, const unsigned char* imageData);
     SiftJob(int w, int h, const float* imageData);
+    /// a describe job (PopSift::describe): copies the image and the keypoints
+    SiftJob(int w, int h, const unsigned char* imageData, const std::vector<popsift::Keypoint>& kps, bool computeOrientations);
+    SiftJob(int w, int h, const float* imageData, const std::vector<popsift::Keypoint>& kps, bool computeOrientations);
     ~SiftJob();
 
     popsift::FeaturesHost* get();
@@ -49,6 +55,8 @@ public:
     int                  height() const { return _h; }
     const unsigned char* pixels() const { return _imageData; }
     bool                 isFloat() const { return _isFloat; }
+    int                  describeFlags() const { return _describe; }
+    const std::vector<popsift::Keypoint>& keypoints() const { return _keypoints; }
 };
 
 class PopSift
@@ -74,6 +82,14 @@ public:
 
     SiftJob* enqueue(int w, int h, const unsigned char* imageData);
     SiftJob* enqueue(int w, int h, const float* imageData);
+
+    /// Orientations (computeOrientations) and descriptors at the caller's keypoints instead of detected ones (extension;
+    /// C ABI ps_describe_u8 / ps_describe_f32).  The job's features hold one Feature per keypoint, in input order, with
+    /// num_ori = 0 for a rejected keypoint.  Describe and enqueue jobs share one FIFO; get() / getDev() as for enqueue.
+    SiftJob* describe(int w, int h, const unsigned char* imageData, const std::vector<popsift::Keypoint>& kps,
+                      bool computeOrientations = false);
+    SiftJob* describe(int w, int h, const float* imageData, const std::vector<popsift::Keypoint>& kps,
+                      bool computeOrientations = false);
 
     /// number of images in flight on the device (extension; the reference has 1)
     void setSlots(int n);

@@ -225,6 +225,45 @@ int ps_descriptors_to_u8(int device, const ps_descriptor* d_in, int n, uint8_t* 
  * -> s32), PS_MATCH_EXACT a CUDA-core kernel pair by pair. */
 int ps_match_u8_batch(int device, int n_sets, const uint8_t* const* d_sets, const int32_t* n_desc,
                       int n_pairs, const int32_t* pairs, int32_t* d_out, int flags);
+/* ---- describe: orientations and descriptors at caller-supplied keypoints (an addition to the reference's interface;
+ * VLFeat's vl_sift 'Frames' / 'Orientations', OpenCV's Feature2D::compute).  Used for tracking, upright SIFT, dense SIFT,
+ * keypoints from another detector and re-describing stored keypoints under another desc_mode / norm_mode. */
+
+/* A keypoint to describe, in input-image units exactly like ps_feature (24 bytes). */
+typedef struct ps_keypoint {
+    float   xpos, ypos, sigma;
+    float   orientation;   /* radians; used unless PS_DESCRIBE_ORIENT */
+    int32_t octave;        /* -1: derived from sigma (rule below); else the octave, as ps_feature::debug_octave */
+    int32_t level;         /* -1: derived from sigma; else the Gaussian level (ps_extremum::lpos), 0 .. L+2 */
+} ps_keypoint;
+enum { PS_DESCRIBE_GIVEN = 0, PS_DESCRIBE_ORIENT = 1 };
+/* Builds the slot's pyramid of the image (same rules as ps_submit_u8 / ps_submit_f32: lifetime, page-locked staging, size
+ * checks), skips the extrema stage and the grid filter, and describes the n keypoints of the host array kps (copied
+ * before the call returns).  Results are read with ps_counts / ps_download / ps_download_dev as after a submission:
+ *   - one Feature per keypoint, in input order: n_feat == n, Feature i is keypoint i, with the keypoint's own xpos, ypos
+ *     and sigma bits and debug_octave = the octave used (-1 for a rejected keypoint); the descriptors of Feature i follow
+ *     those of Feature i - 1, and ps_download_dev's reverse map points into input order;
+ *   - PS_DESCRIBE_GIVEN: num_ori = 1, orientation[0] = the given angle, one descriptor at it;
+ *   - PS_DESCRIBE_ORIENT: the orientation stage runs at the keypoint (the given angle is ignored): num_ori 1 .. 4 and the
+ *     angles as for a detected extremum;
+ *   - a rejected keypoint keeps its place with num_ori = 0, zero angles and no descriptor (not an error).  Rejected are:
+ *     a non-finite x, y or sigma (under GIVEN also angle); sigma <= 0; an explicit octave outside [0, n_octaves) or an
+ *     explicit level outside [0, L+2] (any negative value other than -1 is explicit); a position outside
+ *     [0, W_o - 1] x [0, H_o - 1] of its octave, where local = image * 2^(up_fac - octave) (exact);
+ *   - a derived octave and level, in float32 with up_fac = (int)upscale, sigma0 = ps_config::sigma, L = levels:
+ *         S      = L * (log2f(sigma) + up_fac - log2f(sigma0))
+ *         octave = clamp(floor((S - 0.5) / L), 0, n_octaves - 1)
+ *         level  = clamp(roundf(S - octave * L), 0, L + 2)        (with the explicit octave if only the level is -1)
+ *     For a detected keypoint with 1 <= lpos <= L this gives back its (octave, lpos), except within float rounding of a
+ *     half-integer scale.
+ * n is limited only by int32 and device memory (the slot's buffers grow).  All desc_modes and norm_modes apply.
+ * Detection and describe calls may alternate on one slot; a describe call launches directly, never through the slot's
+ * CUDA graph, and ps_stage_ms reports 0 ms for its extrema stage.
+ * Returns PS_ERR_ARG for n < 0, kps == NULL with n > 0 or unknown flags, PS_ERR_TOO_LARGE as ps_submit_*; n = 0 is valid
+ * and gives zero features. */
+int ps_describe_u8 (ps_ctx* ctx, int slot, const uint8_t* host_img, int w, int h, const ps_keypoint* kps, int n, int flags);
+int ps_describe_f32(ps_ctx* ctx, int slot, const float*   host_img, int w, int h, const ps_keypoint* kps, int n, int flags);
+
 /* page-locked host memory for images and results (thin wrappers of cudaHostAlloc / cudaFreeHost).
  * ps_submit_* and ps_download detect page-locked buffers and copy straight from / into them; pageable
  * buffers are staged through the slot's own pinned buffers (one extra host memcpy). */

@@ -51,14 +51,17 @@ FEATURE_DTYPE = np.dtype([("octave", "<i4"), ("x", "<f4"), ("y", "<f4"), ("sigma
                           ("ori", "<f4", (4,)), ("pad", "<i4"), ("desc_ptr", "<u8", (4,))])
 EXTREMUM_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("lpos", "<i4"), ("sigma", "<f4"), ("octave", "<i4"),
                            ("num_ori", "<i4"), ("idx_ori", "<i4"), ("ori", "<f4", (4,))])
-assert FEATURE_DTYPE.itemsize == 72 and EXTREMUM_DTYPE.itemsize == 44
+# ps_keypoint: a keypoint for PopSift.describe, in input-image units; octave / level -1 = derived from sigma
+KEYPOINT_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("sigma", "<f4"), ("ori", "<f4"), ("octave", "<i4"), ("level", "<i4")])
+assert FEATURE_DTYPE.itemsize == 72 and EXTREMUM_DTYPE.itemsize == 44 and KEYPOINT_DTYPE.itemsize == 24
+DESCRIBE_GIVEN, DESCRIBE_ORIENT = 0, 1
 
 EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps_geometry", "ps_create", "ps_destroy",
            "ps_last_error", "ps_submit_u8", "ps_submit_f32", "ps_submit_dev_u8", "ps_counts", "ps_download",
            "ps_sync", "ps_debug_plane", "ps_debug_extrema", "ps_slot_geometry", "ps_set_timing", "ps_stage_ms",
            "ps_launch_count", "ps_slot_stream", "ps_run_pyramid_only", "ps_run_level_only", "ps_host_alloc", "ps_host_free",
            "ps_download_dev", "ps_dev_alloc", "ps_dev_free", "ps_dev_to_host", "ps_wait_input", "ps_match", "ps_match_batch", "ps_pointer_device", "ps_host_to_dev",
-           "ps_descriptors_to_u8", "ps_match_u8_batch",
+           "ps_descriptors_to_u8", "ps_match_u8_batch", "ps_describe_u8", "ps_describe_f32",
            "ps_debug_level0_plan", "ps_format_gauss_tables"]
 
 _lib = None
@@ -95,6 +98,9 @@ def load_library():
     if hasattr(L, "ps_match_u8_batch"):
         L.ps_descriptors_to_u8.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p]
         L.ps_match_u8_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+    if hasattr(L, "ps_describe_u8"):
+        L.ps_describe_u8.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
+        L.ps_describe_f32.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -581,6 +587,18 @@ def match_pairs_u8(sets, pairs, flags=0, device=None) -> list:
     return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
 
 
+def keypoints_array(keypoints) -> np.ndarray:
+    """a contiguous KEYPOINT_DTYPE array from a KEYPOINT_DTYPE array or an (n, 4) array of x, y, sigma, angle (octave and
+    level -1)"""
+    if isinstance(keypoints, np.ndarray) and keypoints.dtype == KEYPOINT_DTYPE:
+        return np.ascontiguousarray(keypoints)
+    a = np.asarray(keypoints, dtype=np.float32).reshape(-1, 4)
+    out = np.zeros(len(a), KEYPOINT_DTYPE)
+    out["x"], out["y"], out["sigma"], out["ori"] = a[:, 0], a[:, 1], a[:, 2], a[:, 3]
+    out["octave"] = out["level"] = -1
+    return out
+
+
 class SiftJob:
     """SiftJob (reference src/popsift/popsift.h:44-100): get() blocks until the features are there."""
 
@@ -653,6 +671,33 @@ class PopSift:
         fn = self._lib.ps_submit_u8 if self._imode == self.ByteImages else self._lib.ps_submit_f32
         self._keep[slot] = img           # released when the slot's next image is submitted (its job has completed by then)
         self._check(fn(self._ctx, slot, img.ctypes.data, w, h))
+        job = SiftJob(self, slot)
+        self._busy[slot] = job
+        return job
+
+    def describe(self, w: int, h: int, image, keypoints, orientations: bool = False) -> SiftJob:
+        """Orientations (orientations=True) and descriptors at the caller's keypoints instead of detected ones (C ABI
+        ps_describe_u8 / ps_describe_f32).  `keypoints` is a KEYPOINT_DTYPE array, or an (n, 4) float array of x, y, sigma,
+        angle (radians) in input-image units with octave = level = -1 (derived from sigma).  The job's Features hold one
+        record per keypoint, in input order; a rejected keypoint has num_ori 0.  Same FIFO of slots as enqueue."""
+        img = np.ascontiguousarray(image)
+        want = np.uint8 if self._imode == self.ByteImages else np.float32
+        if img.dtype != want:
+            raise PopSiftError("Image mode error")
+        assert img.size == w * h
+        kps = keypoints_array(keypoints)
+        if self._ctx is None:
+            self._create(w, h)
+        if w > self._max[0] or h > self._max[1]:
+            raise PopSiftError("image larger than the context was created for")
+        slot = self._next
+        self._next = (self._next + 1) % self._nslots
+        if self._busy[slot] is not None:
+            self._busy[slot].getBase()
+        fn = self._lib.ps_describe_u8 if self._imode == self.ByteImages else self._lib.ps_describe_f32
+        self._keep[slot] = img
+        self._check(fn(self._ctx, slot, img.ctypes.data, w, h, kps.ctypes.data, len(kps),
+                       DESCRIBE_ORIENT if orientations else DESCRIBE_GIVEN))
         job = SiftJob(self, slot)
         self._busy[slot] = job
         return job

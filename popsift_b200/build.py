@@ -26,7 +26,7 @@ NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "--fmad=false",   # no implicit contraction anywhere; every fma in the kernels is explicit
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu",
+LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu",
                "host/sift_conf.cpp", "host/features.cpp", "host/popsift.cpp", "host/device_prop.cpp", "host/log_dump.cpp"]
 DEMO_SOURCES = ["app/popsift_demo.cpp", "app/pgmread.cpp"]
 MATCH_SOURCES = ["app/popsift_match.cpp"]            # + app/pgmread.cpp
@@ -47,6 +47,8 @@ MATCH_PAIRS_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_pairs_check.cp
 MATCH_U8_CHECK = os.path.join(BIN_DIR, "match_u8_check")
 MATCH_U8_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_u8_check.cpp")
 PGM_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "pgmread_check.cpp")
+DESCRIBE_CHECK = os.path.join(BIN_DIR, "describe_check")
+DESCRIBE_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "describe_check.cpp")
 
 
 def _newer(target: str, deps) -> bool:
@@ -130,6 +132,10 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if os.path.exists(MATCH_U8_CHECK_SRC) and (force or _newer(MATCH_U8_CHECK, [MATCH_U8_CHECK_SRC, LIB] + hdrs)):
         # popsift::matchPairsU8 against the float matcher on the quantised descriptors, through the C++ and C APIs
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), MATCH_U8_CHECK_SRC, "-o", MATCH_U8_CHECK,
+                               "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
+    if os.path.exists(DESCRIBE_CHECK_SRC) and (force or _newer(DESCRIBE_CHECK, [DESCRIBE_CHECK_SRC, LIB] + hdrs)):
+        # PopSift::describe round trip with describe and enqueue jobs in one FIFO, through the C++ API
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), DESCRIBE_CHECK_SRC, "-o", DESCRIBE_CHECK,
                                "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
     pgm_src = os.path.join(CSRC, "app", "pgmread.cpp")
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):

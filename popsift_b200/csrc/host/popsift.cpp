@@ -56,6 +56,22 @@ SiftJob::SiftJob(int w, int h, const float* imageData) : _w(w), _h(h), _isFloat(
     popsift::detail::parallel_copy(_imageData, imageData, n);
 }
 
+static_assert(sizeof(popsift::Keypoint) == sizeof(ps_keypoint) && sizeof(popsift::Keypoint) == 24, "popsift::Keypoint is ps_keypoint");
+
+SiftJob::SiftJob(int w, int h, const unsigned char* imageData, const std::vector<popsift::Keypoint>& kps, bool computeOrientations)
+    : SiftJob(w, h, imageData)
+{
+    _describe = computeOrientations ? PS_DESCRIBE_ORIENT : PS_DESCRIBE_GIVEN;
+    _keypoints = kps;
+}
+
+SiftJob::SiftJob(int w, int h, const float* imageData, const std::vector<popsift::Keypoint>& kps, bool computeOrientations)
+    : SiftJob(w, h, imageData)
+{
+    _describe = computeOrientations ? PS_DESCRIBE_ORIENT : PS_DESCRIBE_GIVEN;
+    _keypoints = kps;
+}
+
 SiftJob::~SiftJob() { popsift::detail::pinned_pool().put(_imageData); }
 
 void SiftJob::setFeatures(popsift::FeaturesBase* f) { _p.set_value(f); }
@@ -207,8 +223,16 @@ PopSift::PopSift(ImageMode imode, int device) : _pipe(new Pipe), _image_mode(imo
             }
             const int s = p->next_slot;
             finish(s);
-            const int rc = job->isFloat() ? ps_submit_f32(p->ctx, s, reinterpret_cast<const float*>(job->pixels()), w, h)
-                                          : ps_submit_u8(p->ctx, s, job->pixels(), w, h);
+            int rc;
+            if (job->describeFlags() >= 0) {
+                const ps_keypoint* kps = reinterpret_cast<const ps_keypoint*>(job->keypoints().data());
+                const int n = (int)job->keypoints().size();
+                rc = job->isFloat() ? ps_describe_f32(p->ctx, s, reinterpret_cast<const float*>(job->pixels()), w, h, kps, n, job->describeFlags())
+                                    : ps_describe_u8(p->ctx, s, job->pixels(), w, h, kps, n, job->describeFlags());
+            } else {
+                rc = job->isFloat() ? ps_submit_f32(p->ctx, s, reinterpret_cast<const float*>(job->pixels()), w, h)
+                                    : ps_submit_u8(p->ctx, s, job->pixels(), w, h);
+            }
             if (rc != PS_OK) {
                 // the copy out of the job's page-locked image may already be queued: let it finish before
                 // the caller can delete the job (and hand its block back to the pool)
@@ -316,6 +340,40 @@ SiftJob* PopSift::enqueue(int w, int h, const float* imageData)
         return nullptr;
     }
     SiftJob* job = new SiftJob(w, h, imageData);
+    Pipe* p = _pipe.get();
+    { std::lock_guard<std::mutex> lk(p->mu); p->queue.push_back(job); }
+    p->cv.notify_all();
+    return job;
+}
+
+SiftJob* PopSift::describe(int w, int h, const unsigned char* imageData, const std::vector<popsift::Keypoint>& kps, bool computeOrientations)
+{
+    if (_image_mode != ByteImages)
+        throw std::runtime_error("Image mode error\nE    Cannot load byte images into a PopSift pipeline configured for float images");
+    const AllocTest a = testTextureFit(w, h);
+    if (a != Ok) {
+        std::cerr << __FILE__ << ":" << __LINE__ << " Image too large" << std::endl << testTextureFitErrorString(a, w, h);
+        return nullptr;
+    }
+    if (kps.size() > (size_t)INT32_MAX) throw std::runtime_error("PopSift::describe: more than 2^31 - 1 keypoints");
+    SiftJob* job = new SiftJob(w, h, imageData, kps, computeOrientations);
+    Pipe* p = _pipe.get();
+    { std::lock_guard<std::mutex> lk(p->mu); p->queue.push_back(job); }
+    p->cv.notify_all();
+    return job;
+}
+
+SiftJob* PopSift::describe(int w, int h, const float* imageData, const std::vector<popsift::Keypoint>& kps, bool computeOrientations)
+{
+    if (_image_mode != FloatImages)
+        throw std::runtime_error("Image mode error\nE    Cannot load float images into a PopSift pipeline configured for byte images");
+    const AllocTest a = testTextureFit(w, h);
+    if (a != Ok) {
+        std::cerr << __FILE__ << ":" << __LINE__ << " Image too large" << std::endl << testTextureFitErrorString(a, w, h);
+        return nullptr;
+    }
+    if (kps.size() > (size_t)INT32_MAX) throw std::runtime_error("PopSift::describe: more than 2^31 - 1 keypoints");
+    SiftJob* job = new SiftJob(w, h, imageData, kps, computeOrientations);
     Pipe* p = _pipe.get();
     { std::lock_guard<std::mutex> lk(p->mu); p->queue.push_back(job); }
     p->cv.notify_all();

@@ -345,6 +345,12 @@ ori_scatter_kernel(int num_octaves, Consts k, ps_extremum* __restrict__ ext, int
 int launch_orientation(const PyramidView& pyr, const Consts& k, const InitialExtremum* iext, const InitialExtremum* iext_f, ps_extremum* ext,
                        int* feat_to_ext, int* slice_sum, Counters* ct, cudaStream_t st)
 {
+    return launch_orientation_only(pyr, k, iext, iext_f, ext, slice_sum, ct, st) + launch_ori_scatter(pyr.num_octaves, k, ext, feat_to_ext, slice_sum, ct, st);
+}
+
+int launch_orientation_only(const PyramidView& pyr, const Consts& k, const InitialExtremum* iext, const InitialExtremum* iext_f, ps_extremum* ext,
+                            int* slice_sum, Counters* ct, cudaStream_t st)
+{
     // fixed grid: SMs x 8 resident CTAs of 4 warps; warps stride over the device-side count
     static const bool lanesum = [] { const char* e = getenv("POPSIFT_B200_ORI_LANESUM"); return e && e[0] == '1'; }();
     // experiments: POPSIFT_B200_ORI_WARPS=1 -> one warp per CTA like the reference's ori_par; POPSIFT_B200_ORI_GRID=n -> n CTAs
@@ -357,8 +363,13 @@ int launch_orientation(const PyramidView& pyr, const Consts& k, const InitialExt
     else if (batch == 2) orientation_kernel<true, kWarps, 2><<<grid, kWarps * 32, 0, st>>>(pyr, k, iext, iext_f, ext, slice_sum, ct);
     else if (batch == 4) orientation_kernel<true, kWarps, 4><<<grid, kWarps * 32, 0, st>>>(pyr, k, iext, iext_f, ext, slice_sum, ct);
     else                 orientation_kernel<true, kWarps, 1><<<grid, kWarps * 32, 0, st>>>(pyr, k, iext, iext_f, ext, slice_sum, ct);
-    ori_scatter_kernel<<<k.ext_capacity / kSlice + 1, kSlice, 0, st>>>(pyr.num_octaves, k, ext, feat_to_ext, slice_sum, ct);
-    return 2;
+    return 1;
+}
+
+int launch_ori_scatter(int num_octaves, const Consts& k, ps_extremum* ext, int* feat_to_ext, const int* slice_sum, Counters* ct, cudaStream_t st)
+{
+    ori_scatter_kernel<<<k.ext_capacity / kSlice + 1, kSlice, 0, st>>>(num_octaves, k, ext, feat_to_ext, slice_sum, ct);
+    return 1;
 }
 
 } // namespace psb

@@ -72,6 +72,16 @@ struct Slot {
     int w = 0, h = 0;
     int32_t W[kMaxOctaves] = {}, H[kMaxOctaves] = {};
     int num_octaves = 0;
+    // describe path (ps_describe_*): the keypoints (device copy and pinned staging) and, under PS_DESCRIBE_ORIENT, the
+    // per-octave regions the orientation kernel reads, their source indices, its records in octave order and its counters;
+    // all grown on demand
+    ps_keypoint* d_kp = nullptr;  ps_keypoint* h_kp = nullptr;  size_t kp_cap = 0, h_kp_cap = 0;
+    InitialExtremum* d_kiext = nullptr;  int* d_ksrc = nullptr;  ps_extremum* d_kext = nullptr;  size_t korient_cap = 0;
+    Counters* d_kct = nullptr;
+    cudaEvent_t kp_done = nullptr;   // recorded after the host -> device copy of the keypoints
+    bool kp_pending = false;
+    bool describing = false;         // the slot's last submission was a describe call (regrow_slot re-runs its tail)
+    int  describe_n = 0, describe_flags = 0;
 };
 
 } // namespace
@@ -386,6 +396,8 @@ static int run_tail(ps_ctx* ctx, Slot& s, bool tm)
     return PS_OK;
 }
 
+static int run_describe_tail(ps_ctx* ctx, Slot& s, bool tm);
+
 // More extrema or descriptors than the slot's buffers hold: grow them and run the tail of the pipeline again on the
 // planes and initial extrema that are still in the slot (reference: Pyramid::reallocExtrema, sift_pyramid.cu:179-209,
 // called from the orientation / descriptor stages).  Rare: the buffers start at 2 x max_extrema records.
@@ -420,7 +432,7 @@ static int regrow_slot(ps_ctx* ctx, Slot& s)
         reset.ext_total = reset.ori_total = reset.ori_needed = reset.overflow = reset.work_ori = reset.work_desc = 0;
         PS_CUDA(ctx, cudaMemcpyAsync(s.d_ct, &reset, sizeof(Counters), cudaMemcpyHostToDevice, s.stream));
         PS_CUDA(ctx, cudaStreamSynchronize(s.stream));          // `reset` lives on this stack frame
-        int rc = run_tail(ctx, s, false);
+        int rc = s.describing ? run_describe_tail(ctx, s, false) : run_tail(ctx, s, false);
         if (rc != PS_OK) return rc;
         PS_CUDA(ctx, cudaEventRecord(s.done, s.stream));
         PS_CUDA(ctx, cudaEventSynchronize(s.done));
@@ -505,6 +517,7 @@ static int submit_common(ps_ctx* ctx, Slot& s)
     }
     PS_CUDA(ctx, cudaEventRecord(s.done, s.stream));
     s.submitted = true;
+    s.describing = false;
     return PS_OK;
 }
 
@@ -530,6 +543,8 @@ extern "C" void ps_destroy(ps_ctx* ctx)
         cudaFree(s.d_img); cudaFreeHost(s.h_img); cudaFree(s.d_planes); cudaFree(s.d_interm); cudaFree(s.d_iext); cudaFree(s.d_iext_f); cudaFree(s.d_keep); cudaFree(s.d_plan); cudaFree(s.d_ext); cudaFree(s.d_ori_slice);
         cudaFree(s.d_feat); cudaFree(s.d_desc); cudaFree(s.d_f2e); cudaFree(s.d_ct); cudaFreeHost(s.h_ct);
         cudaFreeHost(s.h_feat); cudaFreeHost(s.h_desc);
+        cudaFree(s.d_kp); cudaFreeHost(s.h_kp); cudaFree(s.d_kiext); cudaFree(s.d_ksrc); cudaFree(s.d_kext); cudaFree(s.d_kct);
+        if (s.kp_done) cudaEventDestroy(s.kp_done);
         for (auto& e : s.ev) if (e) cudaEventDestroy(e);
         if (s.done) cudaEventDestroy(s.done);
         if (s.graph_exec) cudaGraphExecDestroy(s.graph_exec);
@@ -661,12 +676,14 @@ extern "C" ps_ctx* ps_create(int device, const ps_config* cfg, int max_w, int ma
         for (auto& ev : s.ev) PS_TRY(cudaEventCreate(&ev));
         PS_TRY(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
         PS_TRY(cudaEventCreateWithFlags(&s.in_done, cudaEventDisableTiming));
+        PS_TRY(cudaEventCreateWithFlags(&s.kp_done, cudaEventDisableTiming));
 #undef PS_TRY
     }
     return ctx;
 }
 
 static bool is_pinned(const void* p);
+static int grow_pinned(ps_ctx* ctx, void** p, size_t* cap, size_t need, size_t elem);
 
 static int stage_input(ps_ctx* ctx, Slot& s, const void* host_img, size_t bytes)
 {
@@ -736,6 +753,146 @@ extern "C" int ps_submit_dev_u8(ps_ctx* ctx, int slot, const uint8_t* dev_img, s
     if (ctx->timing) PS_CUDA(ctx, cudaEventRecord(s->ev[0], s->stream));
     PS_CUDA(ctx, cudaMemcpy2DAsync(s->d_img, u8_pitch(w), dev_img, pitch, (size_t)w, (size_t)h, cudaMemcpyDeviceToDevice, s->stream));
     return submit_common(ctx, *s);
+}
+
+// ---- describe path (ps_describe_*): the slot's pyramid, then orientations / descriptors at the caller's keypoints
+
+// a device buffer of at least `need` records of `elem` bytes; the contents are not kept
+static int grow_dev(ps_ctx* ctx, void** p, size_t* cap, size_t need, size_t elem)
+{
+    if (need <= *cap && *p) return PS_OK;
+    const size_t ncap = std::max<size_t>(need + need / 8, 1024);
+    cudaFree(*p);
+    *p = nullptr; *cap = 0;
+    PS_CUDA(ctx, cudaMalloc(p, ncap * elem));
+    *cap = ncap;
+    return PS_OK;
+}
+
+// everything after the pyramid of a describe call: keypoints -> ext[] in input order (GIVEN directly; ORIENT through the
+// orientation kernel on per-octave regions and back), num_ori scan, descriptors, Feature records, counters to the host.
+// Also what regrow_slot re-runs when the descriptors overflow the slot's buffers.
+static int run_describe_tail(ps_ctx* ctx, Slot& s, bool tm)
+{
+    const int n = s.describe_n;
+    const bool orient = s.describe_flags == PS_DESCRIBE_ORIENT;
+    const int stride = std::max(n, 1);                 // entries per octave region: any octave may take every keypoint
+    const Consts k = slot_consts(ctx, s);
+    const size_t slice_bytes = sizeof(int) * ((size_t)s.ext_cap / PS_ORI_SLICE + 1);
+    int m = 0;
+    PS_CUDA(ctx, cudaMemsetAsync(s.d_ct, 0, sizeof(Counters), s.stream));
+    PS_CUDA(ctx, cudaMemsetAsync(s.d_ori_slice, 0, slice_bytes, s.stream));
+    if (orient) {
+        PS_CUDA(ctx, cudaMemsetAsync(s.d_kct, 0, sizeof(Counters), s.stream));
+        m += launch_kp_ingest(s.view, k, s.d_kp, n, true, s.d_ext, s.d_kiext, s.d_ksrc, stride, s.d_ori_slice, s.d_kct, s.d_ct, s.stream);
+        Consts ko = k;
+        ko.max_extrema = stride;                       // the regions' stride, as the orientation kernel indexes them
+        m += launch_orientation_only(s.view, ko, s.d_kiext, nullptr, s.d_kext, s.d_ori_slice, s.d_kct, s.stream);
+        // the orientation kernel summed num_ori in octave order; the scan needs the sums in input order
+        PS_CUDA(ctx, cudaMemsetAsync(s.d_ori_slice, 0, slice_bytes, s.stream));
+        m += launch_kp_restore(s.num_octaves, s.d_kext, s.d_ksrc, stride, n, s.d_ext, s.d_ori_slice, s.d_kct, s.stream);
+    } else {
+        m += launch_kp_ingest(s.view, k, s.d_kp, n, false, s.d_ext, nullptr, nullptr, stride, s.d_ori_slice, nullptr, s.d_ct, s.stream);
+    }
+    Consts ks = k;
+    ks.max_extrema = stride;                           // ct->ext_ct[0] = n: the scan covers ext[0, n)
+    m += launch_ori_scatter(s.num_octaves, ks, s.d_ext, s.d_f2e, s.d_ori_slice, s.d_ct, s.stream);
+    if (tm) PS_CUDA(ctx, cudaEventRecord(s.ev[4], s.stream));
+    if (ctx->cfg.desc_mode == PS_DESC_LOOP) m += launch_descriptors(s.view, k, s.d_ext, s.d_f2e, s.d_desc, s.d_ct, s.stream);
+    else m += launch_descriptors_mode(ctx->cfg.desc_mode, s.view, k, s.d_ext, s.d_f2e, s.d_desc, s.d_ct, s.stream);
+    m += launch_prep_features(k, s.d_ext, s.d_feat, s.d_ct, s.stream);
+    m += launch_kp_finish(s.d_kp, n, s.d_feat, s.stream);
+    if (tm) PS_CUDA(ctx, cudaEventRecord(s.ev[5], s.stream));
+    ctx->launches += m;
+    PS_CUDA(ctx, cudaGetLastError());
+    PS_CUDA(ctx, cudaMemcpyAsync(s.h_ct, s.d_ct, sizeof(Counters), cudaMemcpyDeviceToHost, s.stream));
+    return PS_OK;
+}
+
+static int describe_common(ps_ctx* ctx, int slot, const void* host_img, int w, int h, bool is_float, const ps_keypoint* kps,
+                           int n, int flags, const char* name)
+{
+    Slot* s = get_slot(ctx, slot);
+    if (!s || !host_img || n < 0 || (n > 0 && !kps) || (flags != PS_DESCRIBE_GIVEN && flags != PS_DESCRIBE_ORIENT))
+        return ctx ? ctx->fail(PS_ERR_ARG, "%s: bad argument", name) : PS_ERR_ARG;
+    if (w < 1 || h < 1 || w > ctx->max_w || h > ctx->max_h)
+        return ctx->fail(PS_ERR_TOO_LARGE, "image %dx%d exceeds context maximum %dx%d", w, h, ctx->max_w, ctx->max_h);
+    PS_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc = build_view(ctx, *s, w, h);
+    if (rc != PS_OK) return rc;
+    s->is_float = is_float;
+    const bool orient = flags == PS_DESCRIBE_ORIENT;
+    // n is known here, so the slot's record buffers grow before the launch (only ORIENT's descriptors, up to 4 per
+    // keypoint, may still overflow: regrow_slot).  The slot's previous work may still read the old buffers.
+    const bool grow_ext = (size_t)n > (size_t)s->ext_cap, grow_desc = n > s->desc_cap;
+    const bool grow_kp = (size_t)n > s->kp_cap || !s->d_kp || (orient && ((size_t)n > s->korient_cap || !s->d_kct));
+    if (grow_ext || grow_desc || grow_kp) PS_CUDA(ctx, cudaStreamSynchronize(s->stream));
+    if (grow_ext) {
+        const int cap = (int)std::min<long long>((long long)n + n / 8 + 1024, 0x7ffffff0);
+        cudaFree(s->d_ext); cudaFree(s->d_feat); cudaFree(s->d_ori_slice);
+        s->d_ext = nullptr; s->d_feat = nullptr; s->d_ori_slice = nullptr; s->ext_cap = 0;
+        PS_CUDA(ctx, cudaMalloc(&s->d_ext, sizeof(ps_extremum) * (size_t)cap));
+        PS_CUDA(ctx, cudaMalloc(&s->d_feat, sizeof(ps_feature) * (size_t)cap));
+        PS_CUDA(ctx, cudaMalloc(&s->d_ori_slice, sizeof(int) * ((size_t)cap / PS_ORI_SLICE + 1)));
+        s->ext_cap = cap;
+    }
+    if (grow_desc) {
+        const int cap = (int)std::min<long long>((long long)n + n / 8 + 1024, 0x3ffffff0);
+        cudaFree(s->d_desc); cudaFree(s->d_f2e);
+        s->d_desc = nullptr; s->d_f2e = nullptr; s->desc_cap = 0;
+        PS_CUDA(ctx, cudaMalloc(&s->d_desc, sizeof(ps_descriptor) * (size_t)cap));
+        PS_CUDA(ctx, cudaMalloc(&s->d_f2e, sizeof(int) * (size_t)cap));
+        s->desc_cap = cap;
+    }
+    if (grow_ext || grow_desc) s->graph_ok = false;      // the captured graph holds the old buffer addresses
+    if ((rc = grow_dev(ctx, (void**)&s->d_kp, &s->kp_cap, (size_t)n, sizeof(ps_keypoint))) != PS_OK) return rc;
+    if (orient && ((size_t)n > s->korient_cap || !s->d_kct)) {
+        // one region of up to korient_cap keypoints per octave, and the orientation kernel's records in octave order
+        const size_t cap = std::max<size_t>((size_t)n + (size_t)n / 8, 1024), regions = cap * (size_t)ctx->max_octaves;
+        cudaFree(s->d_kext); cudaFree(s->d_kiext); cudaFree(s->d_ksrc); cudaFree(s->d_kct);
+        s->d_kext = nullptr; s->d_kiext = nullptr; s->d_ksrc = nullptr; s->d_kct = nullptr; s->korient_cap = 0;
+        PS_CUDA(ctx, cudaMalloc(&s->d_kext, sizeof(ps_extremum) * cap));
+        PS_CUDA(ctx, cudaMalloc(&s->d_kiext, sizeof(InitialExtremum) * regions));
+        PS_CUDA(ctx, cudaMalloc(&s->d_ksrc, sizeof(int) * regions));
+        PS_CUDA(ctx, cudaMalloc(&s->d_kct, sizeof(Counters)));
+        s->korient_cap = cap;
+    }
+    if (ctx->timing) PS_CUDA(ctx, cudaEventRecord(s->ev[0], s->stream));
+    // the keypoints go through the slot's pinned staging, free again once the previous call's copy has left it
+    if (n > 0) {
+        if (s->kp_pending) PS_CUDA(ctx, cudaEventSynchronize(s->kp_done));
+        if ((rc = grow_pinned(ctx, (void**)&s->h_kp, &s->h_kp_cap, (size_t)n, sizeof(ps_keypoint))) != PS_OK) return rc;
+        std::memcpy(s->h_kp, kps, sizeof(ps_keypoint) * (size_t)n);
+        PS_CUDA(ctx, cudaMemcpyAsync(s->d_kp, s->h_kp, sizeof(ps_keypoint) * (size_t)n, cudaMemcpyHostToDevice, s->stream));
+        PS_CUDA(ctx, cudaEventRecord(s->kp_done, s->stream));
+        s->kp_pending = true;
+    }
+    if ((rc = stage_input(ctx, *s, host_img, (size_t)w * h * (is_float ? sizeof(float) : 1))) != PS_OK) return rc;
+    PS_CUDA(ctx, cudaMemsetAsync(s->cand_cnt, 0, s->cand_cnt_bytes, s->stream));
+    const bool tm = ctx->timing;
+    if (tm) PS_CUDA(ctx, cudaEventRecord(s->ev[1], s->stream));
+    if ((rc = run_pyramid(ctx, *s)) != PS_OK) return rc;
+    if (tm) {
+        PS_CUDA(ctx, cudaEventRecord(s->ev[2], s->stream));
+        PS_CUDA(ctx, cudaEventRecord(s->ev[3], s->stream));          // no extrema stage
+    }
+    s->describe_n = n;
+    s->describe_flags = flags;
+    s->describing = true;
+    if ((rc = run_describe_tail(ctx, *s, tm)) != PS_OK) return rc;
+    PS_CUDA(ctx, cudaEventRecord(s->done, s->stream));
+    s->submitted = true;
+    return PS_OK;
+}
+
+extern "C" int ps_describe_u8(ps_ctx* ctx, int slot, const uint8_t* host_img, int w, int h, const ps_keypoint* kps, int n, int flags)
+{
+    return describe_common(ctx, slot, host_img, w, h, false, kps, n, flags, "ps_describe_u8");
+}
+
+extern "C" int ps_describe_f32(ps_ctx* ctx, int slot, const float* host_img, int w, int h, const ps_keypoint* kps, int n, int flags)
+{
+    return describe_common(ctx, slot, host_img, w, h, true, kps, n, flags, "ps_describe_f32");
 }
 
 extern "C" int ps_wait_input(ps_ctx* ctx, int slot)

@@ -165,8 +165,27 @@ int launch_grid_filter(const PyramidView& pyr, const Consts& k, const FilterCfg&
 // iext_f: the grid-filtered extrema (read instead of iext when ct->filtered); may be nullptr when the filter is off
 int launch_orientation(const PyramidView& pyr, const Consts& k, const InitialExtremum* iext, const InitialExtremum* iext_f, ps_extremum* ext,
                        int* feat_to_ext, int* slice_sum, Counters* ct, cudaStream_t st);
+// the two halves of launch_orientation: the orientation kernel alone (writes ext[] in octave order and adds each record's
+// num_ori to slice_sum), and the exclusive scan of ext[].num_ori over the first ext_total records (idx_ori, feat_to_ext,
+// ext_total, ori_total, overflow flags), where ext_total comes from ct's per-octave counts like in the orientation kernel
+int launch_orientation_only(const PyramidView& pyr, const Consts& k, const InitialExtremum* iext, const InitialExtremum* iext_f, ps_extremum* ext,
+                            int* slice_sum, Counters* ct, cudaStream_t st);
+int launch_ori_scatter(int num_octaves, const Consts& k, ps_extremum* ext, int* feat_to_ext, const int* slice_sum, Counters* ct, cudaStream_t st);
 int launch_descriptors(const PyramidView& pyr, const Consts& k, const ps_extremum* ext, const int* feat_to_ext,
                        ps_descriptor* desc, Counters* ct, cudaStream_t st);
+
+// describe path (k_describe.cu): caller-supplied keypoints instead of detected extrema.
+// kp_ingest: validates keypoint i, picks its octave and level and writes its octave-local record.  orient = false: ext[i]
+// (num_ori 1, the given angle) and its num_ori into slice_sum; orient = true: the valid keypoints are appended to the
+// per-octave regions iext[o * stride ..] (count in ct_ori->ext_ct[o], source index in src[]) and only rejected ones get
+// their ext[i].  Either way ct->ext_ct[0] = n, so that launch_ori_scatter with max_extrema >= n scans ext[0, n).
+int launch_kp_ingest(const PyramidView& pyr, const Consts& k, const ps_keypoint* kp, int n, bool orient, ps_extremum* ext,
+                     InitialExtremum* iext, int* src, int stride, int* slice_sum, Counters* ct_ori, Counters* ct, cudaStream_t st);
+// the orientation kernel's records (octave order, ext_sorted) back to input order in ext, with their num_ori into slice_sum
+int launch_kp_restore(int num_octaves, const ps_extremum* ext_sorted, const int* src, int stride, int n, ps_extremum* ext,
+                      int* slice_sum, const Counters* ct_ori, cudaStream_t st);
+// Feature i gets keypoint i's own x, y and sigma bits
+int launch_kp_finish(const ps_keypoint* kp, int n, ps_feature* feat, cudaStream_t st);
 // --desc-mode grid / igrid / iloop / notile (k_desc_modes.cu; reference s_desc_grid.cu, s_desc_igrid.cu, s_desc_iloop.cu,
 // s_desc_notile.cu); PS_DESC_LOOP goes through launch_descriptors
 int launch_descriptors_mode(int mode, const PyramidView& pyr, const Consts& k, const ps_extremum* ext, const int* feat_to_ext,

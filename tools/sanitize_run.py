@@ -75,3 +75,23 @@ if only in ("all", "match-u8"):
     want = api.match_pairs_u8(sets, pairs, api.FeaturesDev.MATCH_EXACT)
     q = api.descriptors_to_u8(rng.normal(scale=100.0, size=(37, 128)).astype(np.float32))
     print("match-u8 rows differing", sum(int((g != w).any(1).sum()) for g, w in zip(got, want)), "quantised", q.shape, flush=True)
+if only in ("all", "describe"):
+    # caller-supplied keypoints (ps_describe_u8), both modes: a grid, random positions including the border and
+    # out-of-range scales, rejected keypoints, and more keypoints than the slot holds (its buffers grow)
+    img = make_frame(641, 479, 16)
+    rng = np.random.default_rng(3)
+    n = 9000
+    kp = np.zeros(n, api.KEYPOINT_DTYPE)
+    kp["x"], kp["y"] = rng.uniform(-2, 642, n), rng.uniform(-2, 480, n)
+    kp["sigma"] = np.exp(rng.uniform(np.log(0.2), np.log(400.0), n))
+    kp["ori"] = rng.uniform(-np.pi, np.pi, n)
+    kp["octave"], kp["level"] = -1, -1
+    kp["x"][:5] = np.nan
+    kp["octave"][5:10], kp["level"][10:15] = 2, 1
+    cfg = api.Config()
+    cfg._c.max_extrema = 2000
+    ps = api.PopSift(cfg, max_width=641, max_height=479, slots=1)
+    for orient in (False, True):
+        f = ps.describe(641, 479, img, kp, orientations=orient).get()
+        print("describe", "orient" if orient else "given", (f.getFeatureCount(), f.getDescriptorCount()), flush=True)
+    ps.uninit()
