@@ -131,4 +131,31 @@ std::vector<std::vector<int>> matchPairs(const std::vector<FeaturesDev*>& sets, 
 std::vector<std::vector<int>> matchPairsU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
                                            int flags = 0);
 
+/// RANSAC settings of verifyPairs (same fields and rules as ps_verify_params in popsift_b200.h).
+struct VerifyParams
+{
+    enum Model { Homography = 0, Fundamental = 1 };
+    int                model = Homography;
+    int                n_samples = 1024;    // minimal samples per pair, 1 .. 65536 (fixed; no early exit)
+    float              threshold = 4.0f;    // pixels: transfer error (H) or Sampson distance (F)
+    bool               refine = true;       // one least-squares refit on the winner's inliers
+    unsigned long long seed = 0;
+};
+
+/// The two-view model of one pair: model maps left to right in pixels (row-major; zero when none was found),
+/// inlier_rows are the left descriptor indices of the inlier correspondences, ascending.
+struct PairGeometry
+{
+    float            model[9];
+    int              n_inliers;
+    std::vector<int> inlier_rows;
+};
+
+/// Geometric verification of matched pairs on the device (an addition to the reference's interface; C ABI
+/// ps_match_correspondences + ps_verify_batch): `matches` is the output of matchPairs / matchPairsU8 on the same sets and
+/// pairs.  Correspondences are gathered from the sets' Features and reverse maps, then every pair gets one RANSAC
+/// homography or fundamental matrix.  Throws like matchPairs.
+std::vector<PairGeometry> verifyPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                      const std::vector<std::vector<int>>& matches, const VerifyParams& params = VerifyParams());
+
 } // namespace popsift

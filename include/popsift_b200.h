@@ -225,6 +225,72 @@ int ps_descriptors_to_u8(int device, const ps_descriptor* d_in, int n, uint8_t* 
  * -> s32), PS_MATCH_EXACT a CUDA-core kernel pair by pair. */
 int ps_match_u8_batch(int device, int n_sets, const uint8_t* const* d_sets, const int32_t* n_desc,
                       int n_pairs, const int32_t* pairs, int32_t* d_out, int flags);
+
+/* ---- geometric verification of matched pairs (an addition to the reference's interface): correspondences from the rows
+ * of ps_match_batch / ps_match_u8_batch, then one RANSAC homography or fundamental matrix per pair, all on the device. */
+
+/* Point correspondences of matched pairs.  Per set i < n_sets (host arrays): d_feat[i] / d_rev[i] are the Feature records
+ * and the descriptor -> feature reverse map of ps_download_dev (DEVICE, on `device`), n_desc[i] the descriptor count.  pairs
+ * and d_match are exactly what ps_match_batch / ps_match_u8_batch took and gave (both write the same row layout).  For
+ * pair p = (l, r), left descriptor row i with accept == 1 and best = b gives the correspondence
+ *     d_corr[4 k ..] = (feat_l[rev_l[i]].xpos, .ypos, feat_r[rev_r[b]].xpos, .ypos),   d_src[k] = i
+ * except that row i is dropped when an accepted row i' with i - 3 <= i' < i has rev_l[i'] == rev_l[i] and
+ * rev_r[best_i'] == rev_r[b] (the up to four orientations of one Feature matching the same point).  Pair p's
+ * correspondences keep row order and start at row sum_{q<p} n_desc[pairs[2q]] of d_corr / d_src (DEVICE, float4 / int32
+ * per row, as many rows as d_match has); their number goes to the HOST array n_corr[p].  A pair with an empty right set
+ * gives none.  Returns when the result is complete; PS_ERR_ARG for negative counts, a set index out of range, a null
+ * pointer where a count is > 0, or a pointer that is not device memory on `device`.  Empty sets and self pairs are valid. */
+int ps_match_correspondences(int device, int n_sets, const ps_feature* const* d_feat, const int32_t* const* d_rev,
+                             const int32_t* n_desc, int n_pairs, const int32_t* pairs, const int32_t* d_match,
+                             float* d_corr, int32_t* d_src, int32_t* n_corr);
+
+enum { PS_GEOM_HOMOGRAPHY = 0, PS_GEOM_FUNDAMENTAL = 1 };
+typedef struct ps_verify_params {      /* 24 bytes */
+    int32_t  model;       /* PS_GEOM_*                                                         */
+    int32_t  n_samples;   /* minimal samples per pair, 1 .. 65536 (fixed; no early exit)        */
+    float    threshold;   /* pixels, input-image units; finite and > 0                          */
+    int32_t  refine;      /* 1: one least-squares refit on the winner's inliers; 0: none        */
+    uint64_t seed;
+} ps_verify_params;
+/* test tap: when given, every hypothesis's inlier count (-1: invalid) and its model in pixels (scaled like the output
+ * model, zero when invalid); pair p's block starts at hypothesis p * k * n_samples (k below) */
+typedef struct ps_verify_taps { int32_t* d_counts; float* d_models; } ps_verify_taps;
+/* Batched RANSAC.  Pair p's correspondences are rows corr_start[p] .. corr_start[p] + n_corr[p] - 1 of d_corr (DEVICE,
+ * 4 floats per row: x_l, y_l, x_r, y_r in pixels; 16-byte aligned); corr_start, n_corr and prm are host memory.
+ *   Normalisation: c_l, c_r = the means of the left / right points, d = (sum |x_l - c_l| + sum |x_r - c_r|) / 2n,
+ *     s = sqrt(2) / d (1 when d == 0), all in double; a point becomes s (x - c) in float32.  One scale for both images, so
+ *     the transfer error and the Sampson distance scale by exactly s and the test below runs against (s t)^2.
+ *   Error and inlier test, in normalised float32 coordinates, without division:
+ *     homography (one-sided transfer error in the right image, as cv::findHomography): (u, v, w) = H x_l,
+ *       inlier when (u - x_r w)^2 + (v - y_r w)^2 < (s t)^2 w^2;
+ *     fundamental (Sampson distance of x_r^T F x_l = 0): a = F x_l, b = F^T x_r, e = x_r . a,
+ *       inlier when e^2 < (s t)^2 (a0^2 + a1^2 + b0^2 + b1^2).
+ *   Samples: sample s of pair p draws m = 4 (H) or 7 (F) distinct indices into the pair's n correspondences with
+ *       mix(z)  = z += 0x9E3779B97F4A7C15; z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9; z = (z ^ z >> 27) * 0x94D049BB133111EB;
+ *                 z ^ z >> 31                                                  (splitmix64, uint64 arithmetic)
+ *       key     = mix(seed ^ mix((uint64)p << 32 | s))
+ *       draw c  = (uint32)(((mix(key + c) >> 32) * n) >> 32),   c = 0, 1, .., 63
+ *     taking draws in order and skipping repeated indices; a sample without m distinct indices after 64 draws is invalid.
+ *   Hypotheses: h = k s + root with k = 1 (H) or 3 (F).  H: the 4-point DLT; the sample is rejected when three of its
+ *     points are collinear in either image (|(b - a) x (c - a)| < 1e-7 in normalised coordinates).  F: the 7-point method,
+ *     F = lambda F1 + (1 - lambda) F2 over the sample's null space, up to three real roots of det F = 0 in ascending
+ *     lambda; a missing root or a failed solve (null space not two-dimensional) gives an invalid hypothesis.
+ *   Selection: the hypothesis with the most inliers wins, ties to the smallest h; invalid hypotheses never win.
+ *   Refit (refine = 1, and at least 4 (H) / 8 (F) inliers): the normalised DLT (H) or the 8-point method with rank-2
+ *     enforcement (F) on the winner's inliers, the smallest eigenvector of the 9 x 9 normal matrix (double, fixed order,
+ *     Jacobi); kept when its inlier count is >= the winner's.  Not iterated.
+ *   Output: d_models[9 p ..] (DEVICE, row-major) maps left to right in pixels.  H is scaled to H22 = 1, or to Frobenius
+ *     norm 1 when |H22| < 1e-8 of that norm; F has Frobenius norm 1 and its largest-magnitude entry positive.
+ *     d_inlier_mask (DEVICE, one byte per d_corr row) is the inlier test above under the output model; d_n_inliers[p]
+ *     (DEVICE) is its sum.  n < 4 (H) / 7 (F), or no valid hypothesis: zero model, count 0, mask 0 -- not an error.
+ *   Determinism: results depend only on (seed, p, the pair's correspondences, prm); two identical calls give identical
+ *     bytes.
+ * Returns when the result is complete.  PS_ERR_ARG for an unknown model, n_samples outside [1, 65536], a threshold that is
+ * not finite and > 0, refine not 0 / 1, negative counts or starts, a null pointer where a count is > 0, or a pointer that
+ * is not device memory on `device`.  n_pairs = 0 is valid. */
+int ps_verify_batch(int device, int n_pairs, const float* d_corr, const int32_t* corr_start, const int32_t* n_corr,
+                    const ps_verify_params* prm, float* d_models, int32_t* d_n_inliers, uint8_t* d_inlier_mask,
+                    const ps_verify_taps* taps);
 /* ---- describe: orientations and descriptors at caller-supplied keypoints (an addition to the reference's interface;
  * VLFeat's vl_sift 'Frames' / 'Orientations', OpenCV's Feature2D::compute).  Used for tracking, upright SIFT, dense SIFT,
  * keypoints from another detector and re-describing stored keypoints under another desc_mode / norm_mode. */

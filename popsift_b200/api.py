@@ -55,6 +55,20 @@ EXTREMUM_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("lpos", "<i4"), ("sigma"
 KEYPOINT_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("sigma", "<f4"), ("ori", "<f4"), ("octave", "<i4"), ("level", "<i4")])
 assert FEATURE_DTYPE.itemsize == 72 and EXTREMUM_DTYPE.itemsize == 44 and KEYPOINT_DTYPE.itemsize == 24
 DESCRIBE_GIVEN, DESCRIBE_ORIENT = 0, 1
+GEOM = {"homography": 0, "fundamental": 1}
+
+
+class PsVerifyParams(C.Structure):
+    """ps_verify_params (24 bytes)"""
+    _fields_ = [("model", C.c_int32), ("n_samples", C.c_int32), ("threshold", C.c_float), ("refine", C.c_int32),
+                ("seed", C.c_uint64)]
+
+
+class PsVerifyTaps(C.Structure):
+    _fields_ = [("d_counts", C.c_void_p), ("d_models", C.c_void_p)]
+
+
+assert C.sizeof(PsVerifyParams) == 24
 
 EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps_geometry", "ps_create", "ps_destroy",
            "ps_last_error", "ps_submit_u8", "ps_submit_f32", "ps_submit_dev_u8", "ps_counts", "ps_download",
@@ -62,7 +76,7 @@ EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps
            "ps_launch_count", "ps_slot_stream", "ps_run_pyramid_only", "ps_run_level_only", "ps_host_alloc", "ps_host_free",
            "ps_download_dev", "ps_dev_alloc", "ps_dev_free", "ps_dev_to_host", "ps_wait_input", "ps_match", "ps_match_batch", "ps_pointer_device", "ps_host_to_dev",
            "ps_descriptors_to_u8", "ps_match_u8_batch", "ps_describe_u8", "ps_describe_f32",
-           "ps_debug_level0_plan", "ps_format_gauss_tables"]
+           "ps_debug_level0_plan", "ps_format_gauss_tables", "ps_match_correspondences", "ps_verify_batch"]
 
 _lib = None
 
@@ -101,6 +115,11 @@ def load_library():
     if hasattr(L, "ps_describe_u8"):
         L.ps_describe_u8.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
         L.ps_describe_f32.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
+    if hasattr(L, "ps_verify_batch"):
+        L.ps_match_correspondences.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.ps_verify_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsVerifyParams),
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsVerifyTaps)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -585,6 +604,190 @@ def match_pairs_u8(sets, pairs, flags=0, device=None) -> list:
             lib.ps_dev_free(p)
     starts = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
     return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
+
+
+class _DevBuffers:
+    """device allocations of one call, freed together"""
+
+    def __init__(self, lib):
+        self.lib, self.ptrs = lib, []
+
+    def alloc(self, nbytes: int) -> int:
+        p = self.lib.ps_dev_alloc(max(int(nbytes), 16))
+        if not p:
+            raise PopSiftError("ps_dev_alloc failed")
+        self.ptrs.append(p)
+        return p
+
+    def upload(self, a: np.ndarray) -> int:
+        a = np.ascontiguousarray(a)
+        p = self.alloc(a.nbytes)
+        if a.nbytes and self.lib.ps_host_to_dev(p, a.ctypes.data, a.nbytes) != 0:
+            raise PopSiftError("host -> device copy failed")
+        return p
+
+    def download(self, ptr: int, shape, dtype) -> np.ndarray:
+        out = np.zeros(shape, dtype)
+        if out.nbytes and self.lib.ps_dev_to_host(out.ctypes.data, ptr, out.nbytes) != 0:
+            raise PopSiftError("device -> host copy failed")
+        return out
+
+    def free(self):
+        while self.ptrs:
+            self.lib.ps_dev_free(self.ptrs.pop())
+
+
+def _first_device(lib, sets) -> int:
+    for s in sets:
+        if isinstance(s, FeaturesDev) and s.getDescriptorCount() > 0:
+            return max(0, lib.ps_pointer_device(s.getDescriptors()))
+    return 0
+
+
+def _verify_params(model="homography", threshold=4.0, n_samples=1024, seed=0, refine=True) -> PsVerifyParams:
+    if isinstance(model, str):
+        if model not in GEOM:
+            raise PopSiftError("model must be one of %s" % ", ".join(GEOM))
+        model = GEOM[model]
+    return PsVerifyParams(int(model), int(n_samples), float(threshold), 1 if refine else 0, int(seed) & ((1 << 64) - 1))
+
+
+def _correspondences_dev(lib, bufs, sets, pairs, d_match, device):
+    """ps_match_correspondences on device-resident match rows: (d_corr, d_src, start, n_corr)"""
+    for s in sets:
+        if not isinstance(s, FeaturesDev):
+            raise PopSiftError("correspondences need FeaturesDev sets (Config.MatchingMode)")
+    counts = [s.getDescriptorCount() for s in sets]
+    start = np.concatenate([[0], np.cumsum([counts[l] for l, _ in pairs])]).astype(np.int32)
+    rows = int(start[-1])
+    d_corr, d_src = bufs.alloc(rows * 16), bufs.alloc(rows * 4)
+    n_corr = np.zeros(max(len(pairs), 1), np.int32)
+    c_feat = (C.c_void_p * max(len(sets), 1))(*[s.getFeatures() for s in sets])
+    c_rev = (C.c_void_p * max(len(sets), 1))(*[s.getReverseMap() for s in sets])
+    c_n = (C.c_int32 * max(len(sets), 1))(*counts)
+    c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
+    rc = lib.ps_match_correspondences(device, len(sets), c_feat, c_rev, c_n, len(pairs), c_pairs, d_match, d_corr, d_src,
+                                      n_corr.ctypes.data)
+    if rc != 0:
+        raise PopSiftError("ps_match_correspondences error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+    return d_corr, d_src, start[:len(pairs)].copy(), n_corr[:len(pairs)].copy()
+
+
+def _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm: PsVerifyParams, taps=False):
+    """ps_verify_batch: host (models (P, 3, 3), counts (P,), mask (rows,) bool[, tap counts, tap models])"""
+    P = len(start)
+    rows = int(max((int(a) + int(b) for a, b in zip(start, n_corr)), default=0))
+    d_models, d_n, d_mask = bufs.alloc(P * 36), bufs.alloc(P * 4), bufs.alloc(rows)
+    k = 1 if prm.model == 0 else 3
+    tp = None
+    if taps:
+        nh = P * k * prm.n_samples
+        tp = PsVerifyTaps(bufs.alloc(nh * 4), bufs.alloc(nh * 36))
+    c_start = np.ascontiguousarray(start, np.int32)
+    c_n = np.ascontiguousarray(n_corr, np.int32)
+    rc = lib.ps_verify_batch(device, P, d_corr, c_start.ctypes.data, c_n.ctypes.data, C.byref(prm), d_models, d_n, d_mask,
+                             C.byref(tp) if tp is not None else None)
+    if rc != 0:
+        raise PopSiftError("ps_verify_batch error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+    out = [bufs.download(d_models, (P, 3, 3), np.float32), bufs.download(d_n, P, np.int32),
+           bufs.download(d_mask, rows, np.uint8).astype(bool)]
+    if taps:
+        nh = k * prm.n_samples
+        out += [bufs.download(tp.d_counts, (P, nh), np.int32), bufs.download(tp.d_models, (P, nh, 3, 3), np.float32)]
+    return out
+
+
+def match_correspondences(sets, pairs, matches, device=None):
+    """Point correspondences of matched pairs (C ABI ps_match_correspondences; an addition to the reference's interface).
+    `sets` are FeaturesDev objects (Config.MatchingMode), `pairs` the (left, right) list and `matches` the per-pair (n_left, 3)
+    rows that match_pairs / match_pairs_u8 gave for them.  Returns (corrs, src): per pair an (n, 4) float32 array of
+    x_l, y_l, x_r, y_r in pixels and the (n,) int32 left descriptor rows they came from."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    if len(matches) != len(pairs):
+        raise PopSiftError("one match array per pair expected")
+    bufs = _DevBuffers(lib)
+    try:
+        device = _first_device(lib, sets) if device is None else device
+        m = np.concatenate([np.asarray(r, np.int32).reshape(-1, 3) for r in matches]) if matches else np.zeros((0, 3), np.int32)
+        d_corr, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, bufs.upload(m), device)
+        rows = len(m)
+        corr = bufs.download(d_corr, (rows, 4), np.float32)
+        src = bufs.download(d_src, rows, np.int32)
+    finally:
+        bufs.free()
+    return ([corr[a:a + n].copy() for a, n in zip(start, n_corr)], [src[a:a + n].copy() for a, n in zip(start, n_corr)])
+
+
+def verify_correspondences(corrs, model="homography", threshold=4.0, n_samples=1024, seed=0, refine=True, taps=False, device=0):
+    """Batched RANSAC on host correspondences (C ABI ps_verify_batch): `corrs` is a list of (n, 4) arrays x_l, y_l, x_r, y_r in
+    pixels.  Returns per pair (model (3, 3) float32 mapping left to right, inlier count, (n,) bool inlier mask); with
+    taps=True also (counts, models): every hypothesis's inlier count (P, k * n_samples; -1 invalid) and pixel model
+    (P, k * n_samples, 3, 3), k = 1 for a homography and 3 for a fundamental matrix."""
+    lib = load_library()
+    prm = _verify_params(model, threshold, n_samples, seed, refine)
+    arrs = [np.ascontiguousarray(c, np.float32).reshape(-1, 4) for c in corrs]
+    n_corr = np.array([len(a) for a in arrs], np.int32)
+    start = np.concatenate([[0], np.cumsum(n_corr)])[:len(arrs)].astype(np.int32)
+    bufs = _DevBuffers(lib)
+    try:
+        allc = np.concatenate(arrs) if arrs else np.zeros((0, 4), np.float32)
+        out = _verify_dev(lib, bufs, device, bufs.upload(allc), start, n_corr, prm, taps)
+    finally:
+        bufs.free()
+    models, counts, mask = out[:3]
+    res = [(models[p], int(counts[p]), mask[start[p]:start[p] + n_corr[p]]) for p in range(len(arrs))]
+    return (res, (out[3], out[4])) if taps else res
+
+
+def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, **params):
+    """Verified matches and a two-view model per pair without leaving the device: match_pairs (or match_pairs_u8 with
+    u8=True) when `matches` is None, then ps_match_correspondences and ps_verify_batch.  `sets` are FeaturesDev objects;
+    params are verify_correspondences' (model, threshold, n_samples, seed, refine).  Returns per pair (model (3, 3) float32
+    in pixels, inlier count, int32 array of the inliers' left descriptor rows)."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    prm = _verify_params(**params)
+    counts = [s.getDescriptorCount() for s in sets]
+    for l, r in pairs:
+        if not (0 <= l < len(sets) and 0 <= r < len(sets)):
+            raise PopSiftError("set index out of range")
+    rows = sum(counts[l] for l, _ in pairs)
+    bufs = _DevBuffers(lib)
+    try:
+        device = _first_device(lib, sets) if device is None else device
+        if matches is not None:
+            if len(matches) != len(pairs):
+                raise PopSiftError("one match array per pair expected")
+            m = np.concatenate([np.asarray(r, np.int32).reshape(-1, 3) for r in matches]) if matches else np.zeros((0, 3), np.int32)
+            d_match = bufs.upload(m)
+        else:
+            d_match = bufs.alloc(rows * 12)
+            c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
+            c_n = (C.c_int32 * max(len(sets), 1))(*counts)
+            if u8:
+                q = []
+                for s in sets:
+                    p = _to_u8_dev(lib, s.getDescriptors(), s.getDescriptorCount(), device)
+                    bufs.ptrs.append(p)
+                    q.append(p)
+                c_sets = (C.c_void_p * max(len(sets), 1))(*q)
+                rc = lib.ps_match_u8_batch(device, len(sets), c_sets, c_n, len(pairs), c_pairs, d_match, flags)
+            else:
+                c_sets = (C.c_void_p * max(len(sets), 1))(*[s.getDescriptors() for s in sets])
+                rc = lib.ps_match_batch(device, len(sets), c_sets, c_n, len(pairs), c_pairs, d_match, flags)
+            if rc != 0:
+                raise PopSiftError("matching error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        d_corr, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_match, device)
+        models, n_in, mask = _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm)
+        src = bufs.download(d_src, rows, np.int32)
+    finally:
+        bufs.free()
+    out = []
+    for p in range(len(pairs)):
+        a, n = int(start[p]), int(n_corr[p])
+        out.append((models[p], int(n_in[p]), src[a:a + n][mask[a:a + n]].copy()))
+    return out
 
 
 def keypoints_array(keypoints) -> np.ndarray:

@@ -26,7 +26,7 @@ NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "--fmad=false",   # no implicit contraction anywhere; every fma in the kernels is explicit
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu",
+LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu",
                "host/sift_conf.cpp", "host/features.cpp", "host/popsift.cpp", "host/device_prop.cpp", "host/log_dump.cpp"]
 DEMO_SOURCES = ["app/popsift_demo.cpp", "app/pgmread.cpp"]
 MATCH_SOURCES = ["app/popsift_match.cpp"]            # + app/pgmread.cpp
@@ -49,6 +49,10 @@ MATCH_U8_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "match_u8_check.cpp")
 PGM_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "pgmread_check.cpp")
 DESCRIBE_CHECK = os.path.join(BIN_DIR, "describe_check")
 DESCRIBE_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "describe_check.cpp")
+VERIFY_SAMPLE_CHECK = os.path.join(BIN_DIR, "verify_sample_check")
+VERIFY_SAMPLE_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "verify_sample_check.cpp")
+VERIFY_CHECK = os.path.join(BIN_DIR, "verify_check")
+VERIFY_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "verify_check.cpp")
 
 
 def _newer(target: str, deps) -> bool:
@@ -136,6 +140,14 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if os.path.exists(DESCRIBE_CHECK_SRC) and (force or _newer(DESCRIBE_CHECK, [DESCRIBE_CHECK_SRC, LIB] + hdrs)):
         # PopSift::describe round trip with describe and enqueue jobs in one FIFO, through the C++ API
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), DESCRIBE_CHECK_SRC, "-o", DESCRIBE_CHECK,
+                               "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
+    sample_hdr = os.path.join(CSRC, "k_verify_sample.h")
+    if os.path.exists(VERIFY_SAMPLE_CHECK_SRC) and (force or _newer(VERIFY_SAMPLE_CHECK, [VERIFY_SAMPLE_CHECK_SRC, sample_hdr])):
+        # host-only: the RANSAC sample hash, the same __host__ __device__ function the kernel uses (no CUDA, no library)
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + CSRC, VERIFY_SAMPLE_CHECK_SRC, "-o", VERIFY_SAMPLE_CHECK])
+    if os.path.exists(VERIFY_CHECK_SRC) and (force or _newer(VERIFY_CHECK, [VERIFY_CHECK_SRC, LIB] + hdrs)):
+        # popsift::verifyPairs against the C ABI (ps_match_correspondences + ps_verify_batch), through the C++ API
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), VERIFY_CHECK_SRC, "-o", VERIFY_CHECK,
                                "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
     pgm_src = os.path.join(CSRC, "app", "pgmread.cpp")
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):

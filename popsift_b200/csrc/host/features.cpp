@@ -217,6 +217,84 @@ std::vector<std::vector<int>> matchPairsU8(const std::vector<FeaturesDev*>& sets
     return out;
 }
 
+std::vector<PairGeometry> verifyPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                      const std::vector<std::vector<int>>& matches, const VerifyParams& params)
+{
+    if (matches.size() != pairs.size()) throw std::runtime_error("popsift::verifyPairs: one match list per pair expected");
+    std::vector<const ps_feature*> d_feat(sets.size());
+    std::vector<const int32_t*> d_rev(sets.size());
+    std::vector<int32_t> n_desc(sets.size());
+    for (size_t i = 0; i < sets.size(); ++i) {
+        if (!sets[i]) throw std::runtime_error("popsift::verifyPairs: null set");
+        d_feat[i] = reinterpret_cast<const ps_feature*>(sets[i]->getFeatures());
+        d_rev[i] = sets[i]->getReverseMap();
+        n_desc[i] = std::max(sets[i]->getDescriptorCount(), 0);
+    }
+    std::vector<int32_t> flat(2 * pairs.size()), start(pairs.size()), n_corr(pairs.size(), 0);
+    size_t rows = 0;
+    for (size_t p = 0; p < pairs.size(); ++p) {
+        const int l = pairs[p].first, r = pairs[p].second;
+        if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error("popsift::verifyPairs: set index out of range");
+        if (matches[p].size() != (size_t)n_desc[l] * 3) throw std::runtime_error("popsift::verifyPairs: match rows do not fit the left set");
+        flat[2 * p] = l; flat[2 * p + 1] = r;
+        start[p] = (int32_t)rows;
+        rows += (size_t)n_desc[l];
+    }
+    std::vector<PairGeometry> out(pairs.size());
+    for (PairGeometry& g : out) { std::fill(g.model, g.model + 9, 0.0f); g.n_inliers = 0; }
+    if (pairs.empty()) return out;
+    int dev = 0;
+    for (size_t i = 0; i < sets.size(); ++i)
+        if (n_desc[i] > 0) { dev = std::max(0, ps_pointer_device(d_feat[i])); break; }
+    // device buffers: match rows, correspondences (16-byte rows), source rows, masks; models and counts per pair
+    const size_t nr = std::max<size_t>(rows, 1);
+    std::vector<void*> owned;
+    auto release = [&]() { for (void* p : owned) ps_dev_free(p); };
+    auto alloc = [&](size_t bytes) {
+        void* p = ps_dev_alloc(bytes);
+        if (!p) { release(); throw std::runtime_error("popsift::verifyPairs: failed to allocate device memory"); }
+        owned.push_back(p);
+        return p;
+    };
+    int32_t* d_match = static_cast<int32_t*>(alloc(nr * 3 * sizeof(int32_t)));
+    float* d_corr = static_cast<float*>(alloc(nr * 4 * sizeof(float)));
+    int32_t* d_src = static_cast<int32_t*>(alloc(nr * sizeof(int32_t)));
+    uint8_t* d_mask = static_cast<uint8_t*>(alloc(nr));
+    float* d_models = static_cast<float*>(alloc(pairs.size() * 9 * sizeof(float)));
+    int32_t* d_n = static_cast<int32_t*>(alloc(pairs.size() * sizeof(int32_t)));
+    int rc = PS_OK;
+    for (size_t p = 0; p < pairs.size() && rc == PS_OK; ++p)
+        if (!matches[p].empty())
+            rc = ps_host_to_dev(d_match + 3 * (size_t)start[p], matches[p].data(), matches[p].size() * sizeof(int32_t));
+    if (rc == PS_OK)
+        rc = ps_match_correspondences(dev, (int)sets.size(), d_feat.data(), d_rev.data(), n_desc.data(), (int)pairs.size(), flat.data(),
+                                      d_match, d_corr, d_src, n_corr.data());
+    ps_verify_params prm;
+    prm.model = params.model;
+    prm.n_samples = params.n_samples;
+    prm.threshold = params.threshold;
+    prm.refine = params.refine ? 1 : 0;
+    prm.seed = params.seed;
+    if (rc == PS_OK)
+        rc = ps_verify_batch(dev, (int)pairs.size(), d_corr, start.data(), n_corr.data(), &prm, d_models, d_n, d_mask, nullptr);
+    std::vector<float> models(pairs.size() * 9);
+    std::vector<int32_t> counts(pairs.size()), src(rows);
+    std::vector<uint8_t> mask(rows);
+    if (rc == PS_OK) rc = ps_dev_to_host(models.data(), d_models, models.size() * sizeof(float));
+    if (rc == PS_OK) rc = ps_dev_to_host(counts.data(), d_n, counts.size() * sizeof(int32_t));
+    if (rc == PS_OK && rows) rc = ps_dev_to_host(src.data(), d_src, rows * sizeof(int32_t));
+    if (rc == PS_OK && rows) rc = ps_dev_to_host(mask.data(), d_mask, rows);
+    release();
+    if (rc != PS_OK) throw std::runtime_error(std::string("popsift::verifyPairs failed: ") + ps_last_error(nullptr));
+    for (size_t p = 0; p < pairs.size(); ++p) {
+        std::copy(models.begin() + 9 * p, models.begin() + 9 * (p + 1), out[p].model);
+        out[p].n_inliers = counts[p];
+        for (int k = 0; k < n_corr[p]; ++k)
+            if (mask[(size_t)start[p] + k]) out[p].inlier_rows.push_back(src[(size_t)start[p] + k]);
+    }
+    return out;
+}
+
 void FeaturesHost::pin() {}
 void FeaturesHost::unpin() {}
 

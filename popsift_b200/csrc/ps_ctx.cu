@@ -1125,6 +1125,65 @@ extern "C" int ps_match_u8_batch(int device, int n_sets, const uint8_t* const* d
     return PS_OK;
 }
 
+extern "C" int ps_match_correspondences(int device, int n_sets, const ps_feature* const* d_feat, const int32_t* const* d_rev,
+                                        const int32_t* n_desc, int n_pairs, const int32_t* pairs, const int32_t* d_match,
+                                        float* d_corr, int32_t* d_src, int32_t* n_corr)
+{
+    if (n_sets < 0 || n_pairs < 0 || (n_sets > 0 && (!d_feat || !d_rev || !n_desc)) || (n_pairs > 0 && (!pairs || !n_corr))) return PS_ERR_ARG;
+    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    for (int i = 0; i < n_sets; ++i) {
+        if (n_desc[i] < 0) return PS_ERR_ARG;
+        if (n_desc[i] > 0 && (ps_pointer_device(d_feat[i]) != device || ps_pointer_device(d_rev[i]) != device)) return PS_ERR_ARG;
+    }
+    int64_t rows = 0;
+    for (int p = 0; p < n_pairs; ++p) {
+        const int l = pairs[2 * p], r = pairs[2 * p + 1];
+        if (l < 0 || l >= n_sets || r < 0 || r >= n_sets) return PS_ERR_ARG;
+        rows += n_desc[l];
+    }
+    if (rows == 0) {
+        for (int p = 0; p < n_pairs; ++p) n_corr[p] = 0;
+        return PS_OK;
+    }
+    if (rows > 0x7fffffff) return PS_ERR_ARG;
+    if (ps_pointer_device(d_match) != device || ps_pointer_device(d_corr) != device || ps_pointer_device(d_src) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    const int n = run_match_correspondences(d_feat, d_rev, n_desc, pairs, n_pairs, d_match, d_corr, d_src, n_corr, nullptr, &err);
+    if (n < 0) { g_create_error = err ? err : "ps_match_correspondences failed"; return PS_ERR_CUDA; }
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string("ps_match_correspondences: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
+}
+
+extern "C" int ps_verify_batch(int device, int n_pairs, const float* d_corr, const int32_t* corr_start, const int32_t* n_corr,
+                               const ps_verify_params* prm, float* d_models, int32_t* d_n_inliers, uint8_t* d_inlier_mask,
+                               const ps_verify_taps* taps)
+{
+    if (n_pairs < 0 || !prm) return PS_ERR_ARG;
+    if (prm->model != PS_GEOM_HOMOGRAPHY && prm->model != PS_GEOM_FUNDAMENTAL) return PS_ERR_ARG;
+    if (prm->n_samples < 1 || prm->n_samples > 65536) return PS_ERR_ARG;
+    if (!std::isfinite(prm->threshold) || !(prm->threshold > 0.0f)) return PS_ERR_ARG;
+    if (prm->refine != 0 && prm->refine != 1) return PS_ERR_ARG;
+    if (n_pairs == 0) return PS_OK;
+    if (!corr_start || !n_corr) return PS_ERR_ARG;
+    int64_t rows = 0;
+    for (int p = 0; p < n_pairs; ++p) {
+        if (corr_start[p] < 0 || n_corr[p] < 0) return PS_ERR_ARG;
+        rows = std::max<int64_t>(rows, (int64_t)corr_start[p] + n_corr[p]);
+    }
+    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (ps_pointer_device(d_models) != device || ps_pointer_device(d_n_inliers) != device) return PS_ERR_ARG;
+    if (rows > 0 && (ps_pointer_device(d_corr) != device || ps_pointer_device(d_inlier_mask) != device)) return PS_ERR_ARG;
+    if (rows > 0 && (reinterpret_cast<uintptr_t>(d_corr) & 15u)) return PS_ERR_ARG;
+    if (taps && (ps_pointer_device(taps->d_counts) != device || ps_pointer_device(taps->d_models) != device)) return PS_ERR_ARG;
+    const char* err = nullptr;
+    const int n = run_verify_batch(n_pairs, d_corr, corr_start, n_corr, *prm, d_models, d_n_inliers, d_inlier_mask, taps, nullptr, &err);
+    if (n < 0) { g_create_error = err ? err : "ps_verify_batch failed"; return PS_ERR_CUDA; }
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string("ps_verify_batch: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
+}
+
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)
 {
     if (bytes == 0) return PS_OK;

@@ -215,4 +215,13 @@ int run_descriptors_to_u8(const ps_descriptor* in, int n, uint8_t* out, cudaStre
 int run_match_u8_batch(const uint8_t* const* sets, const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs,
                        int32_t* out, int flags, cudaStream_t st, const char** err);
 
+// geometric verification (k_verify.cu), arguments already validated.  Correspondences of matched pairs: one gather launch;
+// n_corr (host) is written before the call returns.  Returns the number of kernels launched or -1 (*err set).
+int run_match_correspondences(const ps_feature* const* feat, const int32_t* const* rev, const int32_t* n_desc, const int32_t* pairs,
+                              int n_pairs, const int32_t* match, float* corr, int32_t* src, int32_t* n_corr, cudaStream_t st,
+                              const char** err);
+// batched RANSAC (normalise, solve, score, select / refit, taps); asynchronous on `st`
+int run_verify_batch(int n_pairs, const float* corr, const int32_t* corr_start, const int32_t* n_corr, const ps_verify_params& prm,
+                     float* d_models, int32_t* d_n, uint8_t* d_mask, const ps_verify_taps* taps, cudaStream_t st, const char** err);
+
 } // namespace psb

@@ -95,3 +95,20 @@ if only in ("all", "describe"):
         f = ps.describe(641, 479, img, kp, orientations=orient).get()
         print("describe", "orient" if orient else "given", (f.getFeatureCount(), f.getDescriptorCount()), flush=True)
     ps.uninit()
+if only in ("all", "verify"):
+    # geometric verification: the correspondence gather on real match rows (an empty set, self pairs), then RANSAC with both
+    # models on those and on planted batches with empty, tiny and multi-tile pairs, with taps and refits
+    frames = [make_frame(320, 240, 17), make_frame(320, 240, 17)[:, ::-1].copy(), np.zeros((240, 320), np.uint8)]
+    cfg = api.Config()
+    ps = api.PopSift(cfg, mode=api.Config.MatchingMode, max_width=320, max_height=240, slots=1)
+    sets = [ps.enqueue(320, 240, im).getDev() for im in frames]
+    pairs = [(0, 1), (1, 0), (0, 0), (2, 0), (0, 2)]
+    for model in ("homography", "fundamental"):
+        out = api.verify_pairs(sets, pairs, model=model, n_samples=100, threshold=3.0)
+        print("verify pairs", model, [o[1] for o in out], flush=True)
+    rng = np.random.default_rng(4)
+    corrs = [rng.uniform(0, 640, size=(n, 4)).astype(np.float32) for n in (0, 3, 7, 8, 50, 2500, 5000)]
+    for model in ("homography", "fundamental"):
+        res, taps = api.verify_correspondences(corrs, model=model, n_samples=200, threshold=2.0, taps=True)
+        print("verify", model, [r[1] for r in res], int((taps[0] >= 0).sum()), flush=True)
+    ps.uninit()
