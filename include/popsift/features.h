@@ -158,4 +158,14 @@ struct PairGeometry
 std::vector<PairGeometry> verifyPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
                                       const std::vector<std::vector<int>>& matches, const VerifyParams& params = VerifyParams());
 
+/// Guided matching (an addition to the reference's interface; C ABI ps_match_guided_batch in popsift_b200_guided.h): matchPairs
+/// again with only the right descriptors whose keypoints pass the pair's model as candidates.  `geometry` is what
+/// verifyPairs gave for the same sets and pairs; params.model and params.threshold select the test (the other fields are
+/// unused).  Returns what matchPairs returns and throws like it (also when geometry.size() != pairs.size()).
+std::vector<std::vector<int>> matchPairsGuided(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                               const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags = 0);
+/// matchPairsGuided on 8-bit descriptors (quantised on the device as matchPairsU8 does; C ABI ps_match_u8_guided_batch)
+std::vector<std::vector<int>> matchPairsGuidedU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                                 const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags = 0);
+
 } // namespace popsift

@@ -77,6 +77,8 @@ EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps
            "ps_download_dev", "ps_dev_alloc", "ps_dev_free", "ps_dev_to_host", "ps_wait_input", "ps_match", "ps_match_batch", "ps_pointer_device", "ps_host_to_dev",
            "ps_descriptors_to_u8", "ps_match_u8_batch", "ps_describe_u8", "ps_describe_f32",
            "ps_debug_level0_plan", "ps_format_gauss_tables", "ps_match_correspondences", "ps_verify_batch"]
+# guided matching, declared in popsift_b200_guided.h (same library)
+GUIDED_EXPORTS = ["ps_match_guided_batch", "ps_match_u8_guided_batch"]
 
 _lib = None
 
@@ -120,6 +122,10 @@ def load_library():
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.ps_verify_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsVerifyParams),
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsVerifyTaps)]
+    if hasattr(L, "ps_match_guided_batch"):
+        for name in GUIDED_EXPORTS:
+            getattr(L, name).argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                         C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_int]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -673,11 +679,13 @@ def _correspondences_dev(lib, bufs, sets, pairs, d_match, device):
     return d_corr, d_src, start[:len(pairs)].copy(), n_corr[:len(pairs)].copy()
 
 
-def _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm: PsVerifyParams, taps=False):
-    """ps_verify_batch: host (models (P, 3, 3), counts (P,), mask (rows,) bool[, tap counts, tap models])"""
+def _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm: PsVerifyParams, taps=False, d_models=None):
+    """ps_verify_batch: host (models (P, 3, 3), counts (P,), mask (rows,) bool[, tap counts, tap models]); the models are
+    written to d_models (P x 9 floats of device memory) when given"""
     P = len(start)
     rows = int(max((int(a) + int(b) for a, b in zip(start, n_corr)), default=0))
-    d_models, d_n, d_mask = bufs.alloc(P * 36), bufs.alloc(P * 4), bufs.alloc(rows)
+    d_models = bufs.alloc(P * 36) if d_models is None else d_models
+    d_n, d_mask = bufs.alloc(P * 4), bufs.alloc(rows)
     k = 1 if prm.model == 0 else 3
     tp = None
     if taps:
@@ -740,11 +748,14 @@ def verify_correspondences(corrs, model="homography", threshold=4.0, n_samples=1
     return (res, (out[3], out[4])) if taps else res
 
 
-def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, **params):
+def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, guided=False, **params):
     """Verified matches and a two-view model per pair without leaving the device: match_pairs (or match_pairs_u8 with
     u8=True) when `matches` is None, then ps_match_correspondences and ps_verify_batch.  `sets` are FeaturesDev objects;
     params are verify_correspondences' (model, threshold, n_samples, seed, refine).  Returns per pair (model (3, 3) float32
-    in pixels, inlier count, int32 array of the inliers' left descriptor rows)."""
+    in pixels, inlier count, int32 array of the inliers' left descriptor rows).
+    guided=True adds guided matching on the device-resident models at the same threshold (ps_match_guided_batch, or
+    ps_match_u8_guided_batch with u8=True) and gathers the correspondences again: per pair (model, number of guided
+    correspondences, int32 array of their left descriptor rows)."""
     lib = load_library()
     pairs = [(int(a), int(b)) for a, b in pairs]
     prm = _verify_params(**params)
@@ -756,6 +767,7 @@ def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, **pa
     bufs = _DevBuffers(lib)
     try:
         device = _first_device(lib, sets) if device is None else device
+        q = None                                   # the 8-bit copies of the sets, when matching made them
         if matches is not None:
             if len(matches) != len(pairs):
                 raise PopSiftError("one match array per pair expected")
@@ -779,6 +791,13 @@ def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, **pa
             if rc != 0:
                 raise PopSiftError("matching error %d: %s" % (rc, lib.ps_last_error(None).decode()))
         d_corr, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_match, device)
+        if guided:
+            d_models = bufs.alloc(len(pairs) * 36)
+            models, n_in, mask = _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm, d_models=d_models)
+            d_guided = _match_guided_dev(lib, bufs, sets, pairs, d_models, prm.model, prm.threshold, flags, u8, device, u8_sets=q)
+            _, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_guided, device)
+            src = bufs.download(d_src, rows, np.int32)
+            return [(models[p], int(n_corr[p]), src[int(start[p]):int(start[p]) + int(n_corr[p])].copy()) for p in range(len(pairs))]
         models, n_in, mask = _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm)
         src = bufs.download(d_src, rows, np.int32)
     finally:
@@ -788,6 +807,68 @@ def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, **pa
         a, n = int(start[p]), int(n_corr[p])
         out.append((models[p], int(n_in[p]), src[a:a + n][mask[a:a + n]].copy()))
     return out
+
+
+def _match_guided_dev(lib, bufs, sets, pairs, d_models, model, threshold, flags, u8, device, u8_sets=None) -> int:
+    """ps_match_guided_batch / ps_match_u8_guided_batch on FeaturesDev sets and device-resident models: the device rows.
+    u8_sets: the sets' 8-bit device copies when the caller already has them (u8=True)"""
+    for s in sets:
+        if not isinstance(s, FeaturesDev):
+            raise PopSiftError("guided matching needs FeaturesDev sets (Config.MatchingMode)")
+    counts = [s.getDescriptorCount() for s in sets]
+    rows = sum(counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs)
+    d_out = bufs.alloc(rows * 12)
+    if u8 and u8_sets is not None:
+        descs = list(u8_sets)
+        fn, name = lib.ps_match_u8_guided_batch, "ps_match_u8_guided_batch"
+    elif u8:
+        descs = []
+        for s in sets:
+            p = _to_u8_dev(lib, s.getDescriptors(), s.getDescriptorCount(), device)
+            bufs.ptrs.append(p)
+            descs.append(p)
+        fn, name = lib.ps_match_u8_guided_batch, "ps_match_u8_guided_batch"
+    else:
+        descs = [s.getDescriptors() for s in sets]
+        fn, name = lib.ps_match_guided_batch, "ps_match_guided_batch"
+    n = max(len(sets), 1)
+    c_sets = (C.c_void_p * n)(*descs)
+    c_feat = (C.c_void_p * n)(*[s.getFeatures() for s in sets])
+    c_rev = (C.c_void_p * n)(*[s.getReverseMap() for s in sets])
+    c_n = (C.c_int32 * n)(*counts)
+    c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
+    rc = fn(device, len(sets), c_sets, c_feat, c_rev, c_n, len(pairs), c_pairs, d_models, int(model), float(threshold), d_out, flags)
+    if rc != 0:
+        raise PopSiftError("%s error %d: %s" % (name, rc, lib.ps_last_error(None).decode()))
+    return d_out
+
+
+def match_pairs_guided(sets, pairs, models, model="homography", threshold=4.0, flags=0, u8=False, device=None) -> list:
+    """Guided matching (C ABI ps_match_guided_batch / ps_match_u8_guided_batch in popsift_b200_guided.h; an addition to the
+    reference's interface): match_pairs (match_pairs_u8 with u8=True) where the candidates of a left descriptor are only the
+    right descriptors whose keypoints pass the pair's model at `threshold` pixels.  `sets` are FeaturesDev objects
+    (Config.MatchingMode), `models` the (P, 3, 3) left-to-right pixel models (e.g. from verify_pairs), `model` "homography"
+    or "fundamental".  Entry p is the (n_left, 3) int32 array (best, second, accept); no eligible descriptor gives (0, 0, 0)."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    if isinstance(model, str):
+        if model not in GEOM:
+            raise PopSiftError("model must be one of %s" % ", ".join(GEOM))
+        model = GEOM[model]
+    m = np.ascontiguousarray(models, np.float32).reshape(-1, 9)
+    if len(m) != len(pairs):
+        raise PopSiftError("one model per pair expected")
+    counts = [s.getDescriptorCount() for s in sets]
+    rows = [counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs]
+    bufs = _DevBuffers(lib)
+    try:
+        device = _first_device(lib, sets) if device is None else device
+        d_out = _match_guided_dev(lib, bufs, sets, pairs, bufs.upload(m), model, threshold, flags, u8, device)
+        out = bufs.download(d_out, (sum(rows), 3), np.int32)
+    finally:
+        bufs.free()
+    starts = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
+    return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
 
 
 def keypoints_array(keypoints) -> np.ndarray:

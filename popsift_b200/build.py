@@ -53,6 +53,10 @@ VERIFY_SAMPLE_CHECK = os.path.join(BIN_DIR, "verify_sample_check")
 VERIFY_SAMPLE_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "verify_sample_check.cpp")
 VERIFY_CHECK = os.path.join(BIN_DIR, "verify_check")
 VERIFY_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "verify_check.cpp")
+GUIDED_MASK = os.path.join(BIN_DIR, "guided_mask")
+GUIDED_MASK_SRC = os.path.join(ROOT, "tests", "cpp", "guided_mask.cpp")
+GUIDED_CHECK = os.path.join(BIN_DIR, "guided_check")
+GUIDED_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "guided_check.cpp")
 
 
 def _newer(target: str, deps) -> bool:
@@ -148,6 +152,15 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if os.path.exists(VERIFY_CHECK_SRC) and (force or _newer(VERIFY_CHECK, [VERIFY_CHECK_SRC, LIB] + hdrs)):
         # popsift::verifyPairs against the C ABI (ps_match_correspondences + ps_verify_batch), through the C++ API
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), VERIFY_CHECK_SRC, "-o", VERIFY_CHECK,
+                               "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
+    guided_hdr = os.path.join(CSRC, "k_guided.h")
+    if os.path.exists(GUIDED_MASK_SRC) and (force or _newer(GUIDED_MASK, [GUIDED_MASK_SRC, guided_hdr])):
+        # host-only: guided matching's eligibility mask, the same __host__ __device__ function the kernels use (no CUDA, no
+        # library); no contraction, so that every rounding is the one the function spells out
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-I" + CSRC, GUIDED_MASK_SRC, "-o", GUIDED_MASK])
+    if os.path.exists(GUIDED_CHECK_SRC) and (force or _newer(GUIDED_CHECK, [GUIDED_CHECK_SRC, LIB] + hdrs)):
+        # popsift::matchPairsGuided(U8) against the C ABI (ps_match_guided_batch / ps_match_u8_guided_batch)
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), GUIDED_CHECK_SRC, "-o", GUIDED_CHECK,
                                "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
     pgm_src = os.path.join(CSRC, "app", "pgmread.cpp")
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):

@@ -4,6 +4,7 @@
 #include "popsift/features.h"
 #include "pinned_pool.h"
 #include "popsift_b200.h"
+#include "popsift_b200_guided.h"
 
 #include <algorithm>
 #include <cmath>
@@ -293,6 +294,94 @@ std::vector<PairGeometry> verifyPairs(const std::vector<FeaturesDev*>& sets, con
             if (mask[(size_t)start[p] + k]) out[p].inlier_rows.push_back(src[(size_t)start[p] + k]);
     }
     return out;
+}
+
+namespace {
+
+// matchPairsGuided / matchPairsGuidedU8: the C ABI call on the sets' descriptors (float) or their 8-bit copies
+std::vector<std::vector<int>> match_guided(const char* name, bool u8, const std::vector<FeaturesDev*>& sets,
+                                           const std::vector<std::pair<int, int>>& pairs, const std::vector<PairGeometry>& geometry,
+                                           const VerifyParams& params, int flags)
+{
+    const std::string who = std::string("popsift::") + name;
+    if (geometry.size() != pairs.size()) throw std::runtime_error(who + ": one geometry per pair expected");
+    std::vector<const ps_feature*> d_feat(sets.size());
+    std::vector<const int32_t*> d_rev(sets.size());
+    std::vector<int32_t> n_desc(sets.size());
+    for (size_t i = 0; i < sets.size(); ++i) {
+        if (!sets[i]) throw std::runtime_error(who + ": null set");
+        d_feat[i] = reinterpret_cast<const ps_feature*>(sets[i]->getFeatures());
+        d_rev[i] = sets[i]->getReverseMap();
+        n_desc[i] = std::max(sets[i]->getDescriptorCount(), 0);
+    }
+    std::vector<int32_t> flat(2 * pairs.size());
+    std::vector<std::vector<int>> out(pairs.size());
+    size_t rows = 0;
+    for (size_t p = 0; p < pairs.size(); ++p) {
+        const int l = pairs[p].first, r = pairs[p].second;
+        if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error(who + ": set index out of range");
+        flat[2 * p] = l; flat[2 * p + 1] = r;
+        out[p].assign((size_t)n_desc[l] * 3, 0);
+        rows += out[p].size() / 3;
+    }
+    if (rows == 0) return out;
+    int dev = 0;
+    for (size_t i = 0; i < sets.size(); ++i)
+        if (n_desc[i] > 0) { dev = std::max(0, ps_pointer_device(sets[i]->getDescriptors())); break; }
+    std::vector<void*> owned;
+    auto release = [&]() { for (void* p : owned) ps_dev_free(p); };
+    auto alloc = [&](size_t bytes) {
+        void* p = ps_dev_alloc(bytes);
+        if (!p) { release(); throw std::runtime_error(who + ": failed to allocate device memory"); }
+        owned.push_back(p);
+        return p;
+    };
+    std::vector<float> models(pairs.size() * 9);
+    for (size_t p = 0; p < pairs.size(); ++p) std::copy(geometry[p].model, geometry[p].model + 9, models.begin() + 9 * p);
+    float* d_models = static_cast<float*>(alloc(models.size() * sizeof(float)));
+    int32_t* d_out = static_cast<int32_t*>(alloc(rows * 3 * sizeof(int32_t)));
+    int rc = ps_host_to_dev(d_models, models.data(), models.size() * sizeof(float));
+    if (u8) {
+        // the 8-bit copies of every set (cudaMalloc: 256-byte aligned)
+        std::vector<const uint8_t*> d_sets(sets.size(), nullptr);
+        for (size_t i = 0; i < sets.size() && rc == PS_OK; ++i) {
+            if (n_desc[i] == 0) continue;
+            uint8_t* q = static_cast<uint8_t*>(alloc((size_t)n_desc[i] * 128));
+            d_sets[i] = q;
+            rc = ps_descriptors_to_u8(dev, reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors()), n_desc[i], q);
+        }
+        if (rc == PS_OK)
+            rc = ps_match_u8_guided_batch(dev, (int)sets.size(), d_sets.data(), d_feat.data(), d_rev.data(), n_desc.data(), (int)pairs.size(),
+                                          flat.data(), d_models, params.model, params.threshold, d_out, flags);
+    } else {
+        std::vector<const ps_descriptor*> d_sets(sets.size());
+        for (size_t i = 0; i < sets.size(); ++i) d_sets[i] = reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors());
+        if (rc == PS_OK)
+            rc = ps_match_guided_batch(dev, (int)sets.size(), d_sets.data(), d_feat.data(), d_rev.data(), n_desc.data(), (int)pairs.size(),
+                                       flat.data(), d_models, params.model, params.threshold, d_out, flags);
+    }
+    size_t row = 0;
+    for (size_t p = 0; p < pairs.size() && rc == PS_OK; ++p) {
+        rc = ps_dev_to_host(out[p].data(), d_out + 3 * row, out[p].size() * sizeof(int32_t));
+        row += out[p].size() / 3;
+    }
+    release();
+    if (rc != PS_OK) throw std::runtime_error(who + " failed: " + ps_last_error(nullptr));
+    return out;
+}
+
+} // namespace
+
+std::vector<std::vector<int>> matchPairsGuided(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                               const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags)
+{
+    return match_guided("matchPairsGuided", false, sets, pairs, geometry, params, flags);
+}
+
+std::vector<std::vector<int>> matchPairsGuidedU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                                 const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags)
+{
+    return match_guided("matchPairsGuidedU8", true, sets, pairs, geometry, params, flags);
 }
 
 void FeaturesHost::pin() {}

@@ -34,6 +34,7 @@
 #include "ps_internal.h"
 #include "k_match_common.h"
 #include "k_match_plan.h"
+#include "k_guided.h"
 #include "tma_util.h"
 
 #include <algorithm>
@@ -397,6 +398,232 @@ match_rerank_kernel(const RerankPair* __restrict__ pairs, int n_pairs, int64_t r
     if (lane == 0) best.store(out + 3 * (size_t)(P.out_row + row));
 }
 
+// ------------------------------------------------------------------------------------------------ guided matching
+//
+// ps_match_guided_batch (include/popsift_b200_guided.h): the same 2-NN, restricted per left row to the right descriptors
+// that pass the pair's geometric test (k_guided.h).  The EXACT kernel skips ineligible columns (the test is warp-uniform);
+// the tensor-core kernel is match_tc_kernel with the test fused into its epilogue: an ineligible element's value becomes
+// +inf before its key is packed, so that it behaves like a padding column (inf or NaN after the low bits are replaced,
+// dropped by fminf, never < t3) and never becomes a candidate.  The re-rank is match_rerank_kernel unchanged: it only
+// sees candidates, and every candidate is eligible.
+
+// launched only for pairs with a non-empty right set (the model is read unconditionally)
+template <int MODEL>
+__global__ void __launch_bounds__(128, 8)
+match_exact_guided_kernel(const ps_descriptor* __restrict__ l, const ps_feature* __restrict__ fl, const int32_t* __restrict__ revl, int nl,
+                          const ps_descriptor* __restrict__ r, const ps_feature* __restrict__ fr, const int32_t* __restrict__ revr, int nr,
+                          const float* __restrict__ model, float t2, int32_t* __restrict__ out)
+{
+    const int lane = threadIdx.x & 31;
+    const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (row >= nl) return;
+    const float4 l4 = __ldg(reinterpret_cast<const float4*>(l + row) + lane);
+    float m[9];
+    load_model(m, model);
+    const float2 p = feat_xy(fl, revl, row);
+    const GuidedRow gr = guided_row<MODEL>(m, t2, p.x, p.y);
+    Best2 b; b.init();
+    for (int i = 0; i < nr; ++i) {
+        const float2 P = feat_xy(fr, revr, i);                            // the same for every lane
+        if (!guided_ok<MODEL>(gr, guided_col<MODEL>(m, P.x, P.y), t2, P.x, P.y)) continue;
+        b.step(warp_sq_dist(l4, reinterpret_cast<const float4*>(r + i), lane), i);
+    }
+    if (lane == 0) b.store(out + 3 * (size_t)row);
+}
+
+// one thread per pooled row: its pixel position (NaN for padding rows)
+__global__ void __launch_bounds__(256)
+match_coords_kernel(const MatchCoordSet* __restrict__ sets, int n_sets, int rows, float2* __restrict__ out)
+{
+    const int row = blockIdx.x * 256 + threadIdx.x;
+    if (row >= rows) return;
+    int a = 0, b = n_sets - 1;                                    // the last set that starts at or before `row`
+    while (a < b) { const int m = (a + b + 1) >> 1; if (sets[m].row <= row) a = m; else b = m - 1; }
+    const MatchCoordSet cs = sets[a];
+    const int local = row - cs.row;
+    out[row] = local < cs.n ? feat_xy(cs.f, cs.rev, local) : make_float2(NAN, NAN);
+}
+
+// top4_row with constant bounds at every level of the min tree, so that m[] stays in registers
+template <int HALF>
+__device__ __forceinline__ void top4_row_guided(Top4& T, float (&d)[64], int nb, int q)
+{
+    float m[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) m[i] = fminf(d[4 * (i >> 1) + 2 * HALF + (i & 1)], d[4 * ((i + 16) >> 1) + 2 * HALF + (i & 1)]);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) m[i] = fminf(m[i], m[i + 8]);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) m[i] = fminf(m[i], m[i + 4]);
+    m[0] = fminf(m[0], m[2]); m[1] = fminf(m[1], m[3]);
+    float best = fminf(m[0], m[1]);
+    while (best < T.t3) {
+        const int e = (int)(__float_as_uint(best) & 31u);
+        T.insert(best, nb + 8 * (e >> 1) + 2 * q + (e & 1));
+        float nxt = INFINITY;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+            const float k = d[4 * (i >> 1) + 2 * HALF + (i & 1)];
+            nxt = (k > best) ? fminf(nxt, k) : nxt;
+        }
+        best = nxt;
+    }
+}
+
+// match_tc_kernel plus the geometric test.  coords: the group's pooled pixel positions; models: the caller's 9 floats per
+// pair; gpair: group pair -> caller pair.  A right tile's 128 positions (1 KB) come with the tile: the producer copies
+// them with cp.async.bulk into a one-stage buffer (c_full / c_empty) after the tile's last K-block, and the consumers
+// release it when their epilogue has read it.  One stage is what fits next to the 225 KB of operand tiles, and it is
+// enough: the copy for tile j + 1 is issued while the consumers run tile j + 1's MMAs.
+template <int MODEL>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+match_tc_guided_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
+                       const float* __restrict__ norm, const float2* __restrict__ coords, const float* __restrict__ models,
+                       const int32_t* __restrict__ gpair, float t2, const MatchItem* __restrict__ items, int n_items,
+                       int32_t* __restrict__ cand)
+{
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t a_full, a_empty, b_full[STAGES], b_empty[STAGES], c_full, c_empty;
+    __shared__ __align__(128) float2 cpos[BN];
+    uint8_t* smem = smem_raw + ((1024u - (s32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* A_hi = smem;
+    uint8_t* A_lo = smem + NKB * TILE_BYTES;
+    uint8_t* B_st = smem + 2 * NKB * TILE_BYTES;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+    if (threadIdx.x == 0) {
+        mb_init(&a_full, 1);
+        mb_init(&a_empty, 8);
+        for (int s = 0; s < STAGES; ++s) { mb_init(&b_full[s], 1); mb_init(&b_empty[s], 8); }
+        mb_init(&c_full, 1);
+        mb_init(&c_empty, 8);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        // ===== TMA producer (one thread) =====
+        if (threadIdx.x == 0) {
+            int s = 0; unsigned ph = 0, cph = 0;
+            int a_cur = -1; unsigned a_ph = 0;
+            for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+                const MatchItem w = items[it];
+                if (w.a_row != a_cur) {
+                    if (a_cur >= 0) { mb_wait(&a_empty, a_ph); a_ph ^= 1u; }
+                    a_cur = w.a_row;
+                    mb_expect(&a_full, 2 * NKB * TILE_BYTES);
+                    for (int kb = 0; kb < NKB; ++kb) {
+                        tma_tile(A_hi + kb * TILE_BYTES, &tm_hi, kb * KB, w.a_row, &a_full);
+                        tma_tile(A_lo + kb * TILE_BYTES, &tm_lo, kb * KB, w.a_row, &a_full);
+                    }
+                }
+                for (int j = 0; j < w.b_tiles; ++j) {
+                    for (int kb = 0; kb < NKB; ++kb) {
+                        mb_wait(&b_empty[s], ph ^ 1u);
+                        mb_expect(&b_full[s], 2 * TILE_BYTES);
+                        tma_tile(B_st + (s * 2 + 0) * TILE_BYTES, &tm_hi, kb * KB, w.b_row + j * BN, &b_full[s]);
+                        tma_tile(B_st + (s * 2 + 1) * TILE_BYTES, &tm_lo, kb * KB, w.b_row + j * BN, &b_full[s]);
+                        if (++s == STAGES) { s = 0; ph ^= 1u; }
+                    }
+                    mb_wait(&c_empty, cph ^ 1u);                     // the epilogue of the previous tile has read it
+                    mb_expect(&c_full, BN * sizeof(float2));
+                    bulk_copy(cpos, coords + w.b_row + j * BN, BN * sizeof(float2), &c_full);
+                    cph ^= 1u;
+                }
+            }
+        }
+        return;
+    }
+    // ===== consumers: warpgroup c owns rows 64c .. 64c+63 of each item's 128 =====
+    const int c = (warp >> 2) - 1;
+    const int q = lane & 3;
+    const int r0 = 64 * c + 16 * (warp & 3) + (lane >> 2);
+    const unsigned a_off = (unsigned)(64 * c * 128);
+    float d[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) d[i] = 0.0f;
+    int s = 0; unsigned ph = 0, cph = 0;
+    int a_cur = -1; unsigned a_ph = 0;
+    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+        const MatchItem w = items[it];
+        if (w.a_row != a_cur) { mb_wait(&a_full, a_ph); a_ph ^= 1u; a_cur = w.a_row; }
+        const float* __restrict__ rnorm = norm + w.b_row;
+        // the pair's model, and the per-row part of the test for the thread's two left rows (NaN rows: nothing eligible)
+        float m[9];
+        load_model(m, models + 9 * (size_t)__ldg(gpair + w.pair));
+        const float2 p0 = __ldg(coords + w.a_row + r0), p1 = __ldg(coords + w.a_row + r0 + 8);
+        const GuidedRow g0 = guided_row<MODEL>(m, t2, p0.x, p0.y), g1 = guided_row<MODEL>(m, t2, p1.x, p1.y);
+        Top4 T0, T1;
+        for (int j = 0; j < w.b_tiles; ++j) {
+            const int nb0 = j * BN;
+            float2 rn[16];
+#pragma unroll
+            for (int b = 0; b < 16; ++b) rn[b] = __ldg(reinterpret_cast<const float2*>(rnorm + nb0 + 8 * b + 2 * q));
+            int prev = -1;
+            for (int kb = 0; kb < NKB; ++kb) {
+                mb_wait(&b_full[s], ph);
+                wg_fence();
+                const uint64_t a_hi = gmma_desc(A_hi + kb * TILE_BYTES + a_off), a_lo = gmma_desc(A_lo + kb * TILE_BYTES + a_off);
+                const uint64_t b_hi = gmma_desc(B_st + (s * 2 + 0) * TILE_BYTES), b_lo = gmma_desc(B_st + (s * 2 + 1) * TILE_BYTES);
+#pragma unroll
+                for (int k8 = 0; k8 < KB / MMA_K; ++k8) {
+                    const uint64_t adv = (uint64_t)(k8 * MMA_K * 4 / 16);
+                    wgmma_tf32(d, a_hi + adv, b_hi + adv, (kb | k8) != 0);
+                    wgmma_tf32(d, a_hi + adv, b_lo + adv, 1);
+                    wgmma_tf32(d, a_lo + adv, b_hi + adv, 1);
+                }
+                wg_commit();
+                if (prev >= 0) {
+                    wg_wait<1>();
+                    __syncwarp();
+                    if (lane == 0) mb_arrive(&b_empty[prev]);
+                }
+                prev = s;
+                if (++s == STAGES) { s = 0; ph ^= 1u; }
+            }
+            wg_wait<0>();
+            __syncwarp();
+            if (lane == 0) mb_arrive(&b_empty[prev]);
+            mb_wait(&c_full, cph);
+            cph ^= 1u;
+            // keys as in match_tc_kernel; an ineligible element is +inf before packing.  Columns 8b + 2q and 8b + 2q + 1
+            // are one float4 of the position buffer; the per-column part of the test serves both rows.
+#pragma unroll
+            for (int b = 0; b < 16; ++b) {
+                const float4 xy = reinterpret_cast<const float4*>(cpos)[4 * b + q];
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                    const float X = u ? xy.z : xy.x, Y = u ? xy.w : xy.y;
+                    const float cb = guided_col<MODEL>(m, X, Y);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int i = 4 * b + 2 * h + u;
+                        const bool ok = guided_ok<MODEL>(h ? g1 : g0, cb, t2, X, Y);
+                        const float val = ok ? fmaf(-2.0f, d[i], u ? rn[b].y : rn[b].x) : INFINITY;
+                        d[i] = __uint_as_float((__float_as_uint(val) & 0xffffffe0u) | (unsigned)(2 * b + u));
+                    }
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mb_arrive(&c_empty);
+            top4_row_guided<0>(T0, d, w.b_col0 + nb0, q);
+            top4_row_guided<1>(T1, d, w.b_col0 + nb0, q);
+        }
+        T0.merge_xor(1); T1.merge_xor(1);
+        T0.merge_xor(2); T1.merge_xor(2);
+        if (q == 0) {
+            int32_t* cw = cand + (size_t)(w.cand + (int64_t)r0 * w.stride) * kCand;
+            if (w.l_row0 + r0 < w.nl) *reinterpret_cast<int4*>(cw) = make_int4(T0.i0, T0.i1, T0.i2, T0.i3);
+            if (w.l_row0 + r0 + 8 < w.nl) *reinterpret_cast<int4*>(cw + (size_t)8 * w.stride * kCand) = make_int4(T1.i0, T1.i1, T1.i2, T1.i3);
+        }
+        const int nx = it + gridDim.x;
+        if (nx < n_items && items[nx].a_row != a_cur) {
+            __syncwarp();
+            if (lane == 0) mb_arrive(&a_empty);
+        }
+    }
+}
+
 } // namespace
 
 // POPSIFT_B200_MATCH=exact|tc overrides the automatic choice (A/B switch, cross-check)
@@ -470,34 +697,58 @@ size_t match_workspace_cap()
     return cap;
 }
 
-int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs,
-                    int32_t* out, int flags, cudaStream_t st, const char** err)
+namespace {
+
+constexpr int kUnguided = -1;
+
+// The host side of the batched matcher: plan, metadata upload, workspace, launches.  MODE = kUnguided: ps_match_batch;
+// MODE = kGuidedH / kGuidedF: ps_match_guided_batch, which also uses feat, rev, models and t2, and whose pooled rows carry
+// the row's pixel position (8 more bytes per row).  Arguments already validated, flags already resolved.
+template <int MODE>
+int run_batch(const ps_descriptor* const* sets, const ps_feature* const* feat, const int32_t* const* rev, const int32_t* n_desc,
+              int n_sets, const int32_t* pairs, int n_pairs, const float* models, float t2, int32_t* out, int flags,
+              cudaStream_t st, const char** err)
 {
-    *err = nullptr;
-    if (n_pairs <= 0) return 0;
-    flags = match_choice(flags);
-    const MatchPlan plan = plan_match(n_sets, n_desc, n_pairs, pairs, sm_count(), match_workspace_cap());
+    constexpr bool guided = MODE != kUnguided;
+    constexpr size_t row_bytes = guided ? kMatchGuidedRowBytes : kMatchRowBytes;
+    const MatchPlan plan = plan_match(n_sets, n_desc, n_pairs, pairs, sm_count(), match_workspace_cap(), row_bytes);
     int launches = 0;
     if (flags == PS_MATCH_EXACT) {
         // the CUDA-core kernel, pair by pair: the in-library reference
         for (int p = 0; p < n_pairs; ++p) {
             const int l = pairs[2 * p], r = pairs[2 * p + 1];
             if (n_desc[l] <= 0) continue;
-            match_exact_kernel<<<(n_desc[l] + 3) / 4, 128, 0, st>>>(sets[l], n_desc[l], sets[r], n_desc[r], out + 3 * (size_t)plan.out_row[p]);
+            int32_t* o = out + 3 * (size_t)plan.out_row[p];
+            if constexpr (guided) {
+                // an empty right set gives rows (0, 0, 0), and the pair's model need not exist: it is not read
+                if (n_desc[r] <= 0) {
+                    if (cudaMemsetAsync(o, 0, (size_t)n_desc[l] * 3 * sizeof(int32_t), st) != cudaSuccess) {
+                        cudaGetLastError(); *err = "guided matcher: cudaMemsetAsync failed"; return -1;
+                    }
+                    continue;
+                }
+                match_exact_guided_kernel<MODE><<<(n_desc[l] + 3) / 4, 128, 0, st>>>(sets[l], feat[l], rev[l], n_desc[l], sets[r], feat[r], rev[r],
+                                                                                  n_desc[r], models + 9 * (size_t)p, t2, o);
+            } else {
+                match_exact_kernel<<<(n_desc[l] + 3) / 4, 128, 0, st>>>(sets[l], n_desc[l], sets[r], n_desc[r], o);
+            }
             ++launches;
         }
         return launches;
     }
     if (plan.groups.empty()) return 0;
-    // every group's sets, pairs and items, uploaded once; one workspace for the largest group's planes, reused in turn
-    struct Meta { size_t sets, pairs, items; };
+    // every group's sets, pairs and items (guided: also its position sets and its group pair -> caller pair map), uploaded
+    // once; one workspace for the largest group's planes, reused in turn
+    struct Meta { size_t sets, csets, pairs, gpair, items; };
     std::vector<Meta> meta;
     size_t meta_bytes = 0, planes = 0;
     for (const MatchGroup& g : plan.groups) {
         if (g.rows > 0x7fffff80) { *err = "matcher: a group of pairs has more than 2^31 rows"; return -1; }
         Meta m;
         m.sets = meta_bytes;  meta_bytes = align_up(meta_bytes + g.sets.size() * sizeof(SplitSet), 16);
+        m.csets = meta_bytes; meta_bytes = align_up(meta_bytes + (guided ? g.sets.size() * sizeof(MatchCoordSet) : 0), 16);
         m.pairs = meta_bytes; meta_bytes = align_up(meta_bytes + g.pairs.size() * sizeof(RerankPair), 16);
+        m.gpair = meta_bytes; meta_bytes = align_up(meta_bytes + (guided ? g.pairs.size() * sizeof(int32_t) : 0), 16);
         m.items = meta_bytes; meta_bytes = align_up(meta_bytes + g.items.size() * sizeof(MatchItem), 16);
         meta.push_back(m);
         planes = std::max(planes, g.bytes());
@@ -507,12 +758,19 @@ int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int
     for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
         const MatchGroup& g = plan.groups[gi];
         SplitSet* hs = reinterpret_cast<SplitSet*>(host.data() + meta[gi].sets);
-        for (size_t k = 0; k < g.sets.size(); ++k) hs[k] = {sets[g.sets[k].set], n_desc[g.sets[k].set], (int32_t)g.sets[k].row};
+        MatchCoordSet* hc = reinterpret_cast<MatchCoordSet*>(host.data() + meta[gi].csets);
+        for (size_t k = 0; k < g.sets.size(); ++k) {
+            const int si = g.sets[k].set;
+            hs[k] = {sets[si], n_desc[si], (int32_t)g.sets[k].row};
+            if (guided) hc[k] = {feat[si], rev[si], n_desc[si], (int32_t)g.sets[k].row};
+        }
         RerankPair* hp = reinterpret_cast<RerankPair*>(host.data() + meta[gi].pairs);
+        int32_t* hg = reinterpret_cast<int32_t*>(host.data() + meta[gi].gpair);
         for (size_t k = 0; k < g.pairs.size(); ++k) {
             const MatchGroupPair& gp = g.pairs[k];
             const int l = pairs[2 * gp.pair], r = pairs[2 * gp.pair + 1];
             hp[k] = {sets[l], sets[r], plan.out_row[gp.pair], gp.row, gp.cand, n_desc[r], gp.chunks};
+            if (guided) hg[k] = gp.pair;
         }
         if (!g.items.empty()) std::memcpy(host.data() + meta[gi].items, g.items.data(), g.items.size() * sizeof(MatchItem));
     }
@@ -523,8 +781,11 @@ int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int
     if (cudaMallocFromPoolAsync(&ws, meta_bytes + planes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (matcher workspace)"; cudaGetLastError(); return -1; }
     if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "matcher: plan upload failed"; return -1; }
     static_assert(TC_SMEM + 1024 <= 227 * 1024, "matcher shared memory");
+    static_assert(TC_SMEM + 1024 + BN * sizeof(float2) <= 227 * 1024, "guided matcher shared memory");
     static_assert(BM == kMatchTile && BN == kMatchTile && kCand == kMatchCand, "planner and kernel tile sizes");
-    cudaFuncSetAttribute(match_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
+    static_assert(kMatchGuidedRowBytes == kMatchRowBytes + sizeof(float2), "pooled guided row: hi + lo, norm, position");
+    if constexpr (guided) cudaFuncSetAttribute(match_tc_guided_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
+    else cudaFuncSetAttribute(match_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM);
     const int sms = sm_count();
     for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
         const MatchGroup& g = plan.groups[gi];
@@ -535,7 +796,7 @@ int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int
             float* hi = reinterpret_cast<float*>(ws + meta_bytes);
             float* lo = reinterpret_cast<float*>(ws + meta_bytes + (size_t)rows * 512);
             float* norm = reinterpret_cast<float*>(ws + meta_bytes + (size_t)rows * 1024);
-            cand = reinterpret_cast<int32_t*>(ws + meta_bytes + (size_t)rows * 1028);
+            cand = reinterpret_cast<int32_t*>(ws + meta_bytes + (size_t)rows * row_bytes);
             // one tensor map per plane: a left tile and a right tile are both row offsets into it
             CUtensorMap m_hi, m_lo;
             if (!make_tmap_2d(&m_hi, hi, 128, rows, 512, KB, BM, true) || !make_tmap_2d(&m_lo, lo, 128, rows, 512, KB, BM, true)) {
@@ -544,8 +805,16 @@ int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int
             match_split_kernel<<<(rows + 3) / 4, 128, 0, st>>>(reinterpret_cast<const SplitSet*>(ws + meta[gi].sets), (int)g.sets.size(),
                                                                rows, hi, lo, norm);
             const int n_items = (int)g.items.size();
-            match_tc_kernel<<<std::min(sms, n_items), TC_THREADS, TC_SMEM, st>>>(m_hi, m_lo, norm,
-                                                                                reinterpret_cast<const MatchItem*>(ws + meta[gi].items), n_items, cand);
+            const MatchItem* d_items = reinterpret_cast<const MatchItem*>(ws + meta[gi].items);
+            if constexpr (guided) {
+                float2* pos = reinterpret_cast<float2*>(ws + meta_bytes + (size_t)rows * kMatchRowBytes);
+                launch_match_coords(reinterpret_cast<const MatchCoordSet*>(ws + meta[gi].csets), (int)g.sets.size(), rows, pos, st);
+                match_tc_guided_kernel<MODE><<<std::min(sms, n_items), TC_THREADS, TC_SMEM, st>>>(
+                    m_hi, m_lo, norm, pos, models, reinterpret_cast<const int32_t*>(ws + meta[gi].gpair), t2, d_items, n_items, cand);
+                ++launches;
+            } else {
+                match_tc_kernel<<<std::min(sms, n_items), TC_THREADS, TC_SMEM, st>>>(m_hi, m_lo, norm, d_items, n_items, cand);
+            }
             launches += 2;
         }
         match_rerank_kernel<<<(unsigned)((g.left_rows + 3) / 4), 128, 0, st>>>(d_pairs, (int)g.pairs.size(), g.left_rows, cand, out);
@@ -553,6 +822,16 @@ int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int
     }
     cudaFreeAsync(ws, st);
     return launches;
+}
+
+} // namespace
+
+int run_match_batch(const ps_descriptor* const* sets, const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs,
+                    int32_t* out, int flags, cudaStream_t st, const char** err)
+{
+    *err = nullptr;
+    if (n_pairs <= 0) return 0;
+    return run_batch<kUnguided>(sets, nullptr, nullptr, n_desc, n_sets, pairs, n_pairs, nullptr, 0.0f, out, match_choice(flags), st, err);
 }
 
 int run_match(const ps_descriptor* l, int nl, const ps_descriptor* r, int nr, int32_t* out, int flags, cudaStream_t st,
@@ -574,6 +853,23 @@ int run_match(const ps_descriptor* l, int nl, const ps_descriptor* r, int nr, in
     const bool same = l == r && nl == nr;
     const int32_t pair[2] = {0, same ? 0 : 1};
     return run_match_batch(sets, n_desc, same ? 1 : 2, pair, 1, out, PS_MATCH_TENSOR, st, err);
+}
+
+void launch_match_coords(const MatchCoordSet* d_sets, int n_sets, int rows, float2* out, cudaStream_t st)
+{
+    if (rows > 0) match_coords_kernel<<<(rows + 255) / 256, 256, 0, st>>>(d_sets, n_sets, rows, out);
+}
+
+int run_match_guided_batch(const ps_descriptor* const* sets, const ps_feature* const* feat, const int32_t* const* rev,
+                           const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs, const float* models, int model,
+                           float threshold, int32_t* out, int flags, cudaStream_t st, const char** err)
+{
+    *err = nullptr;
+    if (n_pairs <= 0) return 0;
+    flags = match_choice(flags);
+    const float t2 = threshold * threshold;
+    return model == kGuidedH ? run_batch<kGuidedH>(sets, feat, rev, n_desc, n_sets, pairs, n_pairs, models, t2, out, flags, st, err)
+                             : run_batch<kGuidedF>(sets, feat, rev, n_desc, n_sets, pairs, n_pairs, models, t2, out, flags, st, err);
 }
 
 } // namespace psb

@@ -8,6 +8,8 @@
 #include <cstdint>
 #include <vector>
 
+#include "popsift_b200.h"
+
 namespace psb {
 
 __device__ __forceinline__ unsigned s32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -41,7 +43,33 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
 
+// a plain 1-D bulk copy global -> shared, completing on `bar` (src, dst and bytes multiples of 16)
+__device__ __forceinline__ void bulk_copy(void* dst, const void* src, unsigned bytes, uint64_t* bar)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 :: "r"(s32(dst)), "l"(src), "r"(bytes), "r"(s32(bar)) : "memory");
+}
+
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Guided matching: the pixel position of every pooled row of a group, (feat[rev[i]].xpos, .ypos) for the set's row i and
+// NaN for padding rows (k_match.cu), so that the kernels' epilogues read a right tile's 128 points as one 1 KB block.
+struct MatchCoordSet { const ps_feature* f; const int32_t* rev; int32_t n; int32_t row; };
+void launch_match_coords(const MatchCoordSet* d_sets, int n_sets, int rows, float2* out, cudaStream_t st);
+
+// pixel position of descriptor i of a set: its Feature through the reverse map
+__device__ __forceinline__ float2 feat_xy(const ps_feature* __restrict__ f, const int32_t* __restrict__ rev, int i)
+{
+    const ps_feature* p = f + __ldg(rev + i);
+    return make_float2(__ldg(&p->xpos), __ldg(&p->ypos));
+}
+
+// a pair's 3 x 3 model (row-major)
+__device__ __forceinline__ void load_model(float (&m)[9], const float* __restrict__ p)
+{
+#pragma unroll
+    for (int k = 0; k < 9; ++k) m[k] = __ldg(p + k);
+}
 
 // the library's own memory pool of the current device (k_match.cu): a pool gives freed memory back to the OS at the next
 // synchronisation unless told to keep it, and mapping the workspace again on every call costs more than the matching

@@ -24,6 +24,9 @@ constexpr int kMatchMaxChunks = 8;              // bound of S
 constexpr int kMatchCand = 4;                   // candidates one item keeps per left row
 constexpr size_t kMatchRowBytes = 2 * 512 + 4;  // pooled hi + lo row and its norm (float32 descriptors)
 constexpr size_t kMatchU8RowBytes = 128 + 4;    // pooled 8-bit row and its norm key (k_match_u8.cu)
+// guided matching adds the row's pixel position (float2) to either
+constexpr size_t kMatchGuidedRowBytes = kMatchRowBytes + 8;
+constexpr size_t kMatchU8GuidedRowBytes = kMatchU8RowBytes + 8;
 // freed workspace the matcher's memory pool keeps mapped, and the default cap of one group's workspace
 // (POPSIFT_B200_MATCH_WS=bytes overrides the cap)
 constexpr size_t kMatchPoolKeep = (size_t)1 << 30;

@@ -32,6 +32,7 @@
 #include "ps_internal.h"
 #include "k_match_common.h"
 #include "k_match_plan.h"
+#include "k_guided.h"
 #include "tma_util.h"
 
 #include <algorithm>
@@ -331,6 +332,319 @@ match_u8_finalize_kernel(const FinalPair* __restrict__ pairs, int n_pairs, int64
               T.k2 == kNone ? kNone : na + T.k2, T.i2);
 }
 
+// ------------------------------------------------------------------------------------------------ guided matching
+//
+// ps_match_u8_guided_batch (include/popsift_b200_guided.h): the exact 2-NN restricted per left row to the right descriptors
+// that pass the pair's geometric test (k_guided.h).  In match_u8_guided_kernel an ineligible element's packed key becomes
+// kMasked | e: above every real key (< (2^24 + 2^23) << 5) and every padding key (= that), still distinct in its low 5
+// bits, so the min tree and the "next key" scan work unchanged.  Unpacked, its key is above kPadNorm, like a padding
+// column's is equal to it, and the guided finalize drops every entry whose key is >= kPadNorm.
+
+constexpr int kMasked = 0x7fffffe0;
+
+// launched only for pairs with a non-empty right set (the model is read unconditionally)
+template <int MODEL>
+__global__ void __launch_bounds__(128, 8)
+match_u8_exact_guided_kernel(const uint8_t* __restrict__ l, const ps_feature* __restrict__ fl, const int32_t* __restrict__ revl, int nl,
+                             const uint8_t* __restrict__ r, const ps_feature* __restrict__ fr, const int32_t* __restrict__ revr, int nr,
+                             const float* __restrict__ model, float t2, int32_t* __restrict__ out)
+{
+    const int lane = threadIdx.x & 31;
+    const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (row >= nl) return;
+    const unsigned a = __ldg(reinterpret_cast<const unsigned*>(l + (size_t)row * 128) + lane);
+    float m[9];
+    load_model(m, model);
+    const float2 p = feat_xy(fl, revl, row);
+    const GuidedRow gr = guided_row<MODEL>(m, t2, p.x, p.y);
+    int d1 = kNone, d2 = kNone, i1 = 0, i2 = 0;
+    for (int i = 0; i < nr; ++i) {
+        const float2 P = feat_xy(fr, revr, i);                            // the same for every lane
+        if (!guided_ok<MODEL>(gr, guided_col<MODEL>(m, P.x, P.y), t2, P.x, P.y)) continue;
+        const unsigned df = __vabsdiffu4(a, __ldg(reinterpret_cast<const unsigned*>(r + (size_t)i * 128) + lane));
+        const int d = (int)__reduce_add_sync(0xffffffffu, __dp4a(df, df, 0u));
+        if (d < d1) { d2 = d1; i2 = i1; d1 = d; i1 = i; }
+        else if (d < d2) { d2 = d; i2 = i; }
+    }
+    if (lane == 0) store_row(out + 3 * (size_t)row, d1, i1, d2, i2);
+}
+
+// match_u8_kernel plus the geometric test.  coords: the group's pooled pixel positions; models: the caller's 9 floats per
+// pair; gpair: group pair -> caller pair.  A right tile's 128 positions (1 KB) travel with the tile in the same ring stage
+// (same b_full barrier), and the stage is released after the epilogue instead of after the MMAs.
+template <int MODEL>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+match_u8_guided_kernel(const __grid_constant__ CUtensorMap tm, const int32_t* __restrict__ nkey, const float2* __restrict__ coords,
+                       const float* __restrict__ models, const int32_t* __restrict__ gpair, float t2,
+                       const MatchItem* __restrict__ items, int n_items, int4* __restrict__ cand)
+{
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t a_full, a_empty, b_full[STAGES], b_empty[STAGES];
+    uint8_t* smem = smem_raw + ((1024u - (s32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* A = smem;
+    uint8_t* B_st = smem + TILE_BYTES;                           // [STAGES]
+    float2* C_st = reinterpret_cast<float2*>(smem + (1 + STAGES) * TILE_BYTES);   // [STAGES][BN]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+    if (threadIdx.x == 0) {
+        mb_init(&a_full, 1);
+        mb_init(&a_empty, 8);
+        for (int s = 0; s < STAGES; ++s) { mb_init(&b_full[s], 1); mb_init(&b_empty[s], 8); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        // ===== TMA producer (one thread) =====
+        if (threadIdx.x == 0) {
+            int s = 0; unsigned ph = 0;
+            int a_cur = -1; unsigned a_ph = 0;
+            for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+                const MatchItem w = items[it];
+                if (w.a_row != a_cur) {
+                    if (a_cur >= 0) { mb_wait(&a_empty, a_ph); a_ph ^= 1u; }
+                    a_cur = w.a_row;
+                    mb_expect(&a_full, TILE_BYTES);
+                    tma_tile(A, &tm, 0, w.a_row, &a_full);
+                }
+                for (int j = 0; j < w.b_tiles; ++j) {
+                    mb_wait(&b_empty[s], ph ^ 1u);                   // the epilogue that read this slot is done
+                    mb_expect(&b_full[s], TILE_BYTES + BN * sizeof(float2));
+                    tma_tile(B_st + s * TILE_BYTES, &tm, 0, w.b_row + j * BN, &b_full[s]);
+                    bulk_copy(C_st + s * BN, coords + w.b_row + j * BN, BN * sizeof(float2), &b_full[s]);
+                    if (++s == STAGES) { s = 0; ph ^= 1u; }
+                }
+            }
+        }
+        return;
+    }
+    // ===== consumers: warpgroup c owns rows 64c .. 64c+63 of each item's 128 =====
+    const int c = (warp >> 2) - 1;
+    const int q = lane & 3;
+    const int r0 = 64 * c + 16 * (warp & 3) + (lane >> 2);
+    const uint64_t a_desc = gmma_desc(A + 64 * c * 128);
+    int d[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) d[i] = 0;
+    int s = 0; unsigned ph = 0;
+    int a_cur = -1; unsigned a_ph = 0;
+    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+        const MatchItem w = items[it];
+        if (w.a_row != a_cur) { mb_wait(&a_full, a_ph); a_ph ^= 1u; a_cur = w.a_row; }
+        const int32_t* __restrict__ rkey = nkey + w.b_row;
+        // the pair's model, and the per-row part of the test for the thread's two left rows (NaN rows: nothing eligible)
+        float m[9];
+        load_model(m, models + 9 * (size_t)__ldg(gpair + w.pair));
+        const float2 p0 = __ldg(coords + w.a_row + r0), p1 = __ldg(coords + w.a_row + r0 + 8);
+        const GuidedRow g0 = guided_row<MODEL>(m, t2, p0.x, p0.y), g1 = guided_row<MODEL>(m, t2, p1.x, p1.y);
+        Top2 T0, T1;
+        for (int j = 0; j < w.b_tiles; ++j) {
+            const int nb0 = j * BN;
+            int2 nk[16];
+#pragma unroll
+            for (int b = 0; b < 16; ++b) nk[b] = __ldg(reinterpret_cast<const int2*>(rkey + nb0 + 8 * b + 2 * q));
+            mb_wait(&b_full[s], ph);
+            wg_fence();
+            const uint64_t b_desc = gmma_desc(B_st + s * TILE_BYTES);
+#pragma unroll
+            for (int k = 0; k < 128 / MMA_K; ++k)
+                wgmma_u8(d, a_desc + 2 * k, b_desc + 2 * k, k != 0);
+            wg_commit();
+            wg_wait<0>();
+            // packed keys as in match_u8_kernel; an ineligible element gets kMasked | e.  Columns 8b + 2q and 8b + 2q + 1
+            // are one float4 of the stage's positions; the per-column part of the test serves both rows.
+            const float4* cp = reinterpret_cast<const float4*>(C_st + s * BN);
+#pragma unroll
+            for (int b = 0; b < 16; ++b) {
+                const float4 xy = cp[4 * b + q];
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                    const float X = u ? xy.z : xy.x, Y = u ? xy.w : xy.y;
+                    const float cb = guided_col<MODEL>(m, X, Y);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int i = 4 * b + 2 * h + u;
+                        const bool ok = guided_ok<MODEL>(h ? g1 : g0, cb, t2, X, Y);
+                        d[i] = ok ? (u ? nk[b].y : nk[b].x) - 64 * d[i] : (kMasked | (2 * b + u));
+                    }
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mb_arrive(&b_empty[s]);
+            if (++s == STAGES) { s = 0; ph ^= 1u; }
+            top2_row<0>(T0, d, w.b_col0 + nb0, q);
+            top2_row<1>(T1, d, w.b_col0 + nb0, q);
+        }
+        T0.merge_xor(1); T1.merge_xor(1);
+        T0.merge_xor(2); T1.merge_xor(2);
+        if (q == 0) {
+            int4* cw = cand + w.cand + (int64_t)r0 * w.stride;
+            if (w.l_row0 + r0 < w.nl) *cw = make_int4(T0.k1, T0.i1, T0.k2, T0.i2);
+            if (w.l_row0 + r0 + 8 < w.nl) cw[(int64_t)8 * w.stride] = make_int4(T1.k1, T1.i1, T1.k2, T1.i2);
+        }
+        const int nx = it + gridDim.x;
+        if (nx < n_items && items[nx].a_row != a_cur) {
+            __syncwarp();
+            if (lane == 0) mb_arrive(&a_empty);
+        }
+    }
+}
+
+// match_u8_finalize_kernel for guided rows: entries whose key is >= kPadNorm (padding columns and ineligible ones) dropped
+__global__ void __launch_bounds__(128)
+match_u8_guided_finalize_kernel(const FinalPair* __restrict__ pairs, int n_pairs, int64_t rows, const int32_t* __restrict__ nkey,
+                                const int4* __restrict__ cand, int32_t* __restrict__ out)
+{
+    const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= rows) return;
+    int a = 0, b = n_pairs - 1;
+    while (a < b) { const int m = (a + b + 1) >> 1; if (pairs[m].row <= g) a = m; else b = m - 1; }
+    const FinalPair P = pairs[a];
+    const int64_t row = g - P.row;
+    Top2 T;
+    for (int c = 0; c < P.chunks; ++c) {
+        const int4 v = cand[P.cand + row * P.chunks + c];
+        if (v.x < kPadNorm) T.offer(v.x, v.y);
+        if (v.z < kPadNorm) T.offer(v.z, v.w);
+    }
+    const int na = T.k1 == kNone ? 0 : (nkey[P.a_row + row] >> 5) - kKeyBias;
+    store_row(out + 3 * (size_t)(P.out_row + row), T.k1 == kNone ? kNone : na + T.k1, T.i1,
+              T.k2 == kNone ? kNone : na + T.k2, T.i2);
+}
+
+constexpr int kUnguided = -1;
+
+// The host side of the batched 8-bit matcher: plan, metadata upload, workspace, launches.  MODE = kUnguided:
+// ps_match_u8_batch; MODE = kGuidedH / kGuidedF: ps_match_u8_guided_batch, which also uses feat, rev, models and t2, and
+// whose pooled rows carry the row's pixel position (8 more bytes per row).  Arguments already validated, flags resolved.
+template <int MODE>
+int run_u8_batch(const uint8_t* const* sets, const ps_feature* const* feat, const int32_t* const* rev, const int32_t* n_desc,
+                 int n_sets, const int32_t* pairs, int n_pairs, const float* models, float t2, int32_t* out, int flags,
+                 cudaStream_t st, const char** err)
+{
+    constexpr bool guided = MODE != kUnguided;
+    constexpr size_t row_bytes = guided ? kMatchU8GuidedRowBytes : kMatchU8RowBytes;
+    const MatchPlan plan = plan_match(n_sets, n_desc, n_pairs, pairs, sm_count(), match_workspace_cap(), row_bytes);
+    int launches = 0;
+    if (flags == PS_MATCH_EXACT) {
+        // the CUDA-core kernel, pair by pair: the in-library reference
+        for (int p = 0; p < n_pairs; ++p) {
+            const int l = pairs[2 * p], r = pairs[2 * p + 1];
+            if (n_desc[l] <= 0) continue;
+            int32_t* o = out + 3 * (size_t)plan.out_row[p];
+            if constexpr (guided) {
+                // an empty right set gives rows (0, 0, 0), and the pair's model need not exist: it is not read
+                if (n_desc[r] <= 0) {
+                    if (cudaMemsetAsync(o, 0, (size_t)n_desc[l] * 3 * sizeof(int32_t), st) != cudaSuccess) {
+                        cudaGetLastError(); *err = "guided u8 matcher: cudaMemsetAsync failed"; return -1;
+                    }
+                    continue;
+                }
+                match_u8_exact_guided_kernel<MODE><<<(n_desc[l] + 3) / 4, 128, 0, st>>>(sets[l], feat[l], rev[l], n_desc[l], sets[r], feat[r],
+                                                                                     rev[r], n_desc[r], models + 9 * (size_t)p, t2, o);
+            } else {
+                match_u8_exact_kernel<<<(n_desc[l] + 3) / 4, 128, 0, st>>>(sets[l], n_desc[l], sets[r], n_desc[r], o);
+            }
+            ++launches;
+        }
+        return launches;
+    }
+    if (plan.groups.empty()) return 0;
+    // every group's sets, pairs and items (guided: also its position sets and its group pair -> caller pair map), uploaded
+    // once; one workspace for the largest group's plane, reused in turn
+    struct Meta { size_t sets, csets, pairs, gpair, items; };
+    std::vector<Meta> meta;
+    size_t meta_bytes = 0, planes = 0;
+    for (const MatchGroup& g : plan.groups) {
+        if (g.rows > 0x7fffff80) { *err = "matcher: a group of pairs has more than 2^31 rows"; return -1; }
+        Meta m;
+        m.sets = meta_bytes;  meta_bytes = align_up(meta_bytes + g.sets.size() * sizeof(PackSet), 16);
+        m.csets = meta_bytes; meta_bytes = align_up(meta_bytes + (guided ? g.sets.size() * sizeof(MatchCoordSet) : 0), 16);
+        m.pairs = meta_bytes; meta_bytes = align_up(meta_bytes + g.pairs.size() * sizeof(FinalPair), 16);
+        m.gpair = meta_bytes; meta_bytes = align_up(meta_bytes + (guided ? g.pairs.size() * sizeof(int32_t) : 0), 16);
+        m.items = meta_bytes; meta_bytes = align_up(meta_bytes + g.items.size() * sizeof(MatchItem), 16);
+        meta.push_back(m);
+        planes = std::max(planes, g.bytes());
+    }
+    meta_bytes = align_up(meta_bytes, 1024);
+    std::vector<uint8_t> host(meta_bytes);
+    for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
+        const MatchGroup& g = plan.groups[gi];
+        PackSet* hs = reinterpret_cast<PackSet*>(host.data() + meta[gi].sets);
+        MatchCoordSet* hc = reinterpret_cast<MatchCoordSet*>(host.data() + meta[gi].csets);
+        for (size_t k = 0; k < g.sets.size(); ++k) {
+            const int si = g.sets[k].set;
+            hs[k] = {sets[si], n_desc[si], (int32_t)g.sets[k].row};
+            if (guided) hc[k] = {feat[si], rev[si], n_desc[si], (int32_t)g.sets[k].row};
+        }
+        FinalPair* hp = reinterpret_cast<FinalPair*>(host.data() + meta[gi].pairs);
+        int32_t* hg = reinterpret_cast<int32_t*>(host.data() + meta[gi].gpair);
+        for (size_t k = 0; k < g.pairs.size(); ++k) {
+            const MatchGroupPair& gp = g.pairs[k];
+            const int l = pairs[2 * gp.pair], r = pairs[2 * gp.pair + 1];
+            int64_t a_row = 0;
+            for (const MatchGroupSet& s : g.sets) if (s.set == l) a_row = s.row;
+            hp[k] = {plan.out_row[gp.pair], gp.row, gp.cand, (int32_t)a_row, n_desc[r], gp.chunks, 0};
+            if (guided) hg[k] = gp.pair;
+        }
+        if (!g.items.empty()) std::memcpy(host.data() + meta[gi].items, g.items.data(), g.items.size() * sizeof(MatchItem));
+    }
+    cudaMemPool_t pool = match_pool(err);
+    if (!pool) return -1;
+    uint8_t* ws = nullptr;
+    // stream-ordered, so nothing blocks
+    if (cudaMallocFromPoolAsync(&ws, meta_bytes + planes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (u8 matcher workspace)"; cudaGetLastError(); return -1; }
+    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "u8 matcher: plan upload failed"; return -1; }
+    // the guided kernel's ring stages carry a right tile's 128 positions next to the tile
+    constexpr size_t smem_bytes = U8_SMEM + (guided ? (size_t)STAGES * BN * sizeof(float2) : 0);
+    static_assert(smem_bytes + 1024 <= 227 * 1024, "u8 matcher shared memory");
+    static_assert(BM == kMatchTile && BN == kMatchTile && sizeof(int4) == kMatchCand * 4, "planner and kernel tile / slot sizes");
+    static_assert(kMatchU8RowBytes == 128 + sizeof(int32_t), "pooled u8 row: descriptor + norm key");
+    static_assert(kMatchU8GuidedRowBytes == kMatchU8RowBytes + sizeof(float2), "pooled guided u8 row: descriptor, norm key, position");
+    static_assert(kMasked > ((kPadNorm + kKeyBias) << 5 | 31) && (kMasked & 31) == 0, "masked keys above padding keys");
+    if constexpr (guided) cudaFuncSetAttribute(match_u8_guided_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    else cudaFuncSetAttribute(match_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    const int sms = sm_count();
+    for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
+        const MatchGroup& g = plan.groups[gi];
+        const FinalPair* d_pairs = reinterpret_cast<const FinalPair*>(ws + meta[gi].pairs);
+        const int32_t* nkey = nullptr;
+        const int4* cand = nullptr;
+        if (!g.items.empty()) {
+            const int rows = (int)g.rows;
+            uint8_t* plane = ws + meta_bytes;
+            int32_t* nk = reinterpret_cast<int32_t*>(ws + meta_bytes + (size_t)rows * 128);
+            int4* cd = reinterpret_cast<int4*>(ws + meta_bytes + (size_t)rows * row_bytes);
+            // one tensor map: a left tile and a right tile are both row offsets into it
+            CUtensorMap tm;
+            if (!make_tmap_2d(&tm, plane, 128, rows, 128, 128, BM, true)) {
+                cudaFreeAsync(ws, st); *err = "cuTensorMapEncodeTiled failed (u8 matcher)"; return -1;
+            }
+            match_u8_pack_kernel<<<(rows + 3) / 4, 128, 0, st>>>(reinterpret_cast<const PackSet*>(ws + meta[gi].sets), (int)g.sets.size(),
+                                                                 rows, plane, nk);
+            const int n_items = (int)g.items.size();
+            const MatchItem* d_items = reinterpret_cast<const MatchItem*>(ws + meta[gi].items);
+            if constexpr (guided) {
+                float2* pos = reinterpret_cast<float2*>(ws + meta_bytes + (size_t)rows * kMatchU8RowBytes);
+                launch_match_coords(reinterpret_cast<const MatchCoordSet*>(ws + meta[gi].csets), (int)g.sets.size(), rows, pos, st);
+                match_u8_guided_kernel<MODE><<<std::min(sms, n_items), TC_THREADS, smem_bytes, st>>>(
+                    tm, nk, pos, models, reinterpret_cast<const int32_t*>(ws + meta[gi].gpair), t2, d_items, n_items, cd);
+                ++launches;
+            } else {
+                match_u8_kernel<<<std::min(sms, n_items), TC_THREADS, smem_bytes, st>>>(tm, nk, d_items, n_items, cd);
+            }
+            launches += 2;
+            nkey = nk; cand = cd;
+        }
+        const unsigned blocks = (unsigned)((g.left_rows + 127) / 128);
+        if constexpr (guided) match_u8_guided_finalize_kernel<<<blocks, 128, 0, st>>>(d_pairs, (int)g.pairs.size(), g.left_rows, nkey, cand, out);
+        else match_u8_finalize_kernel<<<blocks, 128, 0, st>>>(d_pairs, (int)g.pairs.size(), g.left_rows, nkey, cand, out);
+        ++launches;
+    }
+    cudaFreeAsync(ws, st);
+    return launches;
+}
+
 } // namespace
 
 int run_descriptors_to_u8(const ps_descriptor* in, int n, uint8_t* out, cudaStream_t st)
@@ -346,88 +660,19 @@ int run_match_u8_batch(const uint8_t* const* sets, const int32_t* n_desc, int n_
 {
     *err = nullptr;
     if (n_pairs <= 0) return 0;
+    return run_u8_batch<kUnguided>(sets, nullptr, nullptr, n_desc, n_sets, pairs, n_pairs, nullptr, 0.0f, out, match_choice(flags), st, err);
+}
+
+int run_match_u8_guided_batch(const uint8_t* const* sets, const ps_feature* const* feat, const int32_t* const* rev,
+                              const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs, const float* models, int model,
+                              float threshold, int32_t* out, int flags, cudaStream_t st, const char** err)
+{
+    *err = nullptr;
+    if (n_pairs <= 0) return 0;
     flags = match_choice(flags);
-    const MatchPlan plan = plan_match(n_sets, n_desc, n_pairs, pairs, sm_count(), match_workspace_cap(), kMatchU8RowBytes);
-    int launches = 0;
-    if (flags == PS_MATCH_EXACT) {
-        // the CUDA-core kernel, pair by pair: the in-library reference
-        for (int p = 0; p < n_pairs; ++p) {
-            const int l = pairs[2 * p], r = pairs[2 * p + 1];
-            if (n_desc[l] <= 0) continue;
-            match_u8_exact_kernel<<<(n_desc[l] + 3) / 4, 128, 0, st>>>(sets[l], n_desc[l], sets[r], n_desc[r], out + 3 * (size_t)plan.out_row[p]);
-            ++launches;
-        }
-        return launches;
-    }
-    if (plan.groups.empty()) return 0;
-    // every group's sets, pairs and items, uploaded once; one workspace for the largest group's plane, reused in turn
-    struct Meta { size_t sets, pairs, items; };
-    std::vector<Meta> meta;
-    size_t meta_bytes = 0, planes = 0;
-    for (const MatchGroup& g : plan.groups) {
-        if (g.rows > 0x7fffff80) { *err = "matcher: a group of pairs has more than 2^31 rows"; return -1; }
-        Meta m;
-        m.sets = meta_bytes;  meta_bytes = align_up(meta_bytes + g.sets.size() * sizeof(PackSet), 16);
-        m.pairs = meta_bytes; meta_bytes = align_up(meta_bytes + g.pairs.size() * sizeof(FinalPair), 16);
-        m.items = meta_bytes; meta_bytes = align_up(meta_bytes + g.items.size() * sizeof(MatchItem), 16);
-        meta.push_back(m);
-        planes = std::max(planes, g.bytes());
-    }
-    meta_bytes = align_up(meta_bytes, 1024);
-    std::vector<uint8_t> host(meta_bytes);
-    for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
-        const MatchGroup& g = plan.groups[gi];
-        PackSet* hs = reinterpret_cast<PackSet*>(host.data() + meta[gi].sets);
-        for (size_t k = 0; k < g.sets.size(); ++k) hs[k] = {sets[g.sets[k].set], n_desc[g.sets[k].set], (int32_t)g.sets[k].row};
-        FinalPair* hp = reinterpret_cast<FinalPair*>(host.data() + meta[gi].pairs);
-        for (size_t k = 0; k < g.pairs.size(); ++k) {
-            const MatchGroupPair& gp = g.pairs[k];
-            const int l = pairs[2 * gp.pair], r = pairs[2 * gp.pair + 1];
-            int64_t a_row = 0;
-            for (const MatchGroupSet& s : g.sets) if (s.set == l) a_row = s.row;
-            hp[k] = {plan.out_row[gp.pair], gp.row, gp.cand, (int32_t)a_row, n_desc[r], gp.chunks, 0};
-        }
-        if (!g.items.empty()) std::memcpy(host.data() + meta[gi].items, g.items.data(), g.items.size() * sizeof(MatchItem));
-    }
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    // stream-ordered, so nothing blocks
-    if (cudaMallocFromPoolAsync(&ws, meta_bytes + planes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (u8 matcher workspace)"; cudaGetLastError(); return -1; }
-    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "u8 matcher: plan upload failed"; return -1; }
-    static_assert(U8_SMEM + 1024 <= 227 * 1024, "u8 matcher shared memory");
-    static_assert(BM == kMatchTile && BN == kMatchTile && sizeof(int4) == kMatchCand * 4, "planner and kernel tile / slot sizes");
-    static_assert(kMatchU8RowBytes == 128 + sizeof(int32_t), "pooled u8 row: descriptor + norm key");
-    cudaFuncSetAttribute(match_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)U8_SMEM);
-    const int sms = sm_count();
-    for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
-        const MatchGroup& g = plan.groups[gi];
-        const int32_t* nkey = nullptr;
-        const int4* cand = nullptr;
-        if (!g.items.empty()) {
-            const int rows = (int)g.rows;
-            uint8_t* plane = ws + meta_bytes;
-            int32_t* nk = reinterpret_cast<int32_t*>(ws + meta_bytes + (size_t)rows * 128);
-            int4* cd = reinterpret_cast<int4*>(ws + meta_bytes + (size_t)rows * kMatchU8RowBytes);
-            // one tensor map: a left tile and a right tile are both row offsets into it
-            CUtensorMap tm;
-            if (!make_tmap_2d(&tm, plane, 128, rows, 128, 128, BM, true)) {
-                cudaFreeAsync(ws, st); *err = "cuTensorMapEncodeTiled failed (u8 matcher)"; return -1;
-            }
-            match_u8_pack_kernel<<<(rows + 3) / 4, 128, 0, st>>>(reinterpret_cast<const PackSet*>(ws + meta[gi].sets), (int)g.sets.size(),
-                                                                 rows, plane, nk);
-            const int n_items = (int)g.items.size();
-            match_u8_kernel<<<std::min(sms, n_items), TC_THREADS, U8_SMEM, st>>>(tm, nk, reinterpret_cast<const MatchItem*>(ws + meta[gi].items),
-                                                                               n_items, cd);
-            launches += 2;
-            nkey = nk; cand = cd;
-        }
-        match_u8_finalize_kernel<<<(unsigned)((g.left_rows + 127) / 128), 128, 0, st>>>(reinterpret_cast<const FinalPair*>(ws + meta[gi].pairs),
-                                                                                       (int)g.pairs.size(), g.left_rows, nkey, cand, out);
-        ++launches;
-    }
-    cudaFreeAsync(ws, st);
-    return launches;
+    const float t2 = threshold * threshold;
+    return model == kGuidedH ? run_u8_batch<kGuidedH>(sets, feat, rev, n_desc, n_sets, pairs, n_pairs, models, t2, out, flags, st, err)
+                             : run_u8_batch<kGuidedF>(sets, feat, rev, n_desc, n_sets, pairs, n_pairs, models, t2, out, flags, st, err);
 }
 
 } // namespace psb

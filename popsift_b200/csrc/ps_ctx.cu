@@ -8,6 +8,7 @@
 //   ps_descriptor[desc_cap], int feat_to_ext[desc_cap], Counters.
 // There is no intermediate (row-filtered) plane in HBM: the row pass lives in shared memory.
 #include "ps_internal.h"
+#include "popsift_b200_guided.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1182,6 +1183,61 @@ extern "C" int ps_verify_batch(int device, int n_pairs, const float* d_corr, con
     const cudaError_t e = cudaStreamSynchronize(nullptr);
     if (e != cudaSuccess) { g_create_error = std::string("ps_verify_batch: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
     return PS_OK;
+}
+
+// both guided entry points: the argument checks of ps_match_batch / ps_match_u8_batch and ps_match_correspondences, the
+// model and threshold, and d_models when some pair has rows and a non-empty right set; then the run
+static int match_guided(const char* name, bool u8, int device, int n_sets, const void* const* d_sets, const ps_feature* const* d_feat,
+                        const int32_t* const* d_rev, const int32_t* n_desc, int n_pairs, const int32_t* pairs,
+                        const float* d_models, int model, float threshold, int32_t* d_out, int flags)
+{
+    if (n_sets < 0 || n_pairs < 0 || (n_sets > 0 && (!d_sets || !d_feat || !d_rev || !n_desc)) || (n_pairs > 0 && !pairs)) return PS_ERR_ARG;
+    if (model != PS_GEOM_HOMOGRAPHY && model != PS_GEOM_FUNDAMENTAL) return PS_ERR_ARG;
+    if (!std::isfinite(threshold) || !(threshold > 0.0f)) return PS_ERR_ARG;
+    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    for (int i = 0; i < n_sets; ++i) {
+        if (n_desc[i] < 0) return PS_ERR_ARG;
+        if (n_desc[i] == 0) continue;
+        if (!d_sets[i] || ps_pointer_device(d_sets[i]) != device) return PS_ERR_ARG;
+        if (u8 && (reinterpret_cast<uintptr_t>(d_sets[i]) & 15u)) return PS_ERR_ARG;
+        if (ps_pointer_device(d_feat[i]) != device || ps_pointer_device(d_rev[i]) != device) return PS_ERR_ARG;
+    }
+    int64_t rows = 0;
+    bool work = false;                                    // some pair has rows and a non-empty right set
+    for (int p = 0; p < n_pairs; ++p) {
+        const int l = pairs[2 * p], r = pairs[2 * p + 1];
+        if (l < 0 || l >= n_sets || r < 0 || r >= n_sets) return PS_ERR_ARG;
+        rows += n_desc[l];
+        work |= n_desc[l] > 0 && n_desc[r] > 0;
+    }
+    if (rows == 0) return PS_OK;
+    if (!d_out) return PS_ERR_ARG;
+    if (work && ps_pointer_device(d_models) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    const int n = u8 ? run_match_u8_guided_batch(reinterpret_cast<const uint8_t* const*>(d_sets), d_feat, d_rev, n_desc, n_sets, pairs, n_pairs,
+                                                 d_models, model, threshold, d_out, flags, nullptr, &err)
+                     : run_match_guided_batch(reinterpret_cast<const ps_descriptor* const*>(d_sets), d_feat, d_rev, n_desc, n_sets, pairs,
+                                              n_pairs, d_models, model, threshold, d_out, flags, nullptr, &err);
+    if (n < 0) { g_create_error = err ? err : std::string(name) + " failed"; return PS_ERR_CUDA; }
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string(name) + ": " + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
+}
+
+extern "C" int ps_match_guided_batch(int device, int n_sets, const ps_descriptor* const* d_sets, const ps_feature* const* d_feat,
+                                     const int32_t* const* d_rev, const int32_t* n_desc, int n_pairs, const int32_t* pairs,
+                                     const float* d_models, int model, float threshold, int32_t* d_out, int flags)
+{
+    return match_guided("ps_match_guided_batch", false, device, n_sets, reinterpret_cast<const void* const*>(d_sets), d_feat, d_rev,
+                        n_desc, n_pairs, pairs, d_models, model, threshold, d_out, flags);
+}
+
+extern "C" int ps_match_u8_guided_batch(int device, int n_sets, const uint8_t* const* d_sets, const ps_feature* const* d_feat,
+                                        const int32_t* const* d_rev, const int32_t* n_desc, int n_pairs, const int32_t* pairs,
+                                        const float* d_models, int model, float threshold, int32_t* d_out, int flags)
+{
+    return match_guided("ps_match_u8_guided_batch", true, device, n_sets, reinterpret_cast<const void* const*>(d_sets), d_feat, d_rev,
+                        n_desc, n_pairs, pairs, d_models, model, threshold, d_out, flags);
 }
 
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)

@@ -224,4 +224,16 @@ int run_match_correspondences(const ps_feature* const* feat, const int32_t* cons
 int run_verify_batch(int n_pairs, const float* corr, const int32_t* corr_start, const int32_t* n_corr, const ps_verify_params& prm,
                      float* d_models, int32_t* d_n, uint8_t* d_mask, const ps_verify_taps* taps, cudaStream_t st, const char** err);
 
+// guided matching (include/popsift_b200_guided.h), arguments already validated: run_match_batch / run_match_u8_batch with
+// right descriptor j of pair p eligible for left descriptor i only when their keypoints pass the test of k_guided.h under
+// the pair's model (models: DEVICE, 9 floats per pair; model: PS_GEOM_*; threshold in pixels).  EXACT runs the CUDA-core
+// guided kernels pair by pair; AUTO / TENSOR plan with rows 8 bytes larger (the pixel position) and run one split / pack,
+// one position, one guided tensor-core and one re-rank / finalize launch per group.
+int run_match_guided_batch(const ps_descriptor* const* sets, const ps_feature* const* feat, const int32_t* const* rev,
+                           const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs, const float* models, int model,
+                           float threshold, int32_t* out, int flags, cudaStream_t st, const char** err);
+int run_match_u8_guided_batch(const uint8_t* const* sets, const ps_feature* const* feat, const int32_t* const* rev,
+                              const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs, const float* models, int model,
+                              float threshold, int32_t* out, int flags, cudaStream_t st, const char** err);
+
 } // namespace psb
