@@ -6,7 +6,12 @@
 // level): see the scan kernel below.  Survivors of the 26-neighbour test are refined in registers
 // and appended with one warp-ballot + one atomicAdd per warp.
 //
-// Parity contract: with bit-identical DoG planes, the accepted set and (x, y, lpos) of every
+// DoG samples are never read from the slot's DoG region (an extraction does not write it): every reader loads the two
+// Gaussian levels and forms DoG[z] = __fsub_rn(G[z+1], G[z]), the subtraction that defines the plane (reference
+// make_dog), so each sample has the bits the plane would hold.  The octave's planes [(L+3) G] are contiguous: G[z+1]
+// is G[z] + plane.
+//
+// Parity contract: with bit-identical Gaussian planes, the accepted set and (x, y, lpos) of every
 // extremum are bit-identical to the reference's.  The floating-point pattern below is the one in
 // the reference's sm_100 SASS (cuobjdump of oracle/_ref/libpopsift_ref.so):
 //   detK = fma(a1,a2, -(b1*b2));  det = fma(i02,det2, fma(i00,det0, i01*det1));  rsd = __frcp_rn(det)
@@ -20,8 +25,9 @@ namespace psb {
 
 namespace {
 
+// DoG samples of one octave; `gauss` is its first Gaussian plane, nplanes the number of DoG planes (L+2)
 struct DogView {
-    const float* base;
+    const float* gauss;
     int w, h, pitch, nplanes;
     size_t plane;
     __device__ __forceinline__ float at(int x, int y, int z) const
@@ -29,7 +35,8 @@ struct DogView {
         x = min(max(x, 0), w - 1);
         y = min(max(y, 0), h - 1);
         z = min(max(z, 0), nplanes - 1);
-        return __ldg(base + z * plane + (size_t)y * pitch + x);
+        const float* p = gauss + z * plane + (size_t)y * pitch + x;
+        return __fsub_rn(__ldg(p + plane), __ldg(p));
     }
 };
 
@@ -141,11 +148,12 @@ __device__ __noinline__ bool refine(const DogView& dv, const Consts& k, int x, i
 // ---- scan kernel -------------------------------------------------------------------------------
 //
 // A warp owns 30 output columns (lanes 1..30; lanes 0 and 31 only carry the x-halo) and walks down
-// SCAN_ROWS rows.  For every row it loads one value per DoG plane (coalesced 128-byte reads), forms the
-// horizontal 3-max / 3-min of each plane with two shuffles, and keeps the last three rows in registers.
+// SCAN_ROWS rows.  For every row it loads one value per Gaussian plane (coalesced 128-byte reads), subtracts
+// adjacent planes into DoG values, forms the horizontal 3-max / 3-min of each DoG plane with two shuffles, and
+// keeps the last three rows in registers.
 // The 26-neighbour test of a voxel is then a handful of max/min over those registers:
 //     strict maximum  <=>  v > max( 3x3 of plane l-1, 3x3 of plane l+1, 8 neighbours in plane l )
-// All NLEV levels of the octave are evaluated in the same pass, so each DoG value is loaded from HBM
+// All NLEV levels of the octave are evaluated in the same pass, so each Gaussian value is loaded from HBM
 // once (the reference re-reads 27 texels per candidate, s_extrema.cu:56-120).  The verdict is identical:
 // a voxel survives iff it is strictly greater, or strictly smaller, than all 26 neighbours.
 constexpr int SCAN_COLS = 30;      // output columns per warp
@@ -183,7 +191,7 @@ find_extrema_kernel(PyramidView pyr, Consts k, ScanParams sp, InitialExtremum* _
     if (MODE == PS_MODE_OPENCV) xout = xout && !(x < 5 || x >= W - 5);
 
     DogView dv;
-    dv.base = ov.dog; dv.w = W; dv.h = H; dv.pitch = ov.pitch; dv.plane = ov.plane;
+    dv.gauss = ov.gauss; dv.w = W; dv.h = H; dv.pitch = ov.pitch; dv.plane = ov.plane;
     dv.nplanes = pyr.levels + 2;
 
     float thr;
@@ -191,25 +199,25 @@ find_extrema_kernel(PyramidView pyr, Consts k, ScanParams sp, InitialExtremum* _
     else if (MODE == PS_MODE_VLFEAT) thr = __fmul_rn(__fmul_rn(0.8f, 2.0f), k.threshold);
     else thr = __fmul_rn(1.6f, k.threshold);
 
-    constexpr int NP = NLEV + 2;
-    const float* colp = ov.dog + (size_t)(lvl0 - 1) * ov.plane + xc;
+    constexpr int NP = NLEV + 2;                    // DoG planes lvl0-1 .. lvl0+NLEV: Gaussian planes lvl0-1 .. lvl0+NLEV+1
+    const float* colp = ov.gauss + (size_t)(lvl0 - 1) * ov.plane + xc;
     // ring of three rows: value, horizontal 3-max, horizontal 3-min
     float v[3][NP], hx[3][NP], hn[3][NP];
 
     // rows y+1, y+2, y+3: three rows of loads stay in flight per warp (~46 KB per SM, enough to cover
     // the HBM latency at full bandwidth) while row y is evaluated
-    float pend[3][NP];
+    float pend[3][NP + 1];
     const unsigned plane_u = (unsigned)ov.plane;     // a whole octave (<= 15 planes) stays below 2^32 floats
     auto issue_row = [&](int slot, int y) {
         const int yc = min(max(y, 0), H - 1);
         const float* rowp = colp + (size_t)yc * ov.pitch;
 #pragma unroll
-        for (int p = 0; p < NP; ++p) pend[slot][p] = __ldg(rowp + p * plane_u);
+        for (int p = 0; p < NP + 1; ++p) pend[slot][p] = __ldg(rowp + p * plane_u);
     };
     auto finish_row = [&](int slot, int ps) {
 #pragma unroll
         for (int p = 0; p < NP; ++p) {
-            const float c = pend[ps][p];
+            const float c = __fsub_rn(pend[ps][p + 1], pend[ps][p]);
             const float l = __shfl_up_sync(0xffffffffu, c, 1);
             const float r = __shfl_down_sync(0xffffffffu, c, 1);
             v[slot][p] = c;
@@ -279,15 +287,15 @@ find_extrema_kernel(PyramidView pyr, Consts k, ScanParams sp, InitialExtremum* _
 // ---- candidate-driven scan ---------------------------------------------------------------------
 //
 // The pyramid kernels report every DoG pixel pair in which a sample has |value| >= threshold into the
-// list region of the block that produced it (CandSink) while they write the plane.  On real and
+// list region of the block that produced it (CandSink) while they write the Gaussian level.  On real and
 // synthetic images that is a few samples per thousand, so testing only those against their 26
 // neighbours replaces the dense scan's read of every DoG plane.  Accepted set and refinement are those of the dense
 // kernel: same comparisons, same refine<MODE>.
 constexpr int kScanThreads = 256;
 
-// one octave's DoG planes, by value (a reference to the kernel's PyramidView parameter would make every
-// thread copy the whole structure to local memory)
-struct DogOct { const float* dog; int w, h, pitch, nplanes; size_t plane; };
+// one octave's Gaussian planes (DoG[z] = G[z+1] - G[z]), by value (a reference to the kernel's PyramidView parameter
+// would make every thread copy the whole structure to local memory)
+struct DogOct { const float* gauss; int w, h, pitch, nplanes; size_t plane; };
 
 // Region-driven form (default).  A list region = the candidates one block of one level kernel reported; block b of this
 // kernel takes regions b, b + gridDim.x, ... (no prefix sum, no search: a region's octave, level and list follow from
@@ -304,10 +312,11 @@ constexpr int kQ3 = 1024;          // stage-3 queue entries per block; overflowi
 struct Q2Entry { unsigned xy; unsigned ol; };      // x | y << 16 ;  octave | level << 8 | is_max << 16
 
 // Stage 1 on a reported PAIR (x even, x + 1): the two samples share their rows and most of their neighbours, so one
-// thread tests both from three aligned float4 loads + three scalars (columns x-1 .. x+2 of rows y-1, y, y+1) instead of
-// nine scalar loads per sample.  The candidates of a warp are scattered (a few per thousand pixels), every load
-// instruction touches 32 different cache lines: the number of load instructions, not their width, sets the time
-// (9 per sample: 74 us of L1 wavefronts at 4K; 3 per sample now).  Returns bit 0 / bit 1 = sample x / x + 1 survives;
+// thread tests both from six aligned float4 loads + six scalars (columns x-1 .. x+2 of rows y-1, y, y+1 of the two
+// Gaussian planes) instead of eighteen scalar loads per sample.  The candidates of a warp are scattered (a few per
+// thousand pixels), every load instruction touches 32 different cache lines: the number of load instructions, not their
+// width, sets the time (9 per sample from a DoG plane: 74 us of L1 wavefronts at 4K; 3 per sample from a DoG plane,
+// 6 from the Gaussian pair).  Returns bit 0 / bit 1 = sample x / x + 1 survives;
 // bits 2 / 3 = it is a maximum.
 template <int MODE>
 __device__ __forceinline__ unsigned stage1_pair(const DogOct& ov, int level, float thr, int x, int y)
@@ -316,7 +325,7 @@ __device__ __forceinline__ unsigned stage1_pair(const DogOct& ov, int level, flo
     bool iny = y >= 1 && y <= H - 2;
     if (MODE == PS_MODE_OPENCV) iny = iny && !(y < 5 || y >= H - 5);
     if (!iny) return 0u;
-    const float* row = ov.dog + (size_t)level * ov.plane + (size_t)y * ov.pitch;
+    const float* row = ov.gauss + (size_t)level * ov.plane + (size_t)y * ov.pitch;     // G[level] (G[level+1]: + plane)
     const int xa = x & ~3;                                 // aligned group holding x and x + 1 (x is even)
     const bool lowhalf = (x & 2) == 0;                     // x, x+1 are the group's first two floats: x-1 is outside
     const int xs = lowhalf ? max(x - 1, 0) : x + 2;        // the one column outside the group
@@ -324,8 +333,11 @@ __device__ __forceinline__ unsigned stage1_pair(const DogOct& ov, int level, flo
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
         const float* p = row + (long long)(r - 1) * ov.pitch;
-        const float4 g = __ldg(reinterpret_cast<const float4*>(p + xa));
-        const float e = __ldg(p + xs);
+        const float4 g0 = __ldg(reinterpret_cast<const float4*>(p + xa));
+        const float4 g1 = __ldg(reinterpret_cast<const float4*>(p + ov.plane + xa));
+        const float e0 = __ldg(p + xs), e1 = __ldg(p + ov.plane + xs);
+        const float4 g = make_float4(__fsub_rn(g1.x, g0.x), __fsub_rn(g1.y, g0.y), __fsub_rn(g1.z, g0.z), __fsub_rn(g1.w, g0.w));
+        const float e = __fsub_rn(e1, e0);
         if (lowhalf) { a[r] = e; b[r] = g.x; c[r] = g.y; d[r] = g.z; }
         else         { a[r] = g.y; b[r] = g.z; c[r] = g.w; d[r] = e; }
     }
@@ -350,20 +362,26 @@ __device__ __forceinline__ unsigned stage1_pair(const DogOct& ov, int level, flo
     return out;
 }
 
+// the centre and the 3x3 neighbourhoods of DoG planes level-1 and level+1: from Gaussian planes level-1 .. level+2
+__device__ __forceinline__ float dog_at(const float* g, long long off, size_t plane)
+{
+    return __fsub_rn(__ldg(g + off + plane), __ldg(g + off));
+}
+
 __device__ __forceinline__ bool stage2(const DogOct& ov, int level, int x, int y, bool is_max, float& cval)
 {
-    const float* pc = ov.dog + (size_t)level * ov.plane + (size_t)y * ov.pitch + x;
-    const float c = __ldg(pc);
+    const float* pc = ov.gauss + (size_t)level * ov.plane + (size_t)y * ov.pitch + x;       // G[level] at (x, y)
+    const size_t P = ov.plane;
+    const long long pitch = ov.pitch;
+    const float c = dog_at(pc, 0, P);
     cval = c;
     float mx = -INFINITY, mn = INFINITY;
 #pragma unroll
     for (int dz = -1; dz <= 1; dz += 2) {
-        const float* p = dz < 0 ? pc - ov.plane : pc + ov.plane;
-        const float* ra = p - ov.pitch;
-        const float* rb = p + ov.pitch;
-        const float n0 = __ldg(p - 1), n1 = __ldg(p), n2 = __ldg(p + 1);
-        const float n3 = __ldg(ra - 1), n4 = __ldg(ra), n5 = __ldg(ra + 1);
-        const float n6 = __ldg(rb - 1), n7 = __ldg(rb), n8 = __ldg(rb + 1);
+        const float* p = dz < 0 ? pc - P : pc + P;          // G[level-1] (DoG level-1) or G[level+1] (DoG level+1)
+        const float n0 = dog_at(p, -1, P), n1 = dog_at(p, 0, P), n2 = dog_at(p, 1, P);
+        const float n3 = dog_at(p, -pitch - 1, P), n4 = dog_at(p, -pitch, P), n5 = dog_at(p, -pitch + 1, P);
+        const float n6 = dog_at(p, pitch - 1, P), n7 = dog_at(p, pitch, P), n8 = dog_at(p, pitch + 1, P);
         mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(n0, n1), fmaxf(n2, n3)), fmaxf(fmaxf(n4, n5), fmaxf(fmaxf(n6, n7), n8))));
         mn = fminf(mn, fminf(fminf(fminf(n0, n1), fminf(n2, n3)), fminf(fminf(n4, n5), fminf(fminf(n6, n7), n8))));
     }
@@ -377,7 +395,7 @@ __device__ __forceinline__ void stage3(const PyramidView& pyr, const Consts& k, 
     const int o = (int)(q.ol & 0xffu), level = (int)((q.ol >> 8) & 0xffu);
     const OctaveView& ov = pyr.oct[o];
     DogView dv;
-    dv.base = ov.dog; dv.w = ov.w; dv.h = ov.h; dv.pitch = ov.pitch; dv.plane = ov.plane;
+    dv.gauss = ov.gauss; dv.w = ov.w; dv.h = ov.h; dv.pitch = ov.pitch; dv.plane = ov.plane;
     dv.nplanes = pyr.levels + 2;
     InitialExtremum e;
     e.xpos = e.ypos = e.sigma = 0.f; e.lpos = 0;
@@ -407,7 +425,7 @@ cand_extrema_kernel(PyramidView pyr, Consts k, InitialExtremum* __restrict__ iex
     auto octave_view = [&](int o) {
         DogOct d;
         const OctaveView& ov = pyr.oct[o];
-        d.dog = ov.dog; d.w = ov.w; d.h = ov.h; d.pitch = ov.pitch; d.plane = ov.plane; d.nplanes = L + 2;
+        d.gauss = ov.gauss; d.w = ov.w; d.h = ov.h; d.pitch = ov.pitch; d.plane = ov.plane; d.nplanes = L + 2;
         return d;
     };
     // stage 2 on one warp-full (or the remainder) of this warp's queue, survivors -> the block's stage-3 queue

@@ -5,8 +5,10 @@
 // reference src/popsift/s_pyramid_build_ra.cu:17-55, s_pyramid_build_aa.cu:17-86,
 // s_pyramid_build.cu:50-92,547-586) is done here with ONE kernel per level on linear HBM planes:
 //   source tile (+halo, clamp-to-edge) -> shared memory -> row pass -> shared memory ->
-//   column pass in registers -> level l, DoG[l-1] = G[l] - G[l-1] and (for level L) the
-//   2:1 decimated level 0 of the next octave, all written from the same registers.
+//   column pass in registers -> level l and (for level L) the 2:1 decimated level 0 of the
+//   next octave, written from the same registers.  The DoG planes are not written during an
+//   extraction (the extrema stage forms DoG[l-1] = G[l] - G[l-1] where it reads it);
+//   dog_planes_kernel fills them on request.
 //
 // Parity contract (tests/test_gpu_parity.py): every plane is BIT-IDENTICAL to the reference's.
 // That fixes the floating-point evaluation order, taken from the reference's sm_100 SASS:
@@ -86,7 +88,7 @@ __device__ __forceinline__ float col_at(const float* __restrict__ m, int y, int 
 
 template <int R>
 __global__ void __launch_bounds__(NT)
-blur_level_kernel(const float* __restrict__ src, float* __restrict__ dst, float* __restrict__ dog,
+blur_level_kernel(const float* __restrict__ src, float* __restrict__ dst,
                   float* __restrict__ next0, int W, int H, int pitch, int next_pitch, Taps taps)
 {
     extern __shared__ float smem[];
@@ -116,7 +118,6 @@ blur_level_kernel(const float* __restrict__ src, float* __restrict__ dst, float*
         const float v = col_at<R>(m, y, x, taps);
         const size_t o = (size_t)gy * pitch + gx;
         dst[o] = v;
-        dog[o] = __fsub_rn(v, s[(y + R) * SW + x + R]);
         if (next0 != nullptr && !((gx | gy) & 1))
             next0[(size_t)(gy >> 1) * next_pitch + (gx >> 1)] = v;
     }
@@ -124,7 +125,7 @@ blur_level_kernel(const float* __restrict__ src, float* __restrict__ dst, float*
 
 // generic-radius fallback (any span up to 31): same arithmetic, run-time loops
 __global__ void __launch_bounds__(NT)
-blur_level_generic_kernel(const float* __restrict__ src, float* __restrict__ dst, float* __restrict__ dog,
+blur_level_generic_kernel(const float* __restrict__ src, float* __restrict__ dst,
                           float* __restrict__ next0, int W, int H, int pitch, int next_pitch, Taps taps, int R)
 {
     extern __shared__ float smem[];
@@ -166,7 +167,6 @@ blur_level_generic_kernel(const float* __restrict__ src, float* __restrict__ dst
         const float v = __fmaf_rn(p[0], taps.g[0], acc);
         const size_t o = (size_t)gy * pitch + gx;
         dst[o] = v;
-        dog[o] = __fsub_rn(v, s[(y + R) * SW + x + R]);
         if (next0 != nullptr && !((gx | gy) & 1))
             next0[(size_t)(gy >> 1) * next_pitch + (gx >> 1)] = v;
     }
@@ -298,8 +298,8 @@ level0_generic_kernel(const PIX* __restrict__ img, size_t img_pitch, int w, int 
     }
 }
 
-// DoG planes of an octave whose levels were not produced by the fused blur + DoG kernels (reference make_dog,
-// s_pyramid_build.cu:74-92): dog[l] = gauss[l + 1] - gauss[l]
+// DoG planes of an octave on request (ps_debug_plane; reference make_dog, s_pyramid_build.cu:74-92):
+// dog[l] = gauss[l + 1] - gauss[l], the subtraction the extrema stage performs where it reads a DoG sample
 __global__ void dog_planes_kernel(const float* __restrict__ gauss, float* __restrict__ dog, size_t plane, int nplanes, int W, int H, int pitch)
 {
     const size_t n = (size_t)H * pitch;
@@ -329,8 +329,7 @@ int run_blur(const OctaveView& o, int level, const Taps& t, float* next0, int ne
     ensure_smem(blur_level_kernel<R>, tile_smem<R>());
     dim3 grid((o.w + TW - 1) / TW, (o.h + TH - 1) / TH);
     blur_level_kernel<R><<<grid, NT, tile_smem<R>(), st>>>(
-        o.gauss + o.plane * (level - 1), o.gauss + o.plane * level, o.dog + o.plane * (level - 1),
-        next0, o.w, o.h, o.pitch, next_pitch, t);
+        o.gauss + o.plane * (level - 1), o.gauss + o.plane * level, next0, o.w, o.h, o.pitch, next_pitch, t);
     return 1;
 }
 
@@ -490,9 +489,8 @@ int launch_blur_level(const OctaveView& o, int level, const GaussRow& g, const O
     }
     const size_t sm = sizeof(float) * ((TH + 2 * R) * (TW + 2 * R) + (TH + 2 * R) * TW);
     dim3 grid((o.w + TW - 1) / TW, (o.h + TH - 1) / TH);
-    blur_level_generic_kernel<<<grid, NT, sm, st>>>(o.gauss + o.plane * (level - 1), o.gauss + o.plane * level,
-                                                    o.dog + o.plane * (level - 1), next0, o.w, o.h, o.pitch,
-                                                    next_pitch, t, R);
+    blur_level_generic_kernel<<<grid, NT, sm, st>>>(o.gauss + o.plane * (level - 1), o.gauss + o.plane * level, next0,
+                                                    o.w, o.h, o.pitch, next_pitch, t, R);
     return 1;
 }
 

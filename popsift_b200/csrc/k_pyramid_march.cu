@@ -13,8 +13,10 @@
 //      conflict-free LDS.128 (row stride with an odd number of float4 -- the TMA box is that wide) and
 //      produces 16 outputs -> ring buffer HB of row-filtered lines (Q+2R lines);
 //   3. column pass: thread = (pair of adjacent columns, 8 rows); the 8+2R ring lines are loaded once (one
-//      64-bit load per line) and every tap is two FFMAs; the outputs lag the input by R rows: level l, DoG[l-1] (= out - centre
-//      source, still in the staging buffers) and, for level L, the 2:1 decimated level 0 of the next octave.
+//      64-bit load per line) and every tap is two FFMAs; the outputs lag the input by R rows: level l and, for level L, the
+//      2:1 decimated level 0 of the next octave.  Launches that collect candidates also form DoG[l-1] (= out - centre
+//      source, still in the staging buffers) in registers for the threshold test; the DoG plane itself is not stored
+//      (the extrema stage recomputes the same subtraction from G[l] and G[l-1]).
 // Every source row is read from HBM once (+2R warm-up rows per segment), every output written once;
 // the row-filtered intermediate never leaves shared memory.
 //
@@ -51,7 +53,7 @@ struct Geo {
     static constexpr int RP = (R + 3) / 4 * 4;          // halo rounded to float4
     static constexpr int SW = TW + 2 * RP;              // staged columns per row
     static constexpr int SWP = pad_odd4(SW);            // stage row stride
-    // staging buffers: chunk k, chunk k-1 (DoG centre rows) and NBUF-2 chunks in flight.  Two chunks
+    // staging buffers: chunk k, chunk k-1 (DoG centre rows of the candidate test) and NBUF-2 chunks in flight.  Two chunks
     // ahead where four buffers still leave room for 4 CTAs per SM (R <= 8).
     static constexpr int NBUF = (R <= 8) ? 4 : 3;
     static constexpr int AHEAD = NBUF - 2;
@@ -204,13 +206,14 @@ __device__ __forceinline__ f32x2 fma2(f32x2 a, float g, f32x2 c) { return make_f
 
 constexpr int QH = Q / 2;   // output rows per thread in the column pass
 
-// Candidates (CandSink): a lane notes the rows in which one of its two DoG samples passes the peak
-// threshold -- one compare pair and one predicated OR per row in the hot loop -- and afterwards, if it
-// has any, reserves entries of the block's list region with ONE shared-memory atomic and stores them.
-template <int R, bool WRITE_DOG, bool NEXT, bool GUARD, bool CAND>
+// Candidates (CandSink): a lane forms its two DoG samples (output - centre source row) in registers, notes
+// the rows in which one of them passes the peak threshold -- one compare pair and one predicated OR per row
+// in the hot loop -- and afterwards, if it has any, reserves entries of the block's list region with ONE
+// shared-memory atomic and stores them.
+template <int R, bool NEXT, bool GUARD, bool CAND>
 __device__ __forceinline__ void col_emit(const f32x2 (&win)[QH + 2 * R], const float* __restrict__ Scur,
                                          const float* __restrict__ Sprev, int jbase, int y_first, int ys, int ye,
-                                         float* __restrict__ pd, float* __restrict__ pg, float* __restrict__ pn,
+                                         float* __restrict__ pd, float* __restrict__ pn,
                                          int pitch, int next_pitch, const Taps& t, const CandSink& sink, int* cand_n, int x, int W)
 {
     using G = Geo<R>;
@@ -232,22 +235,18 @@ __device__ __forceinline__ void col_emit(const f32x2 (&win)[QH + 2 * R], const f
         if (ok) {
             *reinterpret_cast<f32x2*>(pd) = acc;
             const float a0 = acc.x, a1 = acc.y;
-            if (WRITE_DOG) {
+            if (CAND) {
                 // centre source row: chunk-relative row j-R lives in the current (j >= R) or previous buffer
                 const float* cp = (j >= R) ? Scur + (j - R) * G::SWP : Sprev + (j - R + Q) * G::SWP;
                 const float2 cs = *reinterpret_cast<const float2*>(cp + G::RP + c2);
                 const float g0 = __fsub_rn(a0, cs.x), g1 = __fsub_rn(a1, cs.y);
-                *reinterpret_cast<float2*>(pg) = make_float2(g0, g1);
-                if (CAND) {
-                    // (a pair that straddles the right border may report garbage in its second sample: the
-                    // extrema stage re-tests every sample and ignores border columns)
-                    if (fabsf(g0) >= sink.thr || fabsf(g1) >= sink.thr) pm |= 1u << jj;
-                }
+                // (a pair that straddles the right border may report garbage in its second sample: the
+                // extrema stage re-tests every sample and ignores border columns)
+                if (fabsf(g0) >= sink.thr || fabsf(g1) >= sink.thr) pm |= 1u << jj;
             }
             if (NEXT && ((j & 1) == par)) pn[(size_t)((y_first + j) >> 1) * next_pitch] = a0;
         }
         pd += pitch;
-        if (WRITE_DOG) pg += pitch;
     }
     if (CAND) {
         if (pm != 0u) {
@@ -263,10 +262,10 @@ __device__ __forceinline__ void col_emit(const f32x2 (&win)[QH + 2 * R], const f
     }
 }
 
-template <int R, bool WRITE_DOG, bool NEXT, bool CAND = false>
+template <int R, bool NEXT, bool CAND = false>
 __device__ __forceinline__ void col_pass(const float* __restrict__ HB, const float* __restrict__ Scur,
                                          const float* __restrict__ Sprev, int slot_oldest, int y_first,
-                                         int ys, int ye, int x0, int W, float* __restrict__ dst, float* __restrict__ dog,
+                                         int ys, int ye, int x0, int W, float* __restrict__ dst,
                                          float* __restrict__ next0, int pitch, int next_pitch, const Taps& t,
                                          const CandSink& sink = CandSink(), int* cand_n = nullptr)
 {
@@ -296,18 +295,17 @@ __device__ __forceinline__ void col_pass(const float* __restrict__ HB, const flo
     if (yb + QH <= ys || yb >= ye) return;                     // nothing of this half-block is inside the segment (warp-uniform)
     const long long o = (long long)yb * pitch + x;             // may point outside for guarded samples (never dereferenced)
     float* pd = dst + o;
-    float* pg = WRITE_DOG ? dog + o : nullptr;
     float* pn = NEXT ? next0 + (x >> 1) : nullptr;
     if (yb >= ys && yb + QH <= ye && x0 + TW <= W)
-        col_emit<R, WRITE_DOG, NEXT, false, CAND>(win, Scur, Sprev, jbase, y_first, ys, ye, pd, pg, pn, pitch, next_pitch, t, sink, cand_n, x, W);
+        col_emit<R, NEXT, false, CAND>(win, Scur, Sprev, jbase, y_first, ys, ye, pd, pn, pitch, next_pitch, t, sink, cand_n, x, W);
     else
-        col_emit<R, WRITE_DOG, NEXT, true, CAND>(win, Scur, Sprev, jbase, y_first, ys, ye, pd, pg, pn, pitch, next_pitch, t, sink, cand_n, x, W);
+        col_emit<R, NEXT, true, CAND>(win, Scur, Sprev, jbase, y_first, ys, ye, pd, pn, pitch, next_pitch, t, sink, cand_n, x, W);
 }
 
 template <int R, bool EDGE, bool NEXT, bool CAND>
 __device__ __forceinline__ void march_body(float* __restrict__ smem, uint64_t* __restrict__ full, const CUtensorMap* map,
                                            const float* __restrict__ src, float* __restrict__ dst,
-                                           float* __restrict__ dog, float* __restrict__ next0, int W, int H, int pitch,
+                                           float* __restrict__ next0, int W, int H, int pitch,
                                            int next_pitch, int x0, int ys, int ye, const Taps& taps, const CandSink& sink,
                                            int* cand_n)
 {
@@ -343,8 +341,8 @@ __device__ __forceinline__ void march_body(float* __restrict__ smem, uint64_t* _
         __syncthreads();
         int slot_old = slot_in + Q;       // oldest line = the one after the newest
         if (slot_old >= G::RING) slot_old -= G::RING;
-        col_pass<R, true, NEXT, CAND>(HB, Scur, Sprev, slot_old, ys - 2 * R + k * Q, ys, ye, x0, W, dst, dog, next0, pitch,
-                                      next_pitch, taps, sink, cand_n);
+        col_pass<R, NEXT, CAND>(HB, Scur, Sprev, slot_old, ys - 2 * R + k * Q, ys, ye, x0, W, dst, next0, pitch,
+                                next_pitch, taps, sink, cand_n);
         slot_in = slot_old;
         if (cur == G::NBUF - 1) { cur = 0; parity ^= 1u; } else ++cur;
     }
@@ -355,7 +353,7 @@ __device__ __forceinline__ void march_body(float* __restrict__ smem, uint64_t* _
 template <int R, bool NEXT, bool CAND>
 __global__ void __launch_bounds__(NT, 4)
 march_level_kernel(const __grid_constant__ CUtensorMap tmap, const float* __restrict__ src, float* __restrict__ dst,
-                   float* __restrict__ dog, float* __restrict__ next0, int W, int H, int pitch, int next_pitch, Partition part,
+                   float* __restrict__ next0, int W, int H, int pitch, int next_pitch, Partition part,
                    Taps taps, CandSink sink)
 {
     using G = Geo<R>;
@@ -378,8 +376,8 @@ march_level_kernel(const __grid_constant__ CUtensorMap tmap, const float* __rest
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     __syncthreads();
-    if (!edge) march_body<R, false, NEXT, CAND>(smem, full, &tmap, src, dst, dog, next0, W, H, pitch, next_pitch, x0, ys, ye, taps, sink, &s_cand_n);
-    else       march_body<R, true, NEXT, CAND>(smem, full, &tmap, src, dst, dog, next0, W, H, pitch, next_pitch, x0, ys, ye, taps, sink, &s_cand_n);
+    if (!edge) march_body<R, false, NEXT, CAND>(smem, full, &tmap, src, dst, next0, W, H, pitch, next_pitch, x0, ys, ye, taps, sink, &s_cand_n);
+    else       march_body<R, true, NEXT, CAND>(smem, full, &tmap, src, dst, next0, W, H, pitch, next_pitch, x0, ys, ye, taps, sink, &s_cand_n);
 }
 
 // ---- octave 0, level 0 from the input image -----------------------------------------------------
@@ -452,7 +450,7 @@ __device__ __forceinline__ void level0_body(float* __restrict__ smem, AxisTap* _
         }
         int slot_old = slot_in + Q;
         if (slot_old >= G::RING) slot_old -= G::RING;
-        col_pass<R, false, false>(HB, Scur, Scur, slot_old, ys - 2 * R + k * Q, ys, ye, x0, W, dst, nullptr, nullptr, pitch, 0, inc0);
+        col_pass<R, false>(HB, Scur, Scur, slot_old, ys - 2 * R + k * Q, ys, ye, x0, W, dst, nullptr, pitch, 0, inc0);
         slot_in = slot_old;
         __syncthreads();
     }
@@ -585,7 +583,7 @@ march_level0x2_kernel(const uint8_t* __restrict__ img, size_t img_pitch, int w, 
         __syncthreads();                                  // ring lines of chunk k written; tile k+1 visible
         int slot_old = slot_in + Q;
         if (slot_old >= G::RING) slot_old -= G::RING;
-        col_pass<R, false, false>(HB, S, S, slot_old, ys - 2 * R + k * Q, ys, ye, x0, W, dst, nullptr, nullptr, pitch, 0, inc0);
+        col_pass<R, false>(HB, S, S, slot_old, ys - 2 * R + k * Q, ys, ye, x0, W, dst, nullptr, pitch, 0, inc0);
         slot_in = slot_old;
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -622,7 +620,7 @@ bool pdl_choice()
 }
 
 template <int R, bool NEXT, bool CAND>
-int launch_march(const Partition& part, const float* src, float* dst, float* dog, float* next0, const OctaveView& o,
+int launch_march(const Partition& part, const float* src, float* dst, float* next0, const OctaveView& o,
                  int next_pitch, const Taps& t, const CandSink& sink, cudaStream_t st)
 {
     ensure_smem(march_level_kernel<R, NEXT, CAND>, Geo<R>::smem, true);
@@ -636,7 +634,7 @@ int launch_march(const Partition& part, const float* src, float* dst, float* dog
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = pdl_choice() ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, march_level_kernel<R, NEXT, CAND>, map, src, dst, dog, next0, o.w, o.h, o.pitch, next_pitch,
+    return cudaLaunchKernelEx(&cfg, march_level_kernel<R, NEXT, CAND>, map, src, dst, next0, o.w, o.h, o.pitch, next_pitch,
                               part, t, sink) == cudaSuccess ? 1 : -2;
 }
 
@@ -646,13 +644,12 @@ int run_march(const OctaveView& o, int level, const Taps& t, float* next0, int n
     const Partition part = make_partition(o.w, o.h);
     const float* src = o.gauss + o.plane * (level - 1);
     float* dst = o.gauss + o.plane * level;
-    float* dog = o.dog + o.plane * (level - 1);
     const bool cand = sink && sink->list && o.w <= 65535 && o.h <= 65535 && sink->region == cand_region_cap(part, TW, Q);
     const CandSink cs = cand ? *sink : CandSink();
-    if (next0) return cand ? launch_march<R, true, true>(part, src, dst, dog, next0, o, next_pitch, t, cs, st)
-                           : launch_march<R, true, false>(part, src, dst, dog, next0, o, next_pitch, t, cs, st);
-    return cand ? launch_march<R, false, true>(part, src, dst, dog, next0, o, next_pitch, t, cs, st)
-                : launch_march<R, false, false>(part, src, dst, dog, next0, o, next_pitch, t, cs, st);
+    if (next0) return cand ? launch_march<R, true, true>(part, src, dst, next0, o, next_pitch, t, cs, st)
+                           : launch_march<R, true, false>(part, src, dst, next0, o, next_pitch, t, cs, st);
+    return cand ? launch_march<R, false, true>(part, src, dst, next0, o, next_pitch, t, cs, st)
+                : launch_march<R, false, false>(part, src, dst, next0, o, next_pitch, t, cs, st);
 }
 
 template <int R, typename PIX>

@@ -243,15 +243,14 @@ int run_pyramid(ps_ctx* ctx, Slot& s)
                 }
                 for (int l = 1; l < L + 3; ++l) n += launch_fixed_levelN(ov, l, ctx->absn[l], S, s.d_interm, s.stream);
             }
-            n += launch_dog_planes(ov, L + 2, s.stream);
         }
         ctx->launches += n;
         PS_CUDA(ctx, cudaGetLastError());
         return PS_OK;
     }
     // --gauss-mode relative / vlfeat-hw-interpolated (VLFeat_Relative, s_pyramid_build.cu:515-542): every pass merges pairs of
-    // taps into interpolated fetches; simple per-pixel kernels (k_pyramid.cu), DoG and decimation by their own kernels, dense
-    // extrema scan.
+    // taps into interpolated fetches; simple per-pixel kernels (k_pyramid.cu), decimation by its own kernel, dense extrema
+    // scan.
     if (ctx->cfg.gauss_mode == PS_GAUSS_VLFEAT_RELATIVE) {
         s.view.cands_filled = 0;
         for (int o = 0; o < s.num_octaves; ++o) {
@@ -274,7 +273,6 @@ int run_pyramid(ps_ctx* ctx, Slot& s)
                 n += launch_interp_pass(ov.gauss + ov.plane * (l - 1), s.d_interm, ov.w, ov.h, ov.pitch, ctx->irows[l], ctx->irows[l].span, 1, s.stream);
                 n += launch_interp_pass(s.d_interm, ov.gauss + ov.plane * l, ov.w, ov.h, ov.pitch, ctx->irows[l], ctx->irows[l].span, 0, s.stream);
             }
-            n += launch_dog_planes(ov, L + 2, s.stream);
         }
         ctx->launches += n;
         PS_CUDA(ctx, cudaGetLastError());
@@ -298,7 +296,6 @@ int run_pyramid(ps_ctx* ctx, Slot& s)
             if (r < 0) return ctx->fail(PS_ERR_ARG, "unsupported filter span %d (octave 0, level %d)", ctx->abs0[l].span, l);
             n += r;
         }
-        n += launch_dog_planes(s.view.oct[0], L + 2, s.stream);
         if (s.num_octaves > 1) n += launch_decimate(s.view.oct[0], L, s.view.oct[1], s.stream);
     } else {
     if (s.is_float)
@@ -1260,9 +1257,15 @@ extern "C" int ps_debug_plane(ps_ctx* ctx, int slot, int octave, int level, int 
     PS_CUDA(ctx, cudaSetDevice(ctx->device));
     PS_CUDA(ctx, cudaStreamSynchronize(s->stream));
     const OctaveView& v = s->view.oct[octave];
+    // an extraction writes no DoG plane (OctaveView::dog): the octave's planes are formed from its Gaussian levels here
+    if (which == PS_PLANE_DOG) {
+        ctx->launches += launch_dog_planes(v, L + 2, s->stream);
+        PS_CUDA(ctx, cudaGetLastError());
+    }
     const float* src = (which == PS_PLANE_DOG ? v.dog : v.gauss) + v.plane * level;
-    PS_CUDA(ctx, cudaMemcpy2D(out, (size_t)v.w * sizeof(float), src, (size_t)v.pitch * sizeof(float),
-                              (size_t)v.w * sizeof(float), v.h, cudaMemcpyDeviceToHost));
+    PS_CUDA(ctx, cudaMemcpy2DAsync(out, (size_t)v.w * sizeof(float), src, (size_t)v.pitch * sizeof(float),
+                                   (size_t)v.w * sizeof(float), v.h, cudaMemcpyDeviceToHost, s->stream));
+    PS_CUDA(ctx, cudaStreamSynchronize(s->stream));
     return PS_OK;
 }
 

@@ -45,7 +45,10 @@ struct FilterPlan {
 // One octave's planes in HBM: linear float32, row pitch a multiple of 32 floats (128 B).
 struct OctaveView {
     float* gauss;       // (levels+3) planes, plane stride = plane
-    float* dog;         // (levels+2) planes
+    // (levels+2) planes, DoG[l] = G[l+1] - G[l].  Written only on request (ps_debug_plane -> launch_dog_planes): during an
+    // extraction nothing writes or reads this region; the extrema stage forms every DoG sample it needs from the two
+    // Gaussian planes with the same __fsub_rn, so the region may hold anything (e.g. an earlier image's planes).
+    float* dog;
     // candidate lists of the `levels` scanned DoG planes (see CandSink): level q (DoG plane q+1), block b of
     // the level kernel owns entries [(q*cand_blocks + b) * cand_region, +cand_cnt[q*cand_blocks + b])
     uint32_t* cand;
@@ -70,7 +73,7 @@ struct PyramidView {
 };
 
 // Where a pyramid kernel reports the DoG pixel pairs (x even) in which a sample passes the peak
-// threshold while it writes the DoG plane: the extrema stage then only visits those (a few per thousand
+// threshold while it writes Gaussian level l (DoG[l-1] = G[l] - G[l-1] in registers): the extrema stage then only visits those (a few per thousand
 // pixels) instead of scanning every plane again.  Each block of the kernel owns a private region of the
 // list and a count (zeroed per image), so the kernel needs a shared-memory counter but no global atomic.
 struct CandSink {
@@ -121,12 +124,13 @@ int launch_level0_u8(const uint8_t* img, size_t img_pitch, int w, int h, float u
                      const OctaveView& o0, const GaussRow& dd, const GaussRow& inc0, cudaStream_t st, int octave = 0);
 int launch_level0_f32(const float* img, size_t img_pitch_floats, int w, int h, float upscale, int sift_mode,
                       const OctaveView& o0, const GaussRow& dd, const GaussRow& inc0, cudaStream_t st, int octave = 0);
-// --gauss-mode vlfeat-direct (VLFeat_Relative_All): one level of octave 0 straight from the input image; the DoG planes and
-// the next octave's level 0 then come from their own small kernels
+// --gauss-mode vlfeat-direct (VLFeat_Relative_All): one level of octave 0 straight from the input image; the next
+// octave's level 0 then comes from its own small kernel
 int launch_level0_abs_u8(const uint8_t* img, size_t img_pitch, int w, int h, float upscale, int sift_mode,
                          const OctaveView& o0, int level, const GaussRow& taps, cudaStream_t st);
 int launch_level0_abs_f32(const float* img, size_t img_pitch_floats, int w, int h, float upscale, int sift_mode,
                           const OctaveView& o0, int level, const GaussRow& taps, cudaStream_t st);
+// DoG planes 0 .. nplanes-1 of one octave from its Gaussian planes (on request only: see OctaveView::dog)
 int launch_dog_planes(const OctaveView& o, int nplanes, cudaStream_t st);
 // --gauss-mode relative (VLFeat_Relative): the first horizontal pass alone, and one interpolated pass over a plane
 int launch_level0_rows_u8(const uint8_t* img, size_t img_pitch, int w, int h, float upscale, int sift_mode,
@@ -141,7 +145,7 @@ int launch_fixed_level0_f32(const float* img, size_t img_pitch_floats, int w, in
 int launch_fixed_levelN(const OctaveView& o, int level, const GaussRow& taps, int S, float* scratch, cudaStream_t st);
 int launch_interp_pass(const float* src, float* dst, int W, int H, int pitch, const GaussRow& f, int ispan, int along_x, cudaStream_t st);
 int launch_decimate(const OctaveView& prev, int level, const OctaveView& next, cudaStream_t st);
-// level l >= 1 of one octave: blur level l-1 -> level l, DoG[l-1] = G[l]-G[l-1]; if next0 != nullptr
+// level l >= 1 of one octave: blur level l-1 -> level l (no DoG plane is written); if next0 != nullptr
 // also writes every second pixel into the next octave's level 0.
 // `sink` (optional) receives the threshold-passing samples of the DoG plane; only honoured when
 // blur_level_collects(g) is true.
