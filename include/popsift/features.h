@@ -168,4 +168,25 @@ std::vector<std::vector<int>> matchPairsGuided(const std::vector<FeaturesDev*>& 
 std::vector<std::vector<int>> matchPairsGuidedU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
                                                  const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags = 0);
 
+/// Codebook settings of vladCodebook (same rules as ps_vlad_train in popsift_b200_retrieval.h).
+struct VladParams
+{
+    int                k = 64;       // centroids, 1 .. 1024 (at most the pooled descriptor count)
+    int                iters = 10;   // k-means iterations, 0 .. 1000 (fixed; no convergence test)
+    unsigned long long seed = 0;     // initial draw
+};
+
+/// k-means codebook of the pooled descriptors of `sets` (an addition to the reference's interface; C ABI ps_vlad_train):
+/// k x 128 floats, row-major.  flags as for matchPairs (the assignment is its nearest-neighbour search).  Throws like
+/// matchPairs, and for parameters ps_vlad_train refuses.
+std::vector<float> vladCodebook(const std::vector<FeaturesDev*>& sets, const VladParams& params = VladParams(), int flags = 0);
+
+/// VLAD vectors of `sets` under `codebook` (k x 128 floats; C ABI ps_vlad_encode): sets.size() rows of k * 128 floats.
+std::vector<float> vladEncode(const std::vector<FeaturesDev*>& sets, const std::vector<float>& codebook, int flags = 0);
+
+/// The pair list of image retrieval (C ABI ps_retrieve_pairs): `vectors` holds n rows of vectors.size() / n floats (a
+/// multiple of 4, e.g. vladEncode's output); every row's m best neighbours under the inner product are taken, and the
+/// result is the union of the unordered pairs (i, j), i < j, sorted.
+std::vector<std::pair<int, int>> retrievePairs(const std::vector<float>& vectors, int n, int m);
+
 } // namespace popsift

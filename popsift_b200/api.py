@@ -79,6 +79,8 @@ EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps
            "ps_debug_level0_plan", "ps_format_gauss_tables", "ps_match_correspondences", "ps_verify_batch"]
 # guided matching, declared in popsift_b200_guided.h (same library)
 GUIDED_EXPORTS = ["ps_match_guided_batch", "ps_match_u8_guided_batch"]
+# image retrieval, declared in popsift_b200_retrieval.h (same library)
+RETRIEVAL_EXPORTS = ["ps_vlad_train", "ps_vlad_encode", "ps_retrieve_pairs"]
 
 _lib = None
 
@@ -126,6 +128,10 @@ def load_library():
         for name in GUIDED_EXPORTS:
             getattr(L, name).argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                          C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_int]
+    if hasattr(L, "ps_vlad_train"):
+        L.ps_vlad_train.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_int]
+        L.ps_vlad_encode.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+        L.ps_retrieve_pairs.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -869,6 +875,89 @@ def match_pairs_guided(sets, pairs, models, model="homography", threshold=4.0, f
         bufs.free()
     starts = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
     return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
+
+
+def _desc_sets(lib, bufs, sets):
+    """device pointers and counts of FeaturesDev objects or host (n, 128) float32 arrays (uploaded into bufs)"""
+    ptrs, counts = [], []
+    for s in sets:
+        if isinstance(s, FeaturesDev):
+            ptrs.append(s.getDescriptors()); counts.append(s.getDescriptorCount())
+            continue
+        a = np.ascontiguousarray(s, np.float32).reshape(-1, 128)
+        ptrs.append(bufs.upload(a)); counts.append(len(a))
+    n = max(len(sets), 1)
+    return (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*counts), counts
+
+
+def vlad_codebook(sets, k=64, iters=10, seed=0, flags=0, device=None) -> np.ndarray:
+    """k-means codebook of the pooled descriptors of `sets` (C ABI ps_vlad_train in popsift_b200_retrieval.h; an addition
+    to the reference's interface): FeaturesDev objects or host (n, 128) float32 arrays.  Returns (k, 128) float32."""
+    lib = load_library()
+    bufs = _DevBuffers(lib)
+    try:
+        device = _first_device(lib, sets) if device is None else device
+        c_sets, c_n, _ = _desc_sets(lib, bufs, sets)
+        d_c = bufs.alloc(k * 512)
+        rc = lib.ps_vlad_train(device, len(sets), c_sets, c_n, int(k), int(iters), int(seed) & ((1 << 64) - 1), d_c, flags)
+        if rc != 0:
+            raise PopSiftError("ps_vlad_train error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        return bufs.download(d_c, (k, 128), np.float32)
+    finally:
+        bufs.free()
+
+
+def vlad_encode(sets, codebook, flags=0, assign=False, device=None):
+    """VLAD vectors of `sets` under `codebook` ((k, 128) float32) (C ABI ps_vlad_encode): (n_sets, 128 k) float32, rows
+    intra-normalised, signed-square-rooted and L2-normalised.  assign=True also returns the (N,) int32 centroid of every
+    pooled descriptor (its visual word)."""
+    lib = load_library()
+    cb = np.ascontiguousarray(codebook, np.float32).reshape(-1, 128)
+    k = len(cb)
+    bufs = _DevBuffers(lib)
+    try:
+        device = _first_device(lib, sets) if device is None else device
+        c_sets, c_n, counts = _desc_sets(lib, bufs, sets)
+        N = sum(counts)
+        d_v = bufs.alloc(len(sets) * k * 512)
+        d_a = bufs.alloc(N * 4) if assign else None
+        rc = lib.ps_vlad_encode(device, len(sets), c_sets, c_n, k, bufs.upload(cb), d_v, d_a, flags)
+        if rc != 0:
+            raise PopSiftError("ps_vlad_encode error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        v = bufs.download(d_v, (len(sets), k * 128), np.float32)
+        return (v, bufs.download(d_a, N, np.int32)) if assign else v
+    finally:
+        bufs.free()
+
+
+def retrieve(vectors, m, device=0):
+    """Each row's m nearest rows under the inner product (C ABI ps_retrieve_pairs): `vectors` is (n, dim) float32 with dim
+    a multiple of 4.  Returns (nbr (n, m) int32, score (n, m) float32), best first; empty slots hold -1 and -inf."""
+    lib = load_library()
+    v = np.ascontiguousarray(vectors, np.float32)
+    n, dim = v.shape
+    bufs = _DevBuffers(lib)
+    try:
+        d_n, d_s = bufs.alloc(n * m * 4), bufs.alloc(n * m * 4)
+        rc = lib.ps_retrieve_pairs(device, n, bufs.upload(v), dim, int(m), d_n, d_s)
+        if rc != 0:
+            raise PopSiftError("ps_retrieve_pairs error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        return bufs.download(d_n, (n, m), np.int32), bufs.download(d_s, (n, m), np.float32)
+    finally:
+        bufs.free()
+
+
+def select_pairs(nbr) -> list:
+    """The unordered pairs (i, j), i < j, of the union of every row's neighbours in `nbr` (retrieve's first output),
+    sorted; -1 slots are dropped.  The pair list for match_pairs / verify_pairs."""
+    nbr = np.asarray(nbr)
+    out = set()
+    for i, row in enumerate(nbr):
+        for j in row:
+            j = int(j)
+            if j >= 0 and j != i:
+                out.add((min(i, j), max(i, j)))
+    return sorted(out)
 
 
 def keypoints_array(keypoints) -> np.ndarray:

@@ -26,7 +26,7 @@ NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "--fmad=false",   # no implicit contraction anywhere; every fma in the kernels is explicit
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu",
+LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu", "k_retrieval.cu",
                "host/sift_conf.cpp", "host/features.cpp", "host/popsift.cpp", "host/device_prop.cpp", "host/log_dump.cpp"]
 DEMO_SOURCES = ["app/popsift_demo.cpp", "app/pgmread.cpp"]
 MATCH_SOURCES = ["app/popsift_match.cpp"]            # + app/pgmread.cpp
@@ -57,6 +57,10 @@ GUIDED_MASK = os.path.join(BIN_DIR, "guided_mask")
 GUIDED_MASK_SRC = os.path.join(ROOT, "tests", "cpp", "guided_mask.cpp")
 GUIDED_CHECK = os.path.join(BIN_DIR, "guided_check")
 GUIDED_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "guided_check.cpp")
+RETRIEVAL_HOST = os.path.join(BIN_DIR, "retrieval_host")
+RETRIEVAL_HOST_SRC = os.path.join(ROOT, "tests", "cpp", "retrieval_host.cpp")
+RETRIEVAL_CHECK = os.path.join(BIN_DIR, "retrieval_check")
+RETRIEVAL_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "retrieval_check.cpp")
 
 
 def _newer(target: str, deps) -> bool:
@@ -161,6 +165,15 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if os.path.exists(GUIDED_CHECK_SRC) and (force or _newer(GUIDED_CHECK, [GUIDED_CHECK_SRC, LIB] + hdrs)):
         # popsift::matchPairsGuided(U8) against the C ABI (ps_match_guided_batch / ps_match_u8_guided_batch)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), GUIDED_CHECK_SRC, "-o", GUIDED_CHECK,
+                               "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
+    retr_hdrs = [os.path.join(CSRC, "k_retrieval.h"), sample_hdr]
+    if os.path.exists(RETRIEVAL_HOST_SRC) and (force or _newer(RETRIEVAL_HOST, [RETRIEVAL_HOST_SRC] + retr_hdrs)):
+        # host-only: retrieval's initial draw and score chain, the same __host__ __device__ functions the kernels use (no
+        # CUDA, no library); no contraction, so that every rounding is the one the functions spell out
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-I" + CSRC, RETRIEVAL_HOST_SRC, "-o", RETRIEVAL_HOST])
+    if os.path.exists(RETRIEVAL_CHECK_SRC) and (force or _newer(RETRIEVAL_CHECK, [RETRIEVAL_CHECK_SRC, LIB] + hdrs)):
+        # popsift::vladCodebook / vladEncode / retrievePairs against the C ABI (popsift_b200_retrieval.h)
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), RETRIEVAL_CHECK_SRC, "-o", RETRIEVAL_CHECK,
                                "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
     pgm_src = os.path.join(CSRC, "app", "pgmread.cpp")
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):

@@ -5,6 +5,7 @@
 #include "pinned_pool.h"
 #include "popsift_b200.h"
 #include "popsift_b200_guided.h"
+#include "popsift_b200_retrieval.h"
 
 #include <algorithm>
 #include <cmath>
@@ -418,6 +419,98 @@ std::ostream& operator<<(std::ostream& ostr, const Feature& f)
 {
     f.print(ostr, false);
     return ostr;
+}
+
+namespace {
+
+// the device pointers and counts of FeaturesDev sets, and the device of the first non-empty one
+int vlad_sets(const char* fn, const std::vector<FeaturesDev*>& sets, std::vector<const ps_descriptor*>& d_sets, std::vector<int32_t>& n_desc)
+{
+    d_sets.resize(sets.size());
+    n_desc.resize(sets.size());
+    int dev = -1;
+    for (size_t i = 0; i < sets.size(); ++i) {
+        if (!sets[i]) throw std::runtime_error(std::string(fn) + ": null set");
+        d_sets[i] = reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors());
+        n_desc[i] = sets[i]->getDescriptorCount();
+        if (dev < 0 && n_desc[i] > 0) dev = std::max(0, ps_pointer_device(d_sets[i]));
+    }
+    return std::max(dev, 0);
+}
+
+// a device buffer freed at scope exit
+struct DevBuf {
+    void* p;
+    explicit DevBuf(size_t bytes, const char* fn) : p(ps_dev_alloc(std::max<size_t>(bytes, 16)))
+    {
+        if (!p) throw std::runtime_error(std::string(fn) + ": failed to allocate device memory");
+    }
+    ~DevBuf() { ps_dev_free(p); }
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+};
+
+void check(int rc, const char* fn, const char* entry)
+{
+    if (rc != PS_OK) throw std::runtime_error(std::string(fn) + ": " + entry + " failed: " + ps_last_error(nullptr));
+}
+
+} // namespace
+
+std::vector<float> vladCodebook(const std::vector<FeaturesDev*>& sets, const VladParams& params, int flags)
+{
+    const char* fn = "popsift::vladCodebook";
+    std::vector<const ps_descriptor*> d_sets;
+    std::vector<int32_t> n_desc;
+    const int dev = vlad_sets(fn, sets, d_sets, n_desc);
+    const int k = std::max(params.k, 0);
+    DevBuf c((size_t)k * 128 * sizeof(float), fn);
+    check(ps_vlad_train(dev, (int)sets.size(), d_sets.data(), n_desc.data(), params.k, params.iters, params.seed,
+                        static_cast<float*>(c.p), flags), fn, "ps_vlad_train");
+    std::vector<float> out((size_t)k * 128);
+    check(ps_dev_to_host(out.data(), c.p, out.size() * sizeof(float)), fn, "ps_dev_to_host");
+    return out;
+}
+
+std::vector<float> vladEncode(const std::vector<FeaturesDev*>& sets, const std::vector<float>& codebook, int flags)
+{
+    const char* fn = "popsift::vladEncode";
+    if (codebook.empty() || codebook.size() % 128) throw std::runtime_error(std::string(fn) + ": the codebook is not k x 128 floats");
+    std::vector<const ps_descriptor*> d_sets;
+    std::vector<int32_t> n_desc;
+    const int dev = vlad_sets(fn, sets, d_sets, n_desc);
+    const int k = (int)(codebook.size() / 128);
+    std::vector<float> out(sets.size() * codebook.size());
+    if (sets.empty()) return out;
+    DevBuf c(codebook.size() * sizeof(float), fn), v(out.size() * sizeof(float), fn);
+    check(ps_host_to_dev(c.p, codebook.data(), codebook.size() * sizeof(float)), fn, "ps_host_to_dev");
+    check(ps_vlad_encode(dev, (int)sets.size(), d_sets.data(), n_desc.data(), k, static_cast<const float*>(c.p),
+                         static_cast<float*>(v.p), nullptr, flags), fn, "ps_vlad_encode");
+    check(ps_dev_to_host(out.data(), v.p, out.size() * sizeof(float)), fn, "ps_dev_to_host");
+    return out;
+}
+
+std::vector<std::pair<int, int>> retrievePairs(const std::vector<float>& vectors, int n, int m)
+{
+    const char* fn = "popsift::retrievePairs";
+    if (n < 0 || (n > 0 && vectors.size() % (size_t)n)) throw std::runtime_error(std::string(fn) + ": vectors.size() is not a multiple of n");
+    std::vector<std::pair<int, int>> out;
+    if (n == 0) return out;
+    const int dim = (int)(vectors.size() / n);
+    DevBuf v(vectors.size() * sizeof(float), fn), nb((size_t)n * std::max(m, 1) * sizeof(int32_t), fn), sc((size_t)n * std::max(m, 1) * sizeof(float), fn);
+    check(ps_host_to_dev(v.p, vectors.data(), vectors.size() * sizeof(float)), fn, "ps_host_to_dev");
+    check(ps_retrieve_pairs(0 <= ps_pointer_device(v.p) ? ps_pointer_device(v.p) : 0, n, static_cast<const float*>(v.p), dim, m,
+                            static_cast<int32_t*>(nb.p), static_cast<float*>(sc.p)), fn, "ps_retrieve_pairs");
+    std::vector<int32_t> nbr((size_t)n * m);
+    check(ps_dev_to_host(nbr.data(), nb.p, nbr.size() * sizeof(int32_t)), fn, "ps_dev_to_host");
+    for (int i = 0; i < n; ++i)
+        for (int q = 0; q < m; ++q) {
+            const int j = nbr[(size_t)i * m + q];
+            if (j >= 0 && j != i) out.push_back({std::min(i, j), std::max(i, j)});
+        }
+    std::sort(out.begin(), out.end());
+    out.erase(std::unique(out.begin(), out.end()), out.end());
+    return out;
 }
 
 } // namespace popsift

@@ -9,6 +9,7 @@
 // There is no intermediate (row-filtered) plane in HBM: the row pass lives in shared memory.
 #include "ps_internal.h"
 #include "popsift_b200_guided.h"
+#include "popsift_b200_retrieval.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1235,6 +1236,71 @@ extern "C" int ps_match_u8_guided_batch(int device, int n_sets, const uint8_t* c
 {
     return match_guided("ps_match_u8_guided_batch", true, device, n_sets, reinterpret_cast<const void* const*>(d_sets), d_feat, d_rev,
                         n_desc, n_pairs, pairs, d_models, model, threshold, d_out, flags);
+}
+
+// the set checks of ps_match_batch and the codebook size, for both VLAD entry points; *N = the pool size
+static int vlad_sets(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc, int k, int64_t* N)
+{
+    if (n_sets < 0 || (n_sets > 0 && (!d_sets || !n_desc)) || k < 1 || k > 1024) return PS_ERR_ARG;
+    *N = 0;
+    for (int i = 0; i < n_sets; ++i) {
+        if (n_desc[i] < 0) return PS_ERR_ARG;
+        if (n_desc[i] > 0 && (!d_sets[i] || ps_pointer_device(d_sets[i]) != device)) return PS_ERR_ARG;
+        *N += n_desc[i];
+    }
+    return PS_OK;
+}
+
+extern "C" int ps_vlad_train(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc, int k, int iters,
+                             uint64_t seed, float* d_centroids, int flags)
+{
+    if (n_sets < 0 || k < 1 || k > 1024 || iters < 0 || iters > 1000) return PS_ERR_ARG;
+    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    int64_t N = 0;
+    if (vlad_sets(device, n_sets, d_sets, n_desc, k, &N) != PS_OK) return PS_ERR_ARG;
+    if (N < k || N >= 0x80000000LL) return PS_ERR_ARG;
+    if (ps_pointer_device(d_centroids) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    const int n = run_vlad_train(d_sets, n_desc, n_sets, k, iters, seed, d_centroids, flags, nullptr, &err);
+    if (n < 0) { g_create_error = err ? err : "ps_vlad_train failed"; return PS_ERR_CUDA; }
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string("ps_vlad_train: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
+}
+
+extern "C" int ps_vlad_encode(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc, int k,
+                              const float* d_centroids, float* d_vlad, int32_t* d_assign, int flags)
+{
+    if (n_sets < 0 || k < 1 || k > 1024) return PS_ERR_ARG;
+    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    int64_t N = 0;
+    if (vlad_sets(device, n_sets, d_sets, n_desc, k, &N) != PS_OK) return PS_ERR_ARG;
+    if (n_sets == 0) return PS_OK;
+    if (N >= 0x80000000LL) return PS_ERR_ARG;
+    if (ps_pointer_device(d_centroids) != device || ps_pointer_device(d_vlad) != device) return PS_ERR_ARG;
+    if (d_assign && N > 0 && ps_pointer_device(d_assign) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    const int n = run_vlad_encode(d_sets, n_desc, n_sets, k, d_centroids, d_vlad, d_assign, flags, nullptr, &err);
+    if (n < 0) { g_create_error = err ? err : "ps_vlad_encode failed"; return PS_ERR_CUDA; }
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string("ps_vlad_encode: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
+}
+
+extern "C" int ps_retrieve_pairs(int device, int n, const float* d_vec, int dim, int m, int32_t* d_nbr, float* d_score)
+{
+    if (n < 0 || dim <= 0 || (dim & 3) || m < 1 || m > 128) return PS_ERR_ARG;
+    if (n == 0) return PS_OK;
+    if ((int64_t)n * m >= 0x80000000LL) return PS_ERR_ARG;
+    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (reinterpret_cast<uintptr_t>(d_vec) & 15u) return PS_ERR_ARG;
+    if (ps_pointer_device(d_vec) != device || ps_pointer_device(d_nbr) != device || ps_pointer_device(d_score) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    const int r = run_retrieve_pairs(n, d_vec, dim, m, d_nbr, d_score, nullptr, &err);
+    if (r < 0) { g_create_error = err ? err : "ps_retrieve_pairs failed"; return PS_ERR_CUDA; }
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string("ps_retrieve_pairs: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
 }
 
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)

@@ -240,4 +240,12 @@ int run_match_u8_guided_batch(const uint8_t* const* sets, const ps_feature* cons
                               const int32_t* n_desc, int n_sets, const int32_t* pairs, int n_pairs, const float* models, int model,
                               float threshold, int32_t* out, int flags, cudaStream_t st, const char** err);
 
+// image retrieval (include/popsift_b200_retrieval.h, k_retrieval.cu), arguments already validated; asynchronous on `st`,
+// return the number of kernels launched or -1 (*err set).  Assignment is run_match_batch against the centroids.
+int run_vlad_train(const ps_descriptor* const* sets, const int32_t* n_desc, int n_sets, int k, int iters, uint64_t seed,
+                   float* centroids, int flags, cudaStream_t st, const char** err);
+int run_vlad_encode(const ps_descriptor* const* sets, const int32_t* n_desc, int n_sets, int k, const float* centroids,
+                    float* vlad, int32_t* assign, int flags, cudaStream_t st, const char** err);
+int run_retrieve_pairs(int n, const float* vec, int dim, int m, int32_t* nbr, float* score, cudaStream_t st, const char** err);
+
 } // namespace psb

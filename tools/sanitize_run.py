@@ -112,3 +112,14 @@ if only in ("all", "verify"):
         res, taps = api.verify_correspondences(corrs, model=model, n_samples=200, threshold=2.0, taps=True)
         print("verify", model, [r[1] for r in res], int((taps[0] >= 0).sum()), flush=True)
     ps.uninit()
+if only in ("all", "retrieval"):
+    # image retrieval: a codebook and VLAD vectors over sets with an empty one and one of several aggregation chunks, then
+    # the similarity + top-m on a dim that ends in a partial k-step, n below one tile and m >= n
+    rng = np.random.default_rng(5)
+    sets = [rng.random((n, 128)).astype(np.float32) for n in (300, 0, 4500, 7)]
+    cb = api.vlad_codebook(sets, k=24, iters=2, seed=1)
+    v, a = api.vlad_encode(sets, cb, assign=True)
+    print("vlad", v.shape, int(np.bincount(a, minlength=24).min()), flush=True)
+    for n, dim, m in ((300, 260, 7), (20, 36, 30), (1, 4, 1)):
+        nbr, sc = api.retrieve(rng.normal(size=(n, dim)).astype(np.float32), m)
+        print("retrieve", n, dim, m, int(nbr[0, 0]), flush=True)
