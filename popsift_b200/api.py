@@ -443,43 +443,80 @@ class FeaturesDev:
             self._pf = self._pd = self._pr = None
 
 
+def _last_error(lib) -> str:
+    return lib.ps_last_error(None).decode()
+
+
+def _check(lib, rc, name):
+    if rc != 0:
+        raise PopSiftError("%s error %d: %s" % (name, rc, _last_error(lib)))
+
+
+def _c_pairs(pairs):
+    """the (left, right) pairs as the C ABI's flat int32 array"""
+    flat = [int(v) for pq in pairs for v in pq]
+    return (C.c_int32 * max(len(flat), 1))(*flat)
+
+
+def _pair_rows(counts, pairs) -> list:
+    """each pair's result rows: its left set's count (none for an index out of range, which the C ABI refuses)"""
+    return [counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs]
+
+
+def _split_rows(out, rows) -> list:
+    """out's rows split by pair, rows[p] of them for pair p"""
+    ends = np.cumsum(rows, dtype=np.int64)
+    return [out[e - n:e] for n, e in zip(rows, ends)]
+
+
+def _model_code(model) -> int:
+    """GEOM's code of a model name; a code is returned as it is"""
+    if isinstance(model, str):
+        if model not in GEOM:
+            raise PopSiftError("model must be one of %s" % ", ".join(GEOM))
+        model = GEOM[model]
+    return int(model)
+
+
 def match_descriptors_dev(lib, d_left, n_left, d_right, n_right, flags=0, device=None) -> np.ndarray:
-    out = np.zeros((max(n_left, 0), 3), np.int32)
     if n_left <= 0:
-        return out
-    d_out = lib.ps_dev_alloc(out.nbytes)
-    if not d_out:
-        raise PopSiftError("ps_dev_alloc failed")
+        return np.zeros((0, 3), np.int32)
+    bufs = _DevBuffers(lib)
     try:
+        d_out = bufs.alloc(n_left * 12)
         dev = device if device is not None else max(0, lib.ps_pointer_device(d_left))
-        rc = lib.ps_match(dev, d_left, n_left, d_right, n_right, d_out, flags)
-        if rc != 0:
-            raise PopSiftError("ps_match error %d: %s" % (rc, lib.ps_last_error(None).decode()))
-        if lib.ps_dev_to_host(out.ctypes.data, d_out, out.nbytes) != 0:
-            raise PopSiftError("device -> host copy failed")
+        _check(lib, lib.ps_match(dev, d_left, n_left, d_right, n_right, d_out, flags), "ps_match")
+        return bufs.download(d_out, (n_left, 3), np.int32)
     finally:
-        lib.ps_dev_free(d_out)
-    return out
+        bufs.free()
 
 
 def match_descriptors(left: np.ndarray, right: np.ndarray, flags=0, device=0) -> np.ndarray:
     """host arrays (n, 128) float32 -> (n_left, 3) int32 (best, second, accept); copies through device memory"""
     lib = load_library()
     left = np.ascontiguousarray(left, np.float32); right = np.ascontiguousarray(right, np.float32)
-    import ctypes as _C
-    bufs = []
+    bufs = _DevBuffers(lib)
     try:
-        for a in (left, right):
-            p = lib.ps_dev_alloc(max(a.nbytes, 4))
-            if not p:
-                raise PopSiftError("ps_dev_alloc failed")
-            bufs.append(p)
-            if a.nbytes and lib.ps_host_to_dev(p, a.ctypes.data, a.nbytes) != 0:
-                raise PopSiftError("host -> device copy failed")
-        return match_descriptors_dev(lib, bufs[0], len(left), bufs[1], len(right), flags, device)
+        return match_descriptors_dev(lib, bufs.upload(left), len(left), bufs.upload(right), len(right), flags, device)
     finally:
-        for p in bufs:
-            lib.ps_dev_free(p)
+        bufs.free()
+
+
+def _match_pairs(sets, pairs, flags, device, u8) -> list:
+    """match_pairs (ps_match_batch) or match_pairs_u8 (ps_match_u8_batch)"""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    name = "ps_match_u8_batch" if u8 else "ps_match_batch"
+    bufs = _DevBuffers(lib)
+    try:
+        c_sets, c_n, counts, device = _desc_sets(lib, bufs, sets, device, u8)
+        rows = _pair_rows(counts, pairs)
+        d_out = bufs.alloc(sum(rows) * 12)
+        _check(lib, getattr(lib, name)(device, len(sets), c_sets, c_n, len(pairs), _c_pairs(pairs), d_out, flags), name)
+        out = bufs.download(d_out, (sum(rows), 3), np.int32)
+    finally:
+        bufs.free()
+    return _split_rows(out, rows)
 
 
 def match_pairs(sets, pairs, flags=0, device=None) -> list:
@@ -487,44 +524,7 @@ def match_pairs(sets, pairs, flags=0, device=None) -> list:
     `sets` holds FeaturesDev objects or host (n, 128) float32 arrays (copied through device memory); `pairs` is a list of
     (left, right) indices into `sets`.  Entry p is the (n_left, 3) int32 array (best, second, accept) that
     match_descriptors(sets[l], sets[r], flags) gives."""
-    lib = load_library()
-    pairs = [(int(a), int(b)) for a, b in pairs]
-    owned, ptrs, counts = [], [], []
-    try:
-        for s in sets:
-            if isinstance(s, FeaturesDev):
-                ptrs.append(s.getDescriptors()); counts.append(s.getDescriptorCount())
-                continue
-            a = np.ascontiguousarray(s, np.float32).reshape(-1, 128)
-            p = lib.ps_dev_alloc(max(a.nbytes, 4))
-            if not p:
-                raise PopSiftError("ps_dev_alloc failed")
-            owned.append(p)
-            if a.nbytes and lib.ps_host_to_dev(p, a.ctypes.data, a.nbytes) != 0:
-                raise PopSiftError("host -> device copy failed")
-            ptrs.append(p); counts.append(len(a))
-        if device is None:
-            device = next((lib.ps_pointer_device(p) for p, n in zip(ptrs, counts) if n > 0), 0)
-            device = max(0, device)
-        rows = [counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs]
-        out = np.zeros((sum(rows), 3), np.int32)
-        d_out = lib.ps_dev_alloc(max(out.nbytes, 4))
-        if not d_out:
-            raise PopSiftError("ps_dev_alloc failed")
-        owned.append(d_out)
-        c_sets = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
-        c_n = (C.c_int32 * max(len(counts), 1))(*counts)
-        c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
-        rc = lib.ps_match_batch(device, len(ptrs), c_sets, c_n, len(pairs), c_pairs, d_out, flags)
-        if rc != 0:
-            raise PopSiftError("ps_match_batch error %d: %s" % (rc, lib.ps_last_error(None).decode()))
-        if out.nbytes and lib.ps_dev_to_host(out.ctypes.data, d_out, out.nbytes) != 0:
-            raise PopSiftError("device -> host copy failed")
-    finally:
-        for p in owned:
-            lib.ps_dev_free(p)
-    starts = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
-    return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
+    return _match_pairs(sets, pairs, flags, device, False)
 
 
 def _to_u8_dev(lib, d_in, n, device) -> int:
@@ -535,7 +535,7 @@ def _to_u8_dev(lib, d_in, n, device) -> int:
     rc = lib.ps_descriptors_to_u8(device, d_in, n, q) if n else 0
     if rc != 0:
         lib.ps_dev_free(q)
-        raise PopSiftError("ps_descriptors_to_u8 error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        _check(lib, rc, "ps_descriptors_to_u8")
     return q
 
 
@@ -544,30 +544,14 @@ def descriptors_to_u8(x, device=None) -> np.ndarray:
     NaN -> 0 -- what the reference prints under --write-as-uchar, saturated.  `x` is a FeaturesDev or a host (n, 128)
     float32 array; returns a host (n, 128) uint8 array."""
     lib = load_library()
-    owned = []
+    bufs = _DevBuffers(lib)
     try:
-        if isinstance(x, FeaturesDev):
-            d_in, n = x.getDescriptors(), x.getDescriptorCount()
-        else:
-            a = np.ascontiguousarray(x, np.float32).reshape(-1, 128)
-            n = len(a)
-            d_in = lib.ps_dev_alloc(max(a.nbytes, 4))
-            if not d_in:
-                raise PopSiftError("ps_dev_alloc failed")
-            owned.append(d_in)
-            if a.nbytes and lib.ps_host_to_dev(d_in, a.ctypes.data, a.nbytes) != 0:
-                raise PopSiftError("host -> device copy failed")
-        if device is None:
-            device = max(0, lib.ps_pointer_device(d_in)) if n else 0
-        q = _to_u8_dev(lib, d_in, n, device)
-        owned.append(q)
-        out = np.zeros((n, 128), np.uint8)
-        if out.nbytes and lib.ps_dev_to_host(out.ctypes.data, q, out.nbytes) != 0:
-            raise PopSiftError("device -> host copy failed")
-        return out
+        c_sets, _, (n,), device = _desc_sets(lib, bufs, [x], device)
+        q = _to_u8_dev(lib, c_sets[0], n, device)
+        bufs.ptrs.append(q)
+        return bufs.download(q, (n, 128), np.uint8)
     finally:
-        for p in owned:
-            lib.ps_dev_free(p)
+        bufs.free()
 
 
 def match_pairs_u8(sets, pairs, flags=0, device=None) -> list:
@@ -575,47 +559,7 @@ def match_pairs_u8(sets, pairs, flags=0, device=None) -> list:
     uint8 arrays (copied through device memory) or FeaturesDev objects (quantised on the device by ps_descriptors_to_u8;
     the descriptors never leave it).  Entry p is the (n_left, 3) int32 array (best, second, accept), row for row what
     match_pairs gives on float32 copies of the 8-bit sets under FeaturesDev.MATCH_EXACT."""
-    lib = load_library()
-    pairs = [(int(a), int(b)) for a, b in pairs]
-    owned, ptrs, counts = [], [], []
-    try:
-        if device is None:
-            dev_sets = [s for s in sets if isinstance(s, FeaturesDev) and s.getDescriptorCount() > 0]
-            device = max(0, lib.ps_pointer_device(dev_sets[0].getDescriptors())) if dev_sets else 0
-        for s in sets:
-            if isinstance(s, FeaturesDev):
-                n = s.getDescriptorCount()
-                p = _to_u8_dev(lib, s.getDescriptors(), n, device)
-                owned.append(p)
-                ptrs.append(p); counts.append(n)
-                continue
-            a = np.ascontiguousarray(s, np.uint8).reshape(-1, 128)
-            p = lib.ps_dev_alloc(max(a.nbytes, 16))
-            if not p:
-                raise PopSiftError("ps_dev_alloc failed")
-            owned.append(p)
-            if a.nbytes and lib.ps_host_to_dev(p, a.ctypes.data, a.nbytes) != 0:
-                raise PopSiftError("host -> device copy failed")
-            ptrs.append(p); counts.append(len(a))
-        rows = [counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs]
-        out = np.zeros((sum(rows), 3), np.int32)
-        d_out = lib.ps_dev_alloc(max(out.nbytes, 4))
-        if not d_out:
-            raise PopSiftError("ps_dev_alloc failed")
-        owned.append(d_out)
-        c_sets = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
-        c_n = (C.c_int32 * max(len(counts), 1))(*counts)
-        c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
-        rc = lib.ps_match_u8_batch(device, len(ptrs), c_sets, c_n, len(pairs), c_pairs, d_out, flags)
-        if rc != 0:
-            raise PopSiftError("ps_match_u8_batch error %d: %s" % (rc, lib.ps_last_error(None).decode()))
-        if out.nbytes and lib.ps_dev_to_host(out.ctypes.data, d_out, out.nbytes) != 0:
-            raise PopSiftError("device -> host copy failed")
-    finally:
-        for p in owned:
-            lib.ps_dev_free(p)
-    starts = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
-    return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
+    return _match_pairs(sets, pairs, flags, device, True)
 
 
 class _DevBuffers:
@@ -649,19 +593,30 @@ class _DevBuffers:
             self.lib.ps_dev_free(self.ptrs.pop())
 
 
-def _first_device(lib, sets) -> int:
+def _desc_sets(lib, bufs, sets, device=None, u8=False):
+    """The C ABI arrays of descriptor sets: FeaturesDev objects, or host (n, 128) arrays uploaded into bufs (float32, or
+    uint8 with u8=True).  With u8=True FeaturesDev sets are quantised on the device into bufs.  Returns (c_sets, c_n,
+    counts, device); a device of None becomes that of the first non-empty set, else 0."""
+    ptrs, counts = [], []
     for s in sets:
-        if isinstance(s, FeaturesDev) and s.getDescriptorCount() > 0:
-            return max(0, lib.ps_pointer_device(s.getDescriptors()))
-    return 0
+        if isinstance(s, FeaturesDev):
+            ptrs.append(s.getDescriptors()); counts.append(s.getDescriptorCount())
+            continue
+        a = np.ascontiguousarray(s, np.uint8 if u8 else np.float32).reshape(-1, 128)
+        ptrs.append(bufs.upload(a)); counts.append(len(a))
+    if device is None:
+        device = next((max(0, lib.ps_pointer_device(p)) for p, n in zip(ptrs, counts) if n > 0), 0)
+    if u8:
+        for i, s in enumerate(sets):
+            if isinstance(s, FeaturesDev):
+                ptrs[i] = _to_u8_dev(lib, ptrs[i], counts[i], device)
+                bufs.ptrs.append(ptrs[i])
+    n = max(len(sets), 1)
+    return (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*counts), counts, device
 
 
 def _verify_params(model="homography", threshold=4.0, n_samples=1024, seed=0, refine=True) -> PsVerifyParams:
-    if isinstance(model, str):
-        if model not in GEOM:
-            raise PopSiftError("model must be one of %s" % ", ".join(GEOM))
-        model = GEOM[model]
-    return PsVerifyParams(int(model), int(n_samples), float(threshold), 1 if refine else 0, int(seed) & ((1 << 64) - 1))
+    return PsVerifyParams(_model_code(model), int(n_samples), float(threshold), 1 if refine else 0, int(seed) & ((1 << 64) - 1))
 
 
 def _correspondences_dev(lib, bufs, sets, pairs, d_match, device):
@@ -677,11 +632,9 @@ def _correspondences_dev(lib, bufs, sets, pairs, d_match, device):
     c_feat = (C.c_void_p * max(len(sets), 1))(*[s.getFeatures() for s in sets])
     c_rev = (C.c_void_p * max(len(sets), 1))(*[s.getReverseMap() for s in sets])
     c_n = (C.c_int32 * max(len(sets), 1))(*counts)
-    c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
-    rc = lib.ps_match_correspondences(device, len(sets), c_feat, c_rev, c_n, len(pairs), c_pairs, d_match, d_corr, d_src,
+    rc = lib.ps_match_correspondences(device, len(sets), c_feat, c_rev, c_n, len(pairs), _c_pairs(pairs), d_match, d_corr, d_src,
                                       n_corr.ctypes.data)
-    if rc != 0:
-        raise PopSiftError("ps_match_correspondences error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+    _check(lib, rc, "ps_match_correspondences")
     return d_corr, d_src, start[:len(pairs)].copy(), n_corr[:len(pairs)].copy()
 
 
@@ -701,8 +654,7 @@ def _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm: PsVerifyParams, t
     c_n = np.ascontiguousarray(n_corr, np.int32)
     rc = lib.ps_verify_batch(device, P, d_corr, c_start.ctypes.data, c_n.ctypes.data, C.byref(prm), d_models, d_n, d_mask,
                              C.byref(tp) if tp is not None else None)
-    if rc != 0:
-        raise PopSiftError("ps_verify_batch error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+    _check(lib, rc, "ps_verify_batch")
     out = [bufs.download(d_models, (P, 3, 3), np.float32), bufs.download(d_n, P, np.int32),
            bufs.download(d_mask, rows, np.uint8).astype(bool)]
     if taps:
@@ -722,7 +674,7 @@ def match_correspondences(sets, pairs, matches, device=None):
         raise PopSiftError("one match array per pair expected")
     bufs = _DevBuffers(lib)
     try:
-        device = _first_device(lib, sets) if device is None else device
+        device = _desc_sets(lib, bufs, sets, device)[3]
         m = np.concatenate([np.asarray(r, np.int32).reshape(-1, 3) for r in matches]) if matches else np.zeros((0, 3), np.int32)
         d_corr, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, bufs.upload(m), device)
         rows = len(m)
@@ -769,38 +721,26 @@ def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, guid
     for l, r in pairs:
         if not (0 <= l < len(sets) and 0 <= r < len(sets)):
             raise PopSiftError("set index out of range")
+    if matches is not None and len(matches) != len(pairs):
+        raise PopSiftError("one match array per pair expected")
     rows = sum(counts[l] for l, _ in pairs)
     bufs = _DevBuffers(lib)
     try:
-        device = _first_device(lib, sets) if device is None else device
-        q = None                                   # the 8-bit copies of the sets, when matching made them
+        # the 8-bit copies are made only when matching uses them
+        descs = _desc_sets(lib, bufs, sets, device, u8 and (matches is None or guided))
+        c_sets, c_n, _, device = descs
         if matches is not None:
-            if len(matches) != len(pairs):
-                raise PopSiftError("one match array per pair expected")
             m = np.concatenate([np.asarray(r, np.int32).reshape(-1, 3) for r in matches]) if matches else np.zeros((0, 3), np.int32)
             d_match = bufs.upload(m)
         else:
             d_match = bufs.alloc(rows * 12)
-            c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
-            c_n = (C.c_int32 * max(len(sets), 1))(*counts)
-            if u8:
-                q = []
-                for s in sets:
-                    p = _to_u8_dev(lib, s.getDescriptors(), s.getDescriptorCount(), device)
-                    bufs.ptrs.append(p)
-                    q.append(p)
-                c_sets = (C.c_void_p * max(len(sets), 1))(*q)
-                rc = lib.ps_match_u8_batch(device, len(sets), c_sets, c_n, len(pairs), c_pairs, d_match, flags)
-            else:
-                c_sets = (C.c_void_p * max(len(sets), 1))(*[s.getDescriptors() for s in sets])
-                rc = lib.ps_match_batch(device, len(sets), c_sets, c_n, len(pairs), c_pairs, d_match, flags)
-            if rc != 0:
-                raise PopSiftError("matching error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+            fn = lib.ps_match_u8_batch if u8 else lib.ps_match_batch
+            _check(lib, fn(device, len(sets), c_sets, c_n, len(pairs), _c_pairs(pairs), d_match, flags), "matching")
         d_corr, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_match, device)
         if guided:
             d_models = bufs.alloc(len(pairs) * 36)
             models, n_in, mask = _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm, d_models=d_models)
-            d_guided = _match_guided_dev(lib, bufs, sets, pairs, d_models, prm.model, prm.threshold, flags, u8, device, u8_sets=q)
+            d_guided = _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, prm.model, prm.threshold, flags, u8)
             _, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_guided, device)
             src = bufs.download(d_src, rows, np.int32)
             return [(models[p], int(n_corr[p]), src[int(start[p]):int(start[p]) + int(n_corr[p])].copy()) for p in range(len(pairs))]
@@ -815,37 +755,21 @@ def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, guid
     return out
 
 
-def _match_guided_dev(lib, bufs, sets, pairs, d_models, model, threshold, flags, u8, device, u8_sets=None) -> int:
-    """ps_match_guided_batch / ps_match_u8_guided_batch on FeaturesDev sets and device-resident models: the device rows.
-    u8_sets: the sets' 8-bit device copies when the caller already has them (u8=True)"""
+def _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, model, threshold, flags, u8) -> int:
+    """ps_match_guided_batch / ps_match_u8_guided_batch on FeaturesDev sets, their descriptors as _desc_sets gave them
+    (`descs`, 8-bit with u8=True) and device-resident models: the device rows"""
     for s in sets:
         if not isinstance(s, FeaturesDev):
             raise PopSiftError("guided matching needs FeaturesDev sets (Config.MatchingMode)")
-    counts = [s.getDescriptorCount() for s in sets]
-    rows = sum(counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs)
-    d_out = bufs.alloc(rows * 12)
-    if u8 and u8_sets is not None:
-        descs = list(u8_sets)
-        fn, name = lib.ps_match_u8_guided_batch, "ps_match_u8_guided_batch"
-    elif u8:
-        descs = []
-        for s in sets:
-            p = _to_u8_dev(lib, s.getDescriptors(), s.getDescriptorCount(), device)
-            bufs.ptrs.append(p)
-            descs.append(p)
-        fn, name = lib.ps_match_u8_guided_batch, "ps_match_u8_guided_batch"
-    else:
-        descs = [s.getDescriptors() for s in sets]
-        fn, name = lib.ps_match_guided_batch, "ps_match_guided_batch"
+    c_sets, c_n, counts, device = descs
+    d_out = bufs.alloc(sum(_pair_rows(counts, pairs)) * 12)
+    name = "ps_match_u8_guided_batch" if u8 else "ps_match_guided_batch"
     n = max(len(sets), 1)
-    c_sets = (C.c_void_p * n)(*descs)
     c_feat = (C.c_void_p * n)(*[s.getFeatures() for s in sets])
     c_rev = (C.c_void_p * n)(*[s.getReverseMap() for s in sets])
-    c_n = (C.c_int32 * n)(*counts)
-    c_pairs = (C.c_int32 * max(2 * len(pairs), 1))(*[v for pq in pairs for v in pq])
-    rc = fn(device, len(sets), c_sets, c_feat, c_rev, c_n, len(pairs), c_pairs, d_models, int(model), float(threshold), d_out, flags)
-    if rc != 0:
-        raise PopSiftError("%s error %d: %s" % (name, rc, lib.ps_last_error(None).decode()))
+    rc = getattr(lib, name)(device, len(sets), c_sets, c_feat, c_rev, c_n, len(pairs), _c_pairs(pairs), d_models, int(model),
+                            float(threshold), d_out, flags)
+    _check(lib, rc, name)
     return d_out
 
 
@@ -857,37 +781,19 @@ def match_pairs_guided(sets, pairs, models, model="homography", threshold=4.0, f
     or "fundamental".  Entry p is the (n_left, 3) int32 array (best, second, accept); no eligible descriptor gives (0, 0, 0)."""
     lib = load_library()
     pairs = [(int(a), int(b)) for a, b in pairs]
-    if isinstance(model, str):
-        if model not in GEOM:
-            raise PopSiftError("model must be one of %s" % ", ".join(GEOM))
-        model = GEOM[model]
+    model = _model_code(model)
     m = np.ascontiguousarray(models, np.float32).reshape(-1, 9)
     if len(m) != len(pairs):
         raise PopSiftError("one model per pair expected")
-    counts = [s.getDescriptorCount() for s in sets]
-    rows = [counts[l] if 0 <= l < len(counts) else 0 for l, _ in pairs]
     bufs = _DevBuffers(lib)
     try:
-        device = _first_device(lib, sets) if device is None else device
-        d_out = _match_guided_dev(lib, bufs, sets, pairs, bufs.upload(m), model, threshold, flags, u8, device)
+        descs = _desc_sets(lib, bufs, sets, device, u8)
+        rows = _pair_rows(descs[2], pairs)
+        d_out = _match_guided_dev(lib, bufs, sets, descs, pairs, bufs.upload(m), model, threshold, flags, u8)
         out = bufs.download(d_out, (sum(rows), 3), np.int32)
     finally:
         bufs.free()
-    starts = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
-    return [out[starts[p]:starts[p + 1]] for p in range(len(pairs))]
-
-
-def _desc_sets(lib, bufs, sets):
-    """device pointers and counts of FeaturesDev objects or host (n, 128) float32 arrays (uploaded into bufs)"""
-    ptrs, counts = [], []
-    for s in sets:
-        if isinstance(s, FeaturesDev):
-            ptrs.append(s.getDescriptors()); counts.append(s.getDescriptorCount())
-            continue
-        a = np.ascontiguousarray(s, np.float32).reshape(-1, 128)
-        ptrs.append(bufs.upload(a)); counts.append(len(a))
-    n = max(len(sets), 1)
-    return (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*counts), counts
+    return _split_rows(out, rows)
 
 
 def vlad_codebook(sets, k=64, iters=10, seed=0, flags=0, device=None) -> np.ndarray:
@@ -896,12 +802,10 @@ def vlad_codebook(sets, k=64, iters=10, seed=0, flags=0, device=None) -> np.ndar
     lib = load_library()
     bufs = _DevBuffers(lib)
     try:
-        device = _first_device(lib, sets) if device is None else device
-        c_sets, c_n, _ = _desc_sets(lib, bufs, sets)
+        c_sets, c_n, _, device = _desc_sets(lib, bufs, sets, device)
         d_c = bufs.alloc(k * 512)
-        rc = lib.ps_vlad_train(device, len(sets), c_sets, c_n, int(k), int(iters), int(seed) & ((1 << 64) - 1), d_c, flags)
-        if rc != 0:
-            raise PopSiftError("ps_vlad_train error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        _check(lib, lib.ps_vlad_train(device, len(sets), c_sets, c_n, int(k), int(iters), int(seed) & ((1 << 64) - 1), d_c, flags),
+               "ps_vlad_train")
         return bufs.download(d_c, (k, 128), np.float32)
     finally:
         bufs.free()
@@ -916,14 +820,11 @@ def vlad_encode(sets, codebook, flags=0, assign=False, device=None):
     k = len(cb)
     bufs = _DevBuffers(lib)
     try:
-        device = _first_device(lib, sets) if device is None else device
-        c_sets, c_n, counts = _desc_sets(lib, bufs, sets)
+        c_sets, c_n, counts, device = _desc_sets(lib, bufs, sets, device)
         N = sum(counts)
         d_v = bufs.alloc(len(sets) * k * 512)
         d_a = bufs.alloc(N * 4) if assign else None
-        rc = lib.ps_vlad_encode(device, len(sets), c_sets, c_n, k, bufs.upload(cb), d_v, d_a, flags)
-        if rc != 0:
-            raise PopSiftError("ps_vlad_encode error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        _check(lib, lib.ps_vlad_encode(device, len(sets), c_sets, c_n, k, bufs.upload(cb), d_v, d_a, flags), "ps_vlad_encode")
         v = bufs.download(d_v, (len(sets), k * 128), np.float32)
         return (v, bufs.download(d_a, N, np.int32)) if assign else v
     finally:
@@ -939,9 +840,7 @@ def retrieve(vectors, m, device=0):
     bufs = _DevBuffers(lib)
     try:
         d_n, d_s = bufs.alloc(n * m * 4), bufs.alloc(n * m * 4)
-        rc = lib.ps_retrieve_pairs(device, n, bufs.upload(v), dim, int(m), d_n, d_s)
-        if rc != 0:
-            raise PopSiftError("ps_retrieve_pairs error %d: %s" % (rc, lib.ps_last_error(None).decode()))
+        _check(lib, lib.ps_retrieve_pairs(device, n, bufs.upload(v), dim, int(m), d_n, d_s), "ps_retrieve_pairs")
         return bufs.download(d_n, (n, m), np.int32), bufs.download(d_s, (n, m), np.float32)
     finally:
         bufs.free()
@@ -1019,7 +918,7 @@ class PopSift:
     def _create(self, w, h):
         ctx = self._lib.ps_create(self._device, C.byref(self._config._c), w, h, self._nslots)
         if not ctx:
-            raise PopSiftError(self._lib.ps_last_error(None).decode())
+            raise PopSiftError(_last_error(self._lib))
         self._ctx = ctx
         self._max = (w, h)
 

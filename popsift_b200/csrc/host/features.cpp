@@ -17,6 +17,7 @@
 #include <map>
 #include <mutex>
 #include <new>
+#include <optional>
 #include <stdexcept>
 
 namespace popsift {
@@ -90,6 +91,88 @@ float warp_order_sq_dist(const Descriptor& l, const Descriptor& r)
     return lane[0];
 }
 
+// a device buffer freed at scope exit
+struct DevBuf {
+    void* p;
+    explicit DevBuf(size_t bytes, const std::string& fn) : p(ps_dev_alloc(std::max<size_t>(bytes, 16)))
+    {
+        if (!p) throw std::runtime_error(fn + ": failed to allocate device memory");
+    }
+    ~DevBuf() { ps_dev_free(p); }
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+};
+
+// throws "<who>[: <entry>] failed: <last C ABI error>" unless rc is PS_OK
+void check(int rc, const std::string& who, const char* entry = nullptr)
+{
+    if (rc != PS_OK) throw std::runtime_error(who + (entry ? std::string(": ") + entry : std::string()) + " failed: " + ps_last_error(nullptr));
+}
+
+// the C ABI arguments of a batched call over FeaturesDev sets: each set's device arrays and descriptor count, the device
+// of the first non-empty set, the pair list flattened with each pair's first output row, and the rows of all pairs
+struct Batch {
+    std::string who;
+    std::vector<const ps_descriptor*> desc;
+    std::vector<const ps_feature*> feat;
+    std::vector<const int32_t*> rev;
+    std::vector<int32_t> n_desc;
+    int dev = 0;
+    std::vector<int32_t> flat;
+    std::vector<size_t> start;
+    size_t rows = 0, descs = 0;   // descs: the descriptors of all sets
+
+    Batch(const char* name, const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs)
+        : who(std::string("popsift::") + name), desc(sets.size()), feat(sets.size()), rev(sets.size()), n_desc(sets.size()),
+          flat(2 * pairs.size()), start(pairs.size())
+    {
+        int first = -1;
+        for (size_t i = 0; i < sets.size(); ++i) {
+            if (!sets[i]) throw std::runtime_error(who + ": null set");
+            desc[i] = reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors());
+            feat[i] = reinterpret_cast<const ps_feature*>(sets[i]->getFeatures());
+            rev[i] = sets[i]->getReverseMap();
+            n_desc[i] = sets[i]->getDescriptorCount();
+            if (n_desc[i] > 0 && first < 0) first = (int)i;
+            descs += (size_t)std::max(n_desc[i], 0);
+        }
+        if (first >= 0) dev = std::max(0, ps_pointer_device(desc[first]));
+        for (size_t p = 0; p < pairs.size(); ++p) {
+            const int l = pairs[p].first, r = pairs[p].second;
+            if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error(who + ": set index out of range");
+            flat[2 * p] = l; flat[2 * p + 1] = r;
+            start[p] = rows;
+            rows += pair_rows(p);
+        }
+    }
+
+    size_t pair_rows(size_t p) const { return (size_t)std::max(n_desc[flat[2 * p]], 0); }
+
+    // the 8-bit copies of all sets, back to back in q (128-byte rows keep every set 16-byte aligned)
+    std::vector<const uint8_t*> to_u8(uint8_t* q) const
+    {
+        std::vector<const uint8_t*> u8(n_desc.size(), nullptr);
+        for (size_t i = 0; i < n_desc.size(); ++i) {
+            if (n_desc[i] <= 0) continue;
+            check(ps_descriptors_to_u8(dev, desc[i], n_desc[i], q), who);
+            u8[i] = q;
+            q += (size_t)n_desc[i] * 128;
+        }
+        return u8;
+    }
+
+    // the result rows (best, second, accept) on the device, downloaded and split by pair
+    std::vector<std::vector<int>> download(const int32_t* d_out) const
+    {
+        std::vector<int> all(rows * 3);
+        check(ps_dev_to_host(all.data(), d_out, all.size() * sizeof(int32_t)), who);
+        std::vector<std::vector<int>> out(start.size());
+        for (size_t p = 0; p < out.size(); ++p)
+            out[p].assign(all.begin() + 3 * start[p], all.begin() + 3 * (start[p] + pair_rows(p)));
+        return out;
+    }
+};
+
 } // namespace
 
 // reference features.cu:282-304: 2-nearest-neighbour search of every descriptor of *this among `other`'s, then one
@@ -124,265 +207,121 @@ std::vector<int> FeaturesDev::matchIndices(FeaturesDev* other, int flags)
     const int l_len = getDescriptorCount(), r_len = other->getDescriptorCount();
     std::vector<int> m((size_t)std::max(l_len, 0) * 3, 0);
     if (l_len <= 0) return m;
-    int32_t* d_out = static_cast<int32_t*>(ps_dev_alloc(m.size() * sizeof(int32_t)));
-    if (!d_out) throw std::runtime_error("FeaturesDev::match: failed to allocate device memory");
+    const char* who = "FeaturesDev::match";
+    DevBuf d_out(m.size() * sizeof(int32_t), who);
     const int dev = std::max(0, ps_pointer_device(_ori));
-    int rc = ps_match(dev, reinterpret_cast<const ps_descriptor*>(_ori), l_len, reinterpret_cast<const ps_descriptor*>(other->_ori),
-                      r_len, d_out, flags);
-    if (rc == PS_OK) rc = ps_dev_to_host(m.data(), d_out, m.size() * sizeof(int32_t));
-    ps_dev_free(d_out);
-    if (rc != PS_OK) throw std::runtime_error(std::string("FeaturesDev::match failed: ") + ps_last_error(nullptr));
+    check(ps_match(dev, reinterpret_cast<const ps_descriptor*>(_ori), l_len, reinterpret_cast<const ps_descriptor*>(other->_ori), r_len,
+                   static_cast<int32_t*>(d_out.p), flags), who);
+    check(ps_dev_to_host(m.data(), d_out.p, m.size() * sizeof(int32_t)), who);
     return m;
 }
 
+namespace {
+
+// matchPairs, matchPairsU8 (u8), matchPairsGuided and matchPairsGuidedU8 (geometry non-null): the C ABI call on the sets'
+// descriptors or on their 8-bit copies
+std::vector<std::vector<int>> match_pairs(const char* name, bool u8, const std::vector<FeaturesDev*>& sets,
+                                          const std::vector<std::pair<int, int>>& pairs, const std::vector<PairGeometry>* geometry,
+                                          const VerifyParams* params, int flags)
+{
+    if (geometry && geometry->size() != pairs.size()) throw std::runtime_error(std::string("popsift::") + name + ": one geometry per pair expected");
+    const Batch b(name, sets, pairs);
+    if (b.rows == 0) return std::vector<std::vector<int>>(pairs.size());
+    DevBuf d_out(b.rows * 3 * sizeof(int32_t), b.who);
+    int32_t* out = static_cast<int32_t*>(d_out.p);
+    std::optional<DevBuf> d_models, q;
+    if (geometry) {
+        std::vector<float> models(pairs.size() * 9);
+        for (size_t p = 0; p < pairs.size(); ++p) std::copy((*geometry)[p].model, (*geometry)[p].model + 9, models.begin() + 9 * p);
+        d_models.emplace(models.size() * sizeof(float), b.who);
+        check(ps_host_to_dev(d_models->p, models.data(), models.size() * sizeof(float)), b.who);
+    }
+    std::vector<const uint8_t*> d_u8;
+    if (u8) d_u8 = b.to_u8(static_cast<uint8_t*>(q.emplace(b.descs * 128, b.who).p));
+    const int n_sets = (int)sets.size(), n_pairs = (int)pairs.size();
+    int rc;
+    if (!geometry)
+        rc = u8 ? ps_match_u8_batch(b.dev, n_sets, d_u8.data(), b.n_desc.data(), n_pairs, b.flat.data(), out, flags)
+                : ps_match_batch(b.dev, n_sets, b.desc.data(), b.n_desc.data(), n_pairs, b.flat.data(), out, flags);
+    else {
+        const float* m = static_cast<const float*>(d_models->p);
+        rc = u8 ? ps_match_u8_guided_batch(b.dev, n_sets, d_u8.data(), b.feat.data(), b.rev.data(), b.n_desc.data(), n_pairs, b.flat.data(),
+                                           m, params->model, params->threshold, out, flags)
+                : ps_match_guided_batch(b.dev, n_sets, b.desc.data(), b.feat.data(), b.rev.data(), b.n_desc.data(), n_pairs, b.flat.data(),
+                                        m, params->model, params->threshold, out, flags);
+    }
+    check(rc, b.who);
+    return b.download(out);
+}
+
+} // namespace
+
 std::vector<std::vector<int>> matchPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs, int flags)
 {
-    std::vector<const ps_descriptor*> d_sets(sets.size());
-    std::vector<int32_t> n_desc(sets.size());
-    for (size_t i = 0; i < sets.size(); ++i) {
-        if (!sets[i]) throw std::runtime_error("popsift::matchPairs: null set");
-        d_sets[i] = reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors());
-        n_desc[i] = sets[i]->getDescriptorCount();
-    }
-    std::vector<int32_t> flat(2 * pairs.size());
-    std::vector<std::vector<int>> out(pairs.size());
-    size_t rows = 0;
-    for (size_t p = 0; p < pairs.size(); ++p) {
-        const int l = pairs[p].first, r = pairs[p].second;
-        if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error("popsift::matchPairs: set index out of range");
-        flat[2 * p] = l; flat[2 * p + 1] = r;
-        out[p].assign((size_t)std::max(n_desc[l], 0) * 3, 0);
-        rows += out[p].size() / 3;
-    }
-    if (rows == 0) return out;
-    int32_t* d_out = static_cast<int32_t*>(ps_dev_alloc(rows * 3 * sizeof(int32_t)));
-    if (!d_out) throw std::runtime_error("popsift::matchPairs: failed to allocate device memory");
-    int dev = 0;
-    for (size_t i = 0; i < sets.size(); ++i)
-        if (n_desc[i] > 0) { dev = std::max(0, ps_pointer_device(d_sets[i])); break; }
-    int rc = ps_match_batch(dev, (int)sets.size(), d_sets.data(), n_desc.data(), (int)pairs.size(), flat.data(), d_out, flags);
-    size_t row = 0;
-    for (size_t p = 0; p < pairs.size() && rc == PS_OK; ++p) {
-        rc = ps_dev_to_host(out[p].data(), d_out + 3 * row, out[p].size() * sizeof(int32_t));
-        row += out[p].size() / 3;
-    }
-    ps_dev_free(d_out);
-    if (rc != PS_OK) throw std::runtime_error(std::string("popsift::matchPairs failed: ") + ps_last_error(nullptr));
-    return out;
+    return match_pairs("matchPairs", false, sets, pairs, nullptr, nullptr, flags);
 }
 
 std::vector<std::vector<int>> matchPairsU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs, int flags)
 {
-    std::vector<int32_t> n_desc(sets.size());
-    for (size_t i = 0; i < sets.size(); ++i) {
-        if (!sets[i]) throw std::runtime_error("popsift::matchPairsU8: null set");
-        n_desc[i] = std::max(sets[i]->getDescriptorCount(), 0);
-    }
-    std::vector<int32_t> flat(2 * pairs.size());
-    std::vector<std::vector<int>> out(pairs.size());
-    size_t rows = 0;
-    for (size_t p = 0; p < pairs.size(); ++p) {
-        const int l = pairs[p].first, r = pairs[p].second;
-        if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error("popsift::matchPairsU8: set index out of range");
-        flat[2 * p] = l; flat[2 * p + 1] = r;
-        out[p].assign((size_t)n_desc[l] * 3, 0);
-        rows += out[p].size() / 3;
-    }
-    if (rows == 0) return out;
-    int dev = 0;
-    for (size_t i = 0; i < sets.size(); ++i)
-        if (n_desc[i] > 0) { dev = std::max(0, ps_pointer_device(sets[i]->getDescriptors())); break; }
-    // the 8-bit copies of every set (cudaMalloc: 256-byte aligned) and the result rows
-    std::vector<void*> owned;
-    auto release = [&]() { for (void* p : owned) ps_dev_free(p); };
-    std::vector<const uint8_t*> d_sets(sets.size(), nullptr);
-    int rc = PS_OK;
-    for (size_t i = 0; i < sets.size() && rc == PS_OK; ++i) {
-        if (n_desc[i] == 0) continue;
-        uint8_t* q = static_cast<uint8_t*>(ps_dev_alloc((size_t)n_desc[i] * 128));
-        if (!q) { release(); throw std::runtime_error("popsift::matchPairsU8: failed to allocate device memory"); }
-        owned.push_back(q);
-        d_sets[i] = q;
-        rc = ps_descriptors_to_u8(dev, reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors()), n_desc[i], q);
-    }
-    int32_t* d_out = rc == PS_OK ? static_cast<int32_t*>(ps_dev_alloc(rows * 3 * sizeof(int32_t))) : nullptr;
-    if (rc == PS_OK && !d_out) { release(); throw std::runtime_error("popsift::matchPairsU8: failed to allocate device memory"); }
-    if (d_out) owned.push_back(d_out);
-    if (rc == PS_OK) rc = ps_match_u8_batch(dev, (int)sets.size(), d_sets.data(), n_desc.data(), (int)pairs.size(), flat.data(), d_out, flags);
-    size_t row = 0;
-    for (size_t p = 0; p < pairs.size() && rc == PS_OK; ++p) {
-        rc = ps_dev_to_host(out[p].data(), d_out + 3 * row, out[p].size() * sizeof(int32_t));
-        row += out[p].size() / 3;
-    }
-    release();
-    if (rc != PS_OK) throw std::runtime_error(std::string("popsift::matchPairsU8 failed: ") + ps_last_error(nullptr));
-    return out;
+    return match_pairs("matchPairsU8", true, sets, pairs, nullptr, nullptr, flags);
+}
+
+std::vector<std::vector<int>> matchPairsGuided(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                               const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags)
+{
+    return match_pairs("matchPairsGuided", false, sets, pairs, &geometry, &params, flags);
+}
+
+std::vector<std::vector<int>> matchPairsGuidedU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                                 const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags)
+{
+    return match_pairs("matchPairsGuidedU8", true, sets, pairs, &geometry, &params, flags);
 }
 
 std::vector<PairGeometry> verifyPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
                                       const std::vector<std::vector<int>>& matches, const VerifyParams& params)
 {
     if (matches.size() != pairs.size()) throw std::runtime_error("popsift::verifyPairs: one match list per pair expected");
-    std::vector<const ps_feature*> d_feat(sets.size());
-    std::vector<const int32_t*> d_rev(sets.size());
-    std::vector<int32_t> n_desc(sets.size());
-    for (size_t i = 0; i < sets.size(); ++i) {
-        if (!sets[i]) throw std::runtime_error("popsift::verifyPairs: null set");
-        d_feat[i] = reinterpret_cast<const ps_feature*>(sets[i]->getFeatures());
-        d_rev[i] = sets[i]->getReverseMap();
-        n_desc[i] = std::max(sets[i]->getDescriptorCount(), 0);
-    }
-    std::vector<int32_t> flat(2 * pairs.size()), start(pairs.size()), n_corr(pairs.size(), 0);
-    size_t rows = 0;
-    for (size_t p = 0; p < pairs.size(); ++p) {
-        const int l = pairs[p].first, r = pairs[p].second;
-        if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error("popsift::verifyPairs: set index out of range");
-        if (matches[p].size() != (size_t)n_desc[l] * 3) throw std::runtime_error("popsift::verifyPairs: match rows do not fit the left set");
-        flat[2 * p] = l; flat[2 * p + 1] = r;
-        start[p] = (int32_t)rows;
-        rows += (size_t)n_desc[l];
-    }
+    const Batch b("verifyPairs", sets, pairs);
+    for (size_t p = 0; p < pairs.size(); ++p)
+        if (matches[p].size() != b.pair_rows(p) * 3) throw std::runtime_error(b.who + ": match rows do not fit the left set");
     std::vector<PairGeometry> out(pairs.size());
     for (PairGeometry& g : out) { std::fill(g.model, g.model + 9, 0.0f); g.n_inliers = 0; }
     if (pairs.empty()) return out;
-    int dev = 0;
-    for (size_t i = 0; i < sets.size(); ++i)
-        if (n_desc[i] > 0) { dev = std::max(0, ps_pointer_device(d_feat[i])); break; }
     // device buffers: match rows, correspondences (16-byte rows), source rows, masks; models and counts per pair
-    const size_t nr = std::max<size_t>(rows, 1);
-    std::vector<void*> owned;
-    auto release = [&]() { for (void* p : owned) ps_dev_free(p); };
-    auto alloc = [&](size_t bytes) {
-        void* p = ps_dev_alloc(bytes);
-        if (!p) { release(); throw std::runtime_error("popsift::verifyPairs: failed to allocate device memory"); }
-        owned.push_back(p);
-        return p;
-    };
-    int32_t* d_match = static_cast<int32_t*>(alloc(nr * 3 * sizeof(int32_t)));
-    float* d_corr = static_cast<float*>(alloc(nr * 4 * sizeof(float)));
-    int32_t* d_src = static_cast<int32_t*>(alloc(nr * sizeof(int32_t)));
-    uint8_t* d_mask = static_cast<uint8_t*>(alloc(nr));
-    float* d_models = static_cast<float*>(alloc(pairs.size() * 9 * sizeof(float)));
-    int32_t* d_n = static_cast<int32_t*>(alloc(pairs.size() * sizeof(int32_t)));
-    int rc = PS_OK;
-    for (size_t p = 0; p < pairs.size() && rc == PS_OK; ++p)
+    const size_t nr = std::max<size_t>(b.rows, 1), np = pairs.size();
+    DevBuf match(nr * 3 * sizeof(int32_t), b.who), corr(nr * 4 * sizeof(float), b.who), src(nr * sizeof(int32_t), b.who), mask(nr, b.who),
+        models(np * 9 * sizeof(float), b.who), counts(np * sizeof(int32_t), b.who);
+    for (size_t p = 0; p < np; ++p)
         if (!matches[p].empty())
-            rc = ps_host_to_dev(d_match + 3 * (size_t)start[p], matches[p].data(), matches[p].size() * sizeof(int32_t));
-    if (rc == PS_OK)
-        rc = ps_match_correspondences(dev, (int)sets.size(), d_feat.data(), d_rev.data(), n_desc.data(), (int)pairs.size(), flat.data(),
-                                      d_match, d_corr, d_src, n_corr.data());
+            check(ps_host_to_dev(static_cast<int32_t*>(match.p) + 3 * b.start[p], matches[p].data(), matches[p].size() * sizeof(int32_t)), b.who);
+    std::vector<int32_t> start(b.start.begin(), b.start.end()), n_corr(np, 0);
+    check(ps_match_correspondences(b.dev, (int)sets.size(), b.feat.data(), b.rev.data(), b.n_desc.data(), (int)np, b.flat.data(),
+                                   static_cast<const int32_t*>(match.p), static_cast<float*>(corr.p), static_cast<int32_t*>(src.p), n_corr.data()),
+          b.who);
     ps_verify_params prm;
     prm.model = params.model;
     prm.n_samples = params.n_samples;
     prm.threshold = params.threshold;
     prm.refine = params.refine ? 1 : 0;
     prm.seed = params.seed;
-    if (rc == PS_OK)
-        rc = ps_verify_batch(dev, (int)pairs.size(), d_corr, start.data(), n_corr.data(), &prm, d_models, d_n, d_mask, nullptr);
-    std::vector<float> models(pairs.size() * 9);
-    std::vector<int32_t> counts(pairs.size()), src(rows);
-    std::vector<uint8_t> mask(rows);
-    if (rc == PS_OK) rc = ps_dev_to_host(models.data(), d_models, models.size() * sizeof(float));
-    if (rc == PS_OK) rc = ps_dev_to_host(counts.data(), d_n, counts.size() * sizeof(int32_t));
-    if (rc == PS_OK && rows) rc = ps_dev_to_host(src.data(), d_src, rows * sizeof(int32_t));
-    if (rc == PS_OK && rows) rc = ps_dev_to_host(mask.data(), d_mask, rows);
-    release();
-    if (rc != PS_OK) throw std::runtime_error(std::string("popsift::verifyPairs failed: ") + ps_last_error(nullptr));
-    for (size_t p = 0; p < pairs.size(); ++p) {
-        std::copy(models.begin() + 9 * p, models.begin() + 9 * (p + 1), out[p].model);
-        out[p].n_inliers = counts[p];
+    check(ps_verify_batch(b.dev, (int)np, static_cast<const float*>(corr.p), start.data(), n_corr.data(), &prm, static_cast<float*>(models.p),
+                          static_cast<int32_t*>(counts.p), static_cast<uint8_t*>(mask.p), nullptr),
+          b.who);
+    std::vector<float> h_models(np * 9);
+    std::vector<int32_t> h_counts(np), h_src(b.rows);
+    std::vector<uint8_t> h_mask(b.rows);
+    check(ps_dev_to_host(h_models.data(), models.p, h_models.size() * sizeof(float)), b.who);
+    check(ps_dev_to_host(h_counts.data(), counts.p, h_counts.size() * sizeof(int32_t)), b.who);
+    check(ps_dev_to_host(h_src.data(), src.p, b.rows * sizeof(int32_t)), b.who);
+    check(ps_dev_to_host(h_mask.data(), mask.p, b.rows), b.who);
+    for (size_t p = 0; p < np; ++p) {
+        std::copy(h_models.begin() + 9 * p, h_models.begin() + 9 * (p + 1), out[p].model);
+        out[p].n_inliers = h_counts[p];
         for (int k = 0; k < n_corr[p]; ++k)
-            if (mask[(size_t)start[p] + k]) out[p].inlier_rows.push_back(src[(size_t)start[p] + k]);
+            if (h_mask[b.start[p] + k]) out[p].inlier_rows.push_back(h_src[b.start[p] + k]);
     }
     return out;
-}
-
-namespace {
-
-// matchPairsGuided / matchPairsGuidedU8: the C ABI call on the sets' descriptors (float) or their 8-bit copies
-std::vector<std::vector<int>> match_guided(const char* name, bool u8, const std::vector<FeaturesDev*>& sets,
-                                           const std::vector<std::pair<int, int>>& pairs, const std::vector<PairGeometry>& geometry,
-                                           const VerifyParams& params, int flags)
-{
-    const std::string who = std::string("popsift::") + name;
-    if (geometry.size() != pairs.size()) throw std::runtime_error(who + ": one geometry per pair expected");
-    std::vector<const ps_feature*> d_feat(sets.size());
-    std::vector<const int32_t*> d_rev(sets.size());
-    std::vector<int32_t> n_desc(sets.size());
-    for (size_t i = 0; i < sets.size(); ++i) {
-        if (!sets[i]) throw std::runtime_error(who + ": null set");
-        d_feat[i] = reinterpret_cast<const ps_feature*>(sets[i]->getFeatures());
-        d_rev[i] = sets[i]->getReverseMap();
-        n_desc[i] = std::max(sets[i]->getDescriptorCount(), 0);
-    }
-    std::vector<int32_t> flat(2 * pairs.size());
-    std::vector<std::vector<int>> out(pairs.size());
-    size_t rows = 0;
-    for (size_t p = 0; p < pairs.size(); ++p) {
-        const int l = pairs[p].first, r = pairs[p].second;
-        if (l < 0 || (size_t)l >= sets.size() || r < 0 || (size_t)r >= sets.size()) throw std::runtime_error(who + ": set index out of range");
-        flat[2 * p] = l; flat[2 * p + 1] = r;
-        out[p].assign((size_t)n_desc[l] * 3, 0);
-        rows += out[p].size() / 3;
-    }
-    if (rows == 0) return out;
-    int dev = 0;
-    for (size_t i = 0; i < sets.size(); ++i)
-        if (n_desc[i] > 0) { dev = std::max(0, ps_pointer_device(sets[i]->getDescriptors())); break; }
-    std::vector<void*> owned;
-    auto release = [&]() { for (void* p : owned) ps_dev_free(p); };
-    auto alloc = [&](size_t bytes) {
-        void* p = ps_dev_alloc(bytes);
-        if (!p) { release(); throw std::runtime_error(who + ": failed to allocate device memory"); }
-        owned.push_back(p);
-        return p;
-    };
-    std::vector<float> models(pairs.size() * 9);
-    for (size_t p = 0; p < pairs.size(); ++p) std::copy(geometry[p].model, geometry[p].model + 9, models.begin() + 9 * p);
-    float* d_models = static_cast<float*>(alloc(models.size() * sizeof(float)));
-    int32_t* d_out = static_cast<int32_t*>(alloc(rows * 3 * sizeof(int32_t)));
-    int rc = ps_host_to_dev(d_models, models.data(), models.size() * sizeof(float));
-    if (u8) {
-        // the 8-bit copies of every set (cudaMalloc: 256-byte aligned)
-        std::vector<const uint8_t*> d_sets(sets.size(), nullptr);
-        for (size_t i = 0; i < sets.size() && rc == PS_OK; ++i) {
-            if (n_desc[i] == 0) continue;
-            uint8_t* q = static_cast<uint8_t*>(alloc((size_t)n_desc[i] * 128));
-            d_sets[i] = q;
-            rc = ps_descriptors_to_u8(dev, reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors()), n_desc[i], q);
-        }
-        if (rc == PS_OK)
-            rc = ps_match_u8_guided_batch(dev, (int)sets.size(), d_sets.data(), d_feat.data(), d_rev.data(), n_desc.data(), (int)pairs.size(),
-                                          flat.data(), d_models, params.model, params.threshold, d_out, flags);
-    } else {
-        std::vector<const ps_descriptor*> d_sets(sets.size());
-        for (size_t i = 0; i < sets.size(); ++i) d_sets[i] = reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors());
-        if (rc == PS_OK)
-            rc = ps_match_guided_batch(dev, (int)sets.size(), d_sets.data(), d_feat.data(), d_rev.data(), n_desc.data(), (int)pairs.size(),
-                                       flat.data(), d_models, params.model, params.threshold, d_out, flags);
-    }
-    size_t row = 0;
-    for (size_t p = 0; p < pairs.size() && rc == PS_OK; ++p) {
-        rc = ps_dev_to_host(out[p].data(), d_out + 3 * row, out[p].size() * sizeof(int32_t));
-        row += out[p].size() / 3;
-    }
-    release();
-    if (rc != PS_OK) throw std::runtime_error(who + " failed: " + ps_last_error(nullptr));
-    return out;
-}
-
-} // namespace
-
-std::vector<std::vector<int>> matchPairsGuided(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
-                                               const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags)
-{
-    return match_guided("matchPairsGuided", false, sets, pairs, geometry, params, flags);
-}
-
-std::vector<std::vector<int>> matchPairsGuidedU8(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
-                                                 const std::vector<PairGeometry>& geometry, const VerifyParams& params, int flags)
-{
-    return match_guided("matchPairsGuidedU8", true, sets, pairs, geometry, params, flags);
 }
 
 void FeaturesHost::pin() {}
@@ -421,54 +360,15 @@ std::ostream& operator<<(std::ostream& ostr, const Feature& f)
     return ostr;
 }
 
-namespace {
-
-// the device pointers and counts of FeaturesDev sets, and the device of the first non-empty one
-int vlad_sets(const char* fn, const std::vector<FeaturesDev*>& sets, std::vector<const ps_descriptor*>& d_sets, std::vector<int32_t>& n_desc)
-{
-    d_sets.resize(sets.size());
-    n_desc.resize(sets.size());
-    int dev = -1;
-    for (size_t i = 0; i < sets.size(); ++i) {
-        if (!sets[i]) throw std::runtime_error(std::string(fn) + ": null set");
-        d_sets[i] = reinterpret_cast<const ps_descriptor*>(sets[i]->getDescriptors());
-        n_desc[i] = sets[i]->getDescriptorCount();
-        if (dev < 0 && n_desc[i] > 0) dev = std::max(0, ps_pointer_device(d_sets[i]));
-    }
-    return std::max(dev, 0);
-}
-
-// a device buffer freed at scope exit
-struct DevBuf {
-    void* p;
-    explicit DevBuf(size_t bytes, const char* fn) : p(ps_dev_alloc(std::max<size_t>(bytes, 16)))
-    {
-        if (!p) throw std::runtime_error(std::string(fn) + ": failed to allocate device memory");
-    }
-    ~DevBuf() { ps_dev_free(p); }
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
-};
-
-void check(int rc, const char* fn, const char* entry)
-{
-    if (rc != PS_OK) throw std::runtime_error(std::string(fn) + ": " + entry + " failed: " + ps_last_error(nullptr));
-}
-
-} // namespace
-
 std::vector<float> vladCodebook(const std::vector<FeaturesDev*>& sets, const VladParams& params, int flags)
 {
-    const char* fn = "popsift::vladCodebook";
-    std::vector<const ps_descriptor*> d_sets;
-    std::vector<int32_t> n_desc;
-    const int dev = vlad_sets(fn, sets, d_sets, n_desc);
+    const Batch b("vladCodebook", sets, {});
     const int k = std::max(params.k, 0);
-    DevBuf c((size_t)k * 128 * sizeof(float), fn);
-    check(ps_vlad_train(dev, (int)sets.size(), d_sets.data(), n_desc.data(), params.k, params.iters, params.seed,
-                        static_cast<float*>(c.p), flags), fn, "ps_vlad_train");
+    DevBuf c((size_t)k * 128 * sizeof(float), b.who);
+    check(ps_vlad_train(b.dev, (int)sets.size(), b.desc.data(), b.n_desc.data(), params.k, params.iters, params.seed,
+                        static_cast<float*>(c.p), flags), b.who, "ps_vlad_train");
     std::vector<float> out((size_t)k * 128);
-    check(ps_dev_to_host(out.data(), c.p, out.size() * sizeof(float)), fn, "ps_dev_to_host");
+    check(ps_dev_to_host(out.data(), c.p, out.size() * sizeof(float)), b.who, "ps_dev_to_host");
     return out;
 }
 
@@ -476,15 +376,13 @@ std::vector<float> vladEncode(const std::vector<FeaturesDev*>& sets, const std::
 {
     const char* fn = "popsift::vladEncode";
     if (codebook.empty() || codebook.size() % 128) throw std::runtime_error(std::string(fn) + ": the codebook is not k x 128 floats");
-    std::vector<const ps_descriptor*> d_sets;
-    std::vector<int32_t> n_desc;
-    const int dev = vlad_sets(fn, sets, d_sets, n_desc);
+    const Batch b("vladEncode", sets, {});
     const int k = (int)(codebook.size() / 128);
     std::vector<float> out(sets.size() * codebook.size());
     if (sets.empty()) return out;
     DevBuf c(codebook.size() * sizeof(float), fn), v(out.size() * sizeof(float), fn);
     check(ps_host_to_dev(c.p, codebook.data(), codebook.size() * sizeof(float)), fn, "ps_host_to_dev");
-    check(ps_vlad_encode(dev, (int)sets.size(), d_sets.data(), n_desc.data(), k, static_cast<const float*>(c.p),
+    check(ps_vlad_encode(b.dev, (int)sets.size(), b.desc.data(), b.n_desc.data(), k, static_cast<const float*>(c.p),
                          static_cast<float*>(v.p), nullptr, flags), fn, "ps_vlad_encode");
     check(ps_dev_to_host(out.data(), v.p, out.size() * sizeof(float)), fn, "ps_dev_to_host");
     return out;
@@ -499,7 +397,7 @@ std::vector<std::pair<int, int>> retrievePairs(const std::vector<float>& vectors
     const int dim = (int)(vectors.size() / n);
     DevBuf v(vectors.size() * sizeof(float), fn), nb((size_t)n * std::max(m, 1) * sizeof(int32_t), fn), sc((size_t)n * std::max(m, 1) * sizeof(float), fn);
     check(ps_host_to_dev(v.p, vectors.data(), vectors.size() * sizeof(float)), fn, "ps_host_to_dev");
-    check(ps_retrieve_pairs(0 <= ps_pointer_device(v.p) ? ps_pointer_device(v.p) : 0, n, static_cast<const float*>(v.p), dim, m,
+    check(ps_retrieve_pairs(std::max(0, ps_pointer_device(v.p)), n, static_cast<const float*>(v.p), dim, m,
                             static_cast<int32_t*>(nb.p), static_cast<float*>(sc.p)), fn, "ps_retrieve_pairs");
     std::vector<int32_t> nbr((size_t)n * m);
     check(ps_dev_to_host(nbr.data(), nb.p, nbr.size() * sizeof(int32_t)), fn, "ps_dev_to_host");

@@ -1048,80 +1048,105 @@ extern "C" int ps_pointer_device(const void* dev_ptr)
     return at.device;
 }
 
+namespace {
+
+bool set_device(int device)
+{
+    if (cudaSetDevice(device) == cudaSuccess) return true;
+    cudaGetLastError();
+    return false;
+}
+
+// the per-set checks of the batched entry points: no negative count, and every non-empty set's pointer non-null, on
+// `device` and aligned to align_mask + 1 bytes; *N (optional) = the pooled count
+template <class T>
+bool check_sets(int device, int n_sets, const int32_t* n_desc, const T* const* ptrs, uintptr_t align_mask, int64_t* N = nullptr)
+{
+    if (n_sets > 0 && (!n_desc || !ptrs)) return false;
+    int64_t total = 0;
+    for (int i = 0; i < n_sets; ++i) {
+        if (n_desc[i] < 0) return false;
+        if (n_desc[i] > 0 && (!ptrs[i] || (reinterpret_cast<uintptr_t>(ptrs[i]) & align_mask) || ps_pointer_device(ptrs[i]) != device))
+            return false;
+        total += n_desc[i];
+    }
+    if (N) *N = total;
+    return true;
+}
+
+// set indices in range; *rows = the left sets' rows summed over the pairs; *work (optional): some pair has rows and a
+// non-empty right set
+bool check_pairs(int n_sets, const int32_t* n_desc, const int32_t* pairs, int n_pairs, int64_t* rows, bool* work = nullptr)
+{
+    *rows = 0;
+    if (work) *work = false;
+    for (int p = 0; p < n_pairs; ++p) {
+        const int l = pairs[2 * p], r = pairs[2 * p + 1];
+        if (l < 0 || l >= n_sets || r < 0 || r >= n_sets) return false;
+        *rows += n_desc[l];
+        if (work) *work |= n_desc[l] > 0 && n_desc[r] > 0;
+    }
+    return true;
+}
+
+// the tail of every synchronous entry point: a run_* failure (launched < 0) keeps its message, otherwise wait for the
+// legacy stream and report what it returns as "<name>: <cuda error>"
+int finish(const char* name, int launched, const char* err)
+{
+    if (launched < 0) { g_create_error = err ? err : std::string(name) + " failed"; return PS_ERR_CUDA; }
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { g_create_error = std::string(name) + ": " + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
+    return PS_OK;
+}
+
+} // namespace
+
 extern "C" int ps_match(int device, const ps_descriptor* d_left, int n_left, const ps_descriptor* d_right, int n_right,
                         int32_t* d_out, int flags)
 {
     if (n_left < 0 || n_right < 0 || (n_left > 0 && (!d_left || !d_out)) || (n_right > 0 && !d_right)) return PS_ERR_ARG;
     if (n_left == 0) return PS_OK;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (!set_device(device)) return PS_ERR_CUDA;
     const char* err = nullptr;
     const int n = run_match(d_left, n_left, d_right, n_right, d_out, flags, nullptr, &err);
-    if (n < 0) { g_create_error = err ? err : "ps_match failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_match: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_match", n, err);
 }
 
 extern "C" int ps_match_batch(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc,
                               int n_pairs, const int32_t* pairs, int32_t* d_out, int flags)
 {
     if (n_sets < 0 || n_pairs < 0 || (n_sets > 0 && (!d_sets || !n_desc)) || (n_pairs > 0 && !pairs)) return PS_ERR_ARG;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
-    for (int i = 0; i < n_sets; ++i) {
-        if (n_desc[i] < 0) return PS_ERR_ARG;
-        if (n_desc[i] > 0 && (!d_sets[i] || ps_pointer_device(d_sets[i]) != device)) return PS_ERR_ARG;
-    }
+    if (!set_device(device)) return PS_ERR_CUDA;
     int64_t rows = 0;
-    for (int p = 0; p < n_pairs; ++p) {
-        const int l = pairs[2 * p], r = pairs[2 * p + 1];
-        if (l < 0 || l >= n_sets || r < 0 || r >= n_sets) return PS_ERR_ARG;
-        rows += n_desc[l];
-    }
+    if (!check_sets(device, n_sets, n_desc, d_sets, 0) || !check_pairs(n_sets, n_desc, pairs, n_pairs, &rows)) return PS_ERR_ARG;
     if (rows == 0) return PS_OK;
     if (!d_out) return PS_ERR_ARG;
     const char* err = nullptr;
     const int n = run_match_batch(d_sets, n_desc, n_sets, pairs, n_pairs, d_out, flags, nullptr, &err);
-    if (n < 0) { g_create_error = err ? err : "ps_match_batch failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_match_batch: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_match_batch", n, err);
 }
 
 extern "C" int ps_descriptors_to_u8(int device, const ps_descriptor* d_in, int n, uint8_t* d_out)
 {
     if (n < 0 || (n > 0 && (!d_in || !d_out))) return PS_ERR_ARG;
     if (n == 0) return PS_OK;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (!set_device(device)) return PS_ERR_CUDA;
     if (ps_pointer_device(d_in) != device || ps_pointer_device(d_out) != device) return PS_ERR_ARG;
-    run_descriptors_to_u8(d_in, n, d_out, nullptr);
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_descriptors_to_u8: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_descriptors_to_u8", run_descriptors_to_u8(d_in, n, d_out, nullptr), nullptr);
 }
 
 extern "C" int ps_match_u8_batch(int device, int n_sets, const uint8_t* const* d_sets, const int32_t* n_desc,
                                  int n_pairs, const int32_t* pairs, int32_t* d_out, int flags)
 {
     if (n_sets < 0 || n_pairs < 0 || (n_sets > 0 && (!d_sets || !n_desc)) || (n_pairs > 0 && !pairs)) return PS_ERR_ARG;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
-    for (int i = 0; i < n_sets; ++i) {
-        if (n_desc[i] < 0) return PS_ERR_ARG;
-        if (n_desc[i] > 0 && (!d_sets[i] || (reinterpret_cast<uintptr_t>(d_sets[i]) & 15u) || ps_pointer_device(d_sets[i]) != device)) return PS_ERR_ARG;
-    }
+    if (!set_device(device)) return PS_ERR_CUDA;
     int64_t rows = 0;
-    for (int p = 0; p < n_pairs; ++p) {
-        const int l = pairs[2 * p], r = pairs[2 * p + 1];
-        if (l < 0 || l >= n_sets || r < 0 || r >= n_sets) return PS_ERR_ARG;
-        rows += n_desc[l];
-    }
+    if (!check_sets(device, n_sets, n_desc, d_sets, 15u) || !check_pairs(n_sets, n_desc, pairs, n_pairs, &rows)) return PS_ERR_ARG;
     if (rows == 0) return PS_OK;
     if (!d_out) return PS_ERR_ARG;
     const char* err = nullptr;
     const int n = run_match_u8_batch(d_sets, n_desc, n_sets, pairs, n_pairs, d_out, flags, nullptr, &err);
-    if (n < 0) { g_create_error = err ? err : "ps_match_u8_batch failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_match_u8_batch: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_match_u8_batch", n, err);
 }
 
 extern "C" int ps_match_correspondences(int device, int n_sets, const ps_feature* const* d_feat, const int32_t* const* d_rev,
@@ -1129,17 +1154,11 @@ extern "C" int ps_match_correspondences(int device, int n_sets, const ps_feature
                                         float* d_corr, int32_t* d_src, int32_t* n_corr)
 {
     if (n_sets < 0 || n_pairs < 0 || (n_sets > 0 && (!d_feat || !d_rev || !n_desc)) || (n_pairs > 0 && (!pairs || !n_corr))) return PS_ERR_ARG;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
-    for (int i = 0; i < n_sets; ++i) {
-        if (n_desc[i] < 0) return PS_ERR_ARG;
-        if (n_desc[i] > 0 && (ps_pointer_device(d_feat[i]) != device || ps_pointer_device(d_rev[i]) != device)) return PS_ERR_ARG;
-    }
+    if (!set_device(device)) return PS_ERR_CUDA;
     int64_t rows = 0;
-    for (int p = 0; p < n_pairs; ++p) {
-        const int l = pairs[2 * p], r = pairs[2 * p + 1];
-        if (l < 0 || l >= n_sets || r < 0 || r >= n_sets) return PS_ERR_ARG;
-        rows += n_desc[l];
-    }
+    if (!check_sets(device, n_sets, n_desc, d_feat, 0) || !check_sets(device, n_sets, n_desc, d_rev, 0) ||
+        !check_pairs(n_sets, n_desc, pairs, n_pairs, &rows))
+        return PS_ERR_ARG;
     if (rows == 0) {
         for (int p = 0; p < n_pairs; ++p) n_corr[p] = 0;
         return PS_OK;
@@ -1148,10 +1167,7 @@ extern "C" int ps_match_correspondences(int device, int n_sets, const ps_feature
     if (ps_pointer_device(d_match) != device || ps_pointer_device(d_corr) != device || ps_pointer_device(d_src) != device) return PS_ERR_ARG;
     const char* err = nullptr;
     const int n = run_match_correspondences(d_feat, d_rev, n_desc, pairs, n_pairs, d_match, d_corr, d_src, n_corr, nullptr, &err);
-    if (n < 0) { g_create_error = err ? err : "ps_match_correspondences failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_match_correspondences: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_match_correspondences", n, err);
 }
 
 extern "C" int ps_verify_batch(int device, int n_pairs, const float* d_corr, const int32_t* corr_start, const int32_t* n_corr,
@@ -1170,17 +1186,14 @@ extern "C" int ps_verify_batch(int device, int n_pairs, const float* d_corr, con
         if (corr_start[p] < 0 || n_corr[p] < 0) return PS_ERR_ARG;
         rows = std::max<int64_t>(rows, (int64_t)corr_start[p] + n_corr[p]);
     }
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (!set_device(device)) return PS_ERR_CUDA;
     if (ps_pointer_device(d_models) != device || ps_pointer_device(d_n_inliers) != device) return PS_ERR_ARG;
     if (rows > 0 && (ps_pointer_device(d_corr) != device || ps_pointer_device(d_inlier_mask) != device)) return PS_ERR_ARG;
     if (rows > 0 && (reinterpret_cast<uintptr_t>(d_corr) & 15u)) return PS_ERR_ARG;
     if (taps && (ps_pointer_device(taps->d_counts) != device || ps_pointer_device(taps->d_models) != device)) return PS_ERR_ARG;
     const char* err = nullptr;
     const int n = run_verify_batch(n_pairs, d_corr, corr_start, n_corr, *prm, d_models, d_n_inliers, d_inlier_mask, taps, nullptr, &err);
-    if (n < 0) { g_create_error = err ? err : "ps_verify_batch failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_verify_batch: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_verify_batch", n, err);
 }
 
 // both guided entry points: the argument checks of ps_match_batch / ps_match_u8_batch and ps_match_correspondences, the
@@ -1192,22 +1205,12 @@ static int match_guided(const char* name, bool u8, int device, int n_sets, const
     if (n_sets < 0 || n_pairs < 0 || (n_sets > 0 && (!d_sets || !d_feat || !d_rev || !n_desc)) || (n_pairs > 0 && !pairs)) return PS_ERR_ARG;
     if (model != PS_GEOM_HOMOGRAPHY && model != PS_GEOM_FUNDAMENTAL) return PS_ERR_ARG;
     if (!std::isfinite(threshold) || !(threshold > 0.0f)) return PS_ERR_ARG;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
-    for (int i = 0; i < n_sets; ++i) {
-        if (n_desc[i] < 0) return PS_ERR_ARG;
-        if (n_desc[i] == 0) continue;
-        if (!d_sets[i] || ps_pointer_device(d_sets[i]) != device) return PS_ERR_ARG;
-        if (u8 && (reinterpret_cast<uintptr_t>(d_sets[i]) & 15u)) return PS_ERR_ARG;
-        if (ps_pointer_device(d_feat[i]) != device || ps_pointer_device(d_rev[i]) != device) return PS_ERR_ARG;
-    }
+    if (!set_device(device)) return PS_ERR_CUDA;
     int64_t rows = 0;
-    bool work = false;                                    // some pair has rows and a non-empty right set
-    for (int p = 0; p < n_pairs; ++p) {
-        const int l = pairs[2 * p], r = pairs[2 * p + 1];
-        if (l < 0 || l >= n_sets || r < 0 || r >= n_sets) return PS_ERR_ARG;
-        rows += n_desc[l];
-        work |= n_desc[l] > 0 && n_desc[r] > 0;
-    }
+    bool work = false;
+    if (!check_sets(device, n_sets, n_desc, d_sets, u8 ? 15u : 0u) || !check_sets(device, n_sets, n_desc, d_feat, 0) ||
+        !check_sets(device, n_sets, n_desc, d_rev, 0) || !check_pairs(n_sets, n_desc, pairs, n_pairs, &rows, &work))
+        return PS_ERR_ARG;
     if (rows == 0) return PS_OK;
     if (!d_out) return PS_ERR_ARG;
     if (work && ps_pointer_device(d_models) != device) return PS_ERR_ARG;
@@ -1216,10 +1219,7 @@ static int match_guided(const char* name, bool u8, int device, int n_sets, const
                                                  d_models, model, threshold, d_out, flags, nullptr, &err)
                      : run_match_guided_batch(reinterpret_cast<const ps_descriptor* const*>(d_sets), d_feat, d_rev, n_desc, n_sets, pairs,
                                               n_pairs, d_models, model, threshold, d_out, flags, nullptr, &err);
-    if (n < 0) { g_create_error = err ? err : std::string(name) + " failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string(name) + ": " + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish(name, n, err);
 }
 
 extern "C" int ps_match_guided_batch(int device, int n_sets, const ps_descriptor* const* d_sets, const ps_feature* const* d_feat,
@@ -1238,53 +1238,33 @@ extern "C" int ps_match_u8_guided_batch(int device, int n_sets, const uint8_t* c
                         n_desc, n_pairs, pairs, d_models, model, threshold, d_out, flags);
 }
 
-// the set checks of ps_match_batch and the codebook size, for both VLAD entry points; *N = the pool size
-static int vlad_sets(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc, int k, int64_t* N)
-{
-    if (n_sets < 0 || (n_sets > 0 && (!d_sets || !n_desc)) || k < 1 || k > 1024) return PS_ERR_ARG;
-    *N = 0;
-    for (int i = 0; i < n_sets; ++i) {
-        if (n_desc[i] < 0) return PS_ERR_ARG;
-        if (n_desc[i] > 0 && (!d_sets[i] || ps_pointer_device(d_sets[i]) != device)) return PS_ERR_ARG;
-        *N += n_desc[i];
-    }
-    return PS_OK;
-}
-
 extern "C" int ps_vlad_train(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc, int k, int iters,
                              uint64_t seed, float* d_centroids, int flags)
 {
     if (n_sets < 0 || k < 1 || k > 1024 || iters < 0 || iters > 1000) return PS_ERR_ARG;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (!set_device(device)) return PS_ERR_CUDA;
     int64_t N = 0;
-    if (vlad_sets(device, n_sets, d_sets, n_desc, k, &N) != PS_OK) return PS_ERR_ARG;
-    if (N < k || N >= 0x80000000LL) return PS_ERR_ARG;
+    if (!check_sets(device, n_sets, n_desc, d_sets, 0, &N) || N < k || N >= 0x80000000LL) return PS_ERR_ARG;
     if (ps_pointer_device(d_centroids) != device) return PS_ERR_ARG;
     const char* err = nullptr;
     const int n = run_vlad_train(d_sets, n_desc, n_sets, k, iters, seed, d_centroids, flags, nullptr, &err);
-    if (n < 0) { g_create_error = err ? err : "ps_vlad_train failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_vlad_train: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_vlad_train", n, err);
 }
 
 extern "C" int ps_vlad_encode(int device, int n_sets, const ps_descriptor* const* d_sets, const int32_t* n_desc, int k,
                               const float* d_centroids, float* d_vlad, int32_t* d_assign, int flags)
 {
     if (n_sets < 0 || k < 1 || k > 1024) return PS_ERR_ARG;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (!set_device(device)) return PS_ERR_CUDA;
     int64_t N = 0;
-    if (vlad_sets(device, n_sets, d_sets, n_desc, k, &N) != PS_OK) return PS_ERR_ARG;
+    if (!check_sets(device, n_sets, n_desc, d_sets, 0, &N)) return PS_ERR_ARG;
     if (n_sets == 0) return PS_OK;
     if (N >= 0x80000000LL) return PS_ERR_ARG;
     if (ps_pointer_device(d_centroids) != device || ps_pointer_device(d_vlad) != device) return PS_ERR_ARG;
     if (d_assign && N > 0 && ps_pointer_device(d_assign) != device) return PS_ERR_ARG;
     const char* err = nullptr;
     const int n = run_vlad_encode(d_sets, n_desc, n_sets, k, d_centroids, d_vlad, d_assign, flags, nullptr, &err);
-    if (n < 0) { g_create_error = err ? err : "ps_vlad_encode failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_vlad_encode: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_vlad_encode", n, err);
 }
 
 extern "C" int ps_retrieve_pairs(int device, int n, const float* d_vec, int dim, int m, int32_t* d_nbr, float* d_score)
@@ -1292,15 +1272,12 @@ extern "C" int ps_retrieve_pairs(int device, int n, const float* d_vec, int dim,
     if (n < 0 || dim <= 0 || (dim & 3) || m < 1 || m > 128) return PS_ERR_ARG;
     if (n == 0) return PS_OK;
     if ((int64_t)n * m >= 0x80000000LL) return PS_ERR_ARG;
-    if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return PS_ERR_CUDA; }
+    if (!set_device(device)) return PS_ERR_CUDA;
     if (reinterpret_cast<uintptr_t>(d_vec) & 15u) return PS_ERR_ARG;
     if (ps_pointer_device(d_vec) != device || ps_pointer_device(d_nbr) != device || ps_pointer_device(d_score) != device) return PS_ERR_ARG;
     const char* err = nullptr;
     const int r = run_retrieve_pairs(n, d_vec, dim, m, d_nbr, d_score, nullptr, &err);
-    if (r < 0) { g_create_error = err ? err : "ps_retrieve_pairs failed"; return PS_ERR_CUDA; }
-    const cudaError_t e = cudaStreamSynchronize(nullptr);
-    if (e != cudaSuccess) { g_create_error = std::string("ps_retrieve_pairs: ") + cudaGetErrorString(e); cudaGetLastError(); return PS_ERR_CUDA; }
-    return PS_OK;
+    return finish("ps_retrieve_pairs", r, err);
 }
 
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)
