@@ -189,4 +189,23 @@ std::vector<float> vladEncode(const std::vector<FeaturesDev*>& sets, const std::
 /// result is the union of the unordered pairs (i, j), i < j, sorted.
 std::vector<std::pair<int, int>> retrievePairs(const std::vector<float>& vectors, int n, int m);
 
+/// Feature tracks (C ABI ps_tracks_from_matches in popsift_b200_tracks.h): the connected components of the matches over
+/// all features of all sets, without those holding two features of one set and those shorter than min_length (>= 2).
+/// Track t's members are set[k] / feature[k] for k in [start[t], start[t + 1]), ascending by set; tracks are sorted by
+/// their smallest member; track_of[i][f] is feature f of set i's track, or -1.
+struct Tracks
+{
+    std::vector<int>              start, set, feature;
+    std::vector<std::vector<int>> track_of;
+    int                           n_components = 0, n_conflicting = 0, n_short = 0;
+};
+
+/// Tracks of the verified inliers: `matches` and `geometry` are what matchPairs(U8) and verifyPairs gave for the same sets
+/// and pairs, and the edges are geometry[p].inlier_rows.  Throws like verifyPairs.
+Tracks buildTracks(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                   const std::vector<std::vector<int>>& matches, const std::vector<PairGeometry>& geometry, int min_length = 2);
+/// Tracks of every correspondence of `matches`: the rows of matchPairsGuided(U8), which already passed the model.
+Tracks buildTracks(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                   const std::vector<std::vector<int>>& matches, int min_length = 2);
+
 } // namespace popsift

@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from collections import namedtuple
 from typing import Optional
 
 import numpy as np
@@ -68,7 +69,13 @@ class PsVerifyTaps(C.Structure):
     _fields_ = [("d_counts", C.c_void_p), ("d_models", C.c_void_p)]
 
 
-assert C.sizeof(PsVerifyParams) == 24
+class PsTrackCounts(C.Structure):
+    """ps_track_counts (20 bytes)"""
+    _fields_ = [("n_tracks", C.c_int32), ("n_members", C.c_int32), ("n_components", C.c_int32), ("n_conflicting", C.c_int32),
+                ("n_short", C.c_int32)]
+
+
+assert C.sizeof(PsVerifyParams) == 24 and C.sizeof(PsTrackCounts) == 20
 
 EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps_geometry", "ps_create", "ps_destroy",
            "ps_last_error", "ps_submit_u8", "ps_submit_f32", "ps_submit_dev_u8", "ps_counts", "ps_download",
@@ -81,6 +88,8 @@ EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps
 GUIDED_EXPORTS = ["ps_match_guided_batch", "ps_match_u8_guided_batch"]
 # image retrieval, declared in popsift_b200_retrieval.h (same library)
 RETRIEVAL_EXPORTS = ["ps_vlad_train", "ps_vlad_encode", "ps_retrieve_pairs"]
+# feature tracks, declared in popsift_b200_tracks.h (same library)
+TRACKS_EXPORTS = ["ps_tracks_from_edges", "ps_tracks_from_matches"]
 
 _lib = None
 
@@ -132,6 +141,12 @@ def load_library():
         L.ps_vlad_train.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_int]
         L.ps_vlad_encode.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.ps_retrieve_pairs.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    if hasattr(L, "ps_tracks_from_edges"):
+        L.ps_tracks_from_edges.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.POINTER(PsTrackCounts)]
+        L.ps_tracks_from_matches.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.POINTER(PsTrackCounts)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -638,13 +653,14 @@ def _correspondences_dev(lib, bufs, sets, pairs, d_match, device):
     return d_corr, d_src, start[:len(pairs)].copy(), n_corr[:len(pairs)].copy()
 
 
-def _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm: PsVerifyParams, taps=False, d_models=None):
+def _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm: PsVerifyParams, taps=False, d_models=None, d_mask=None):
     """ps_verify_batch: host (models (P, 3, 3), counts (P,), mask (rows,) bool[, tap counts, tap models]); the models are
-    written to d_models (P x 9 floats of device memory) when given"""
+    written to d_models (P x 9 floats of device memory) and the mask to d_mask (a byte per row) when given"""
     P = len(start)
     rows = int(max((int(a) + int(b) for a, b in zip(start, n_corr)), default=0))
     d_models = bufs.alloc(P * 36) if d_models is None else d_models
-    d_n, d_mask = bufs.alloc(P * 4), bufs.alloc(rows)
+    d_n = bufs.alloc(P * 4)
+    d_mask = bufs.alloc(rows) if d_mask is None else d_mask
     k = 1 if prm.model == 0 else 3
     tp = None
     if taps:
@@ -717,6 +733,30 @@ def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, guid
     lib = load_library()
     pairs = [(int(a), int(b)) for a, b in pairs]
     prm = _verify_params(**params)
+    bufs = _DevBuffers(lib)
+    try:
+        ch = _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, prm)
+        src = bufs.download(ch.d_src, ch.rows, np.int32)
+    finally:
+        bufs.free()
+    out = []
+    for p in range(len(pairs)):
+        a, n = int(ch.start[p]), int(ch.n_corr[p])
+        if guided:
+            out.append((ch.models[p], n, src[a:a + n].copy()))
+        else:
+            out.append((ch.models[p], int(ch.n_in[p]), src[a:a + n][ch.mask[a:a + n]].copy()))
+    return out
+
+
+_Chain = namedtuple("_Chain", "device rows d_match d_src start n_corr d_mask models n_in mask")
+
+
+def _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, prm) -> _Chain:
+    """verify_pairs' device chain: match_pairs (match_pairs_u8) unless `matches` is given, ps_match_correspondences,
+    ps_verify_batch, and with guided=True guided matching and the correspondences again.  Device arrays in bufs: d_match,
+    the rows the final correspondences came from; d_src, start, n_corr, those correspondences; d_mask, the verification's
+    inlier mask, or None after guided matching (every guided correspondence passed the model).  Host: models, n_in, mask."""
     counts = [s.getDescriptorCount() for s in sets]
     for l, r in pairs:
         if not (0 <= l < len(sets) and 0 <= r < len(sets)):
@@ -724,35 +764,94 @@ def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, guid
     if matches is not None and len(matches) != len(pairs):
         raise PopSiftError("one match array per pair expected")
     rows = sum(counts[l] for l, _ in pairs)
+    # the 8-bit copies are made only when matching uses them
+    descs = _desc_sets(lib, bufs, sets, device, u8 and (matches is None or guided))
+    c_sets, c_n, _, device = descs
+    if matches is not None:
+        m = np.concatenate([np.asarray(r, np.int32).reshape(-1, 3) for r in matches]) if matches else np.zeros((0, 3), np.int32)
+        d_match = bufs.upload(m)
+    else:
+        d_match = bufs.alloc(rows * 12)
+        fn = lib.ps_match_u8_batch if u8 else lib.ps_match_batch
+        _check(lib, fn(device, len(sets), c_sets, c_n, len(pairs), _c_pairs(pairs), d_match, flags), "matching")
+    d_corr, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_match, device)
+    d_models, d_mask = bufs.alloc(len(pairs) * 36), bufs.alloc(rows)
+    models, n_in, mask = _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm, d_models=d_models, d_mask=d_mask)
+    if guided:
+        d_match = _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, prm.model, prm.threshold, flags, u8)
+        _, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_match, device)
+        d_mask = mask = None
+    return _Chain(device, rows, d_match, d_src, start, n_corr, d_mask, models, n_in, mask)
+
+
+Tracks = namedtuple("Tracks", "start set feature track_of n_components n_conflicting n_short")
+Tracks.__doc__ = """Feature tracks: track t's members are set[start[t]:start[t + 1]] / feature[start[t]:start[t + 1]]
+(ascending by set); track_of[i][f] is feature f of set i's track, or -1; the counts of dropped components."""
+
+
+def _tracks_dev(lib, bufs, n_feat, min_length, call) -> Tracks:
+    """the outputs of a track entry point: `call(d_track_of, d_track_start, d_members, counts)` returns its code"""
+    n_feat = [int(n) for n in n_feat]
+    off = np.concatenate([[0], np.cumsum(n_feat, dtype=np.int64)]).astype(np.int64)
+    N = int(off[-1])
+    cap = N // max(int(min_length), 2) + 1
+    d_of, d_start, d_mem = bufs.alloc(N * 4), bufs.alloc(cap * 4), bufs.alloc(N * 4)
+    cnt = PsTrackCounts()
+    _check(lib, call(d_of, d_start, d_mem, cnt), "tracks")
+    start = bufs.download(d_start, cnt.n_tracks + 1, np.int32)
+    mem = bufs.download(d_mem, cnt.n_members, np.int32)
+    of = bufs.download(d_of, N, np.int32)
+    s = (np.searchsorted(off, mem, side="right") - 1).astype(np.int32)
+    return Tracks(start, s, (mem - off[s]).astype(np.int32), [of[off[i]:off[i + 1]] for i in range(len(n_feat))],
+                  cnt.n_components, cnt.n_conflicting, cnt.n_short)
+
+
+def build_tracks(n_feat, edges, min_length=2, device=0) -> Tracks:
+    """Feature tracks of an explicit edge list (C ABI ps_tracks_from_edges in popsift_b200_tracks.h; an addition to the
+    reference's interface): the connected components of the edges over all features, without those holding two features
+    of one set and those shorter than min_length (>= 2).  `n_feat` is each set's feature count, `edges` an (E, 4) int32
+    array of (set_a, feature_a, set_b, feature_b)."""
+    lib = load_library()
+    n_feat = [int(n) for n in n_feat]
+    e = np.ascontiguousarray(edges, np.int64).reshape(-1, 4)
+    nf = np.asarray(n_feat + [0], np.int64)
+    for s, f in ((e[:, 0], e[:, 1]), (e[:, 2], e[:, 3])):
+        if ((s < 0) | (s >= len(n_feat))).any() or ((f < 0) | (f >= nf[np.clip(s, 0, len(n_feat))])).any():
+            raise PopSiftError("edge endpoint out of range")
+    off = np.concatenate([[0], np.cumsum(n_feat, dtype=np.int64)])
+    g = np.stack([off[e[:, 0]] + e[:, 1], off[e[:, 2]] + e[:, 3]], axis=1).astype(np.int32)
+    c_n = (C.c_int32 * max(len(n_feat), 1))(*n_feat)
     bufs = _DevBuffers(lib)
     try:
-        # the 8-bit copies are made only when matching uses them
-        descs = _desc_sets(lib, bufs, sets, device, u8 and (matches is None or guided))
-        c_sets, c_n, _, device = descs
-        if matches is not None:
-            m = np.concatenate([np.asarray(r, np.int32).reshape(-1, 3) for r in matches]) if matches else np.zeros((0, 3), np.int32)
-            d_match = bufs.upload(m)
-        else:
-            d_match = bufs.alloc(rows * 12)
-            fn = lib.ps_match_u8_batch if u8 else lib.ps_match_batch
-            _check(lib, fn(device, len(sets), c_sets, c_n, len(pairs), _c_pairs(pairs), d_match, flags), "matching")
-        d_corr, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_match, device)
-        if guided:
-            d_models = bufs.alloc(len(pairs) * 36)
-            models, n_in, mask = _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm, d_models=d_models)
-            d_guided = _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, prm.model, prm.threshold, flags, u8)
-            _, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_guided, device)
-            src = bufs.download(d_src, rows, np.int32)
-            return [(models[p], int(n_corr[p]), src[int(start[p]):int(start[p]) + int(n_corr[p])].copy()) for p in range(len(pairs))]
-        models, n_in, mask = _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm)
-        src = bufs.download(d_src, rows, np.int32)
+        d_e = bufs.upload(g)
+        return _tracks_dev(lib, bufs, n_feat, min_length, lambda of, st, mem, cnt: lib.ps_tracks_from_edges(
+            device, len(n_feat), c_n, len(g), d_e, int(min_length), of, st, mem, C.byref(cnt)))
     finally:
         bufs.free()
-    out = []
-    for p in range(len(pairs)):
-        a, n = int(start[p]), int(n_corr[p])
-        out.append((models[p], int(n_in[p]), src[a:a + n][mask[a:a + n]].copy()))
-    return out
+
+
+def tracks(sets, pairs, matches=None, min_length=2, guided=False, u8=False, flags=0, device=None, **verify_params) -> Tracks:
+    """Feature tracks of a whole SfM front end on the device (C ABI ps_tracks_from_matches in popsift_b200_tracks.h):
+    verify_pairs' chain on FeaturesDev `sets` and `pairs` (match, correspond, verify with verify_params; guided matching with
+    guided=True), then the tracks of its verified inliers (of every guided correspondence with guided=True).  Only the
+    tracks come back."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    prm = _verify_params(**verify_params)
+    bufs = _DevBuffers(lib)
+    try:
+        ch = _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, prm)
+        n = max(len(sets), 1)
+        n_feat = [s.getFeatureCount() for s in sets]
+        c_nf = (C.c_int32 * n)(*n_feat)
+        c_rev = (C.c_void_p * n)(*[s.getReverseMap() for s in sets])
+        c_nd = (C.c_int32 * n)(*[s.getDescriptorCount() for s in sets])
+        c_corr = np.ascontiguousarray(ch.n_corr, np.int32)
+        return _tracks_dev(lib, bufs, n_feat, min_length, lambda of, st, mem, cnt: lib.ps_tracks_from_matches(
+            ch.device, len(sets), c_nf, c_rev, c_nd, len(pairs), _c_pairs(pairs), ch.d_match, ch.d_src, c_corr.ctypes.data,
+            ch.d_mask, int(min_length), of, st, mem, C.byref(cnt)))
+    finally:
+        bufs.free()
 
 
 def _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, model, threshold, flags, u8) -> int:

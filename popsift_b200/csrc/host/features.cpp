@@ -6,6 +6,7 @@
 #include "popsift_b200.h"
 #include "popsift_b200_guided.h"
 #include "popsift_b200_retrieval.h"
+#include "popsift_b200_tracks.h"
 
 #include <algorithm>
 #include <cmath>
@@ -148,6 +149,16 @@ struct Batch {
 
     size_t pair_rows(size_t p) const { return (size_t)std::max(n_desc[flat[2 * p]], 0); }
 
+    // the caller's rows of every pair (3 ints per left descriptor) into d (rows x 3 int32 of device memory)
+    void upload(const std::vector<std::vector<int>>& matches, int32_t* d) const
+    {
+        if (matches.size() != start.size()) throw std::runtime_error(who + ": one match list per pair expected");
+        for (size_t p = 0; p < start.size(); ++p)
+            if (matches[p].size() != pair_rows(p) * 3) throw std::runtime_error(who + ": match rows do not fit the left set");
+        for (size_t p = 0; p < start.size(); ++p)
+            if (!matches[p].empty()) check(ps_host_to_dev(d + 3 * start[p], matches[p].data(), matches[p].size() * sizeof(int32_t)), who);
+    }
+
     // the 8-bit copies of all sets, back to back in q (128-byte rows keep every set 16-byte aligned)
     std::vector<const uint8_t*> to_u8(uint8_t* q) const
     {
@@ -283,18 +294,15 @@ std::vector<PairGeometry> verifyPairs(const std::vector<FeaturesDev*>& sets, con
 {
     if (matches.size() != pairs.size()) throw std::runtime_error("popsift::verifyPairs: one match list per pair expected");
     const Batch b("verifyPairs", sets, pairs);
-    for (size_t p = 0; p < pairs.size(); ++p)
-        if (matches[p].size() != b.pair_rows(p) * 3) throw std::runtime_error(b.who + ": match rows do not fit the left set");
     std::vector<PairGeometry> out(pairs.size());
     for (PairGeometry& g : out) { std::fill(g.model, g.model + 9, 0.0f); g.n_inliers = 0; }
-    if (pairs.empty()) return out;
     // device buffers: match rows, correspondences (16-byte rows), source rows, masks; models and counts per pair
     const size_t nr = std::max<size_t>(b.rows, 1), np = pairs.size();
-    DevBuf match(nr * 3 * sizeof(int32_t), b.who), corr(nr * 4 * sizeof(float), b.who), src(nr * sizeof(int32_t), b.who), mask(nr, b.who),
+    DevBuf match(nr * 3 * sizeof(int32_t), b.who);
+    b.upload(matches, static_cast<int32_t*>(match.p));
+    if (pairs.empty()) return out;
+    DevBuf corr(nr * 4 * sizeof(float), b.who), src(nr * sizeof(int32_t), b.who), mask(nr, b.who),
         models(np * 9 * sizeof(float), b.who), counts(np * sizeof(int32_t), b.who);
-    for (size_t p = 0; p < np; ++p)
-        if (!matches[p].empty())
-            check(ps_host_to_dev(static_cast<int32_t*>(match.p) + 3 * b.start[p], matches[p].data(), matches[p].size() * sizeof(int32_t)), b.who);
     std::vector<int32_t> start(b.start.begin(), b.start.end()), n_corr(np, 0);
     check(ps_match_correspondences(b.dev, (int)sets.size(), b.feat.data(), b.rev.data(), b.n_desc.data(), (int)np, b.flat.data(),
                                    static_cast<const int32_t*>(match.p), static_cast<float*>(corr.p), static_cast<int32_t*>(src.p), n_corr.data()),
@@ -409,6 +417,82 @@ std::vector<std::pair<int, int>> retrievePairs(const std::vector<float>& vectors
     std::sort(out.begin(), out.end());
     out.erase(std::unique(out.begin(), out.end()), out.end());
     return out;
+}
+
+namespace {
+
+// both buildTracks: the match rows on the device, then the correspondences -- the inlier rows of `geometry`, or (none
+// given) those ps_match_correspondences gathers -- and ps_tracks_from_matches over them without a mask
+Tracks build_tracks(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                    const std::vector<std::vector<int>>& matches, const std::vector<PairGeometry>* geometry, int min_length)
+{
+    if (geometry && geometry->size() != pairs.size()) throw std::runtime_error("popsift::buildTracks: one geometry per pair expected");
+    const Batch b("buildTracks", sets, pairs);
+    const size_t nr = std::max<size_t>(b.rows, 1), np = pairs.size();
+    DevBuf match(nr * 3 * sizeof(int32_t), b.who), src(nr * sizeof(int32_t), b.who);
+    b.upload(matches, static_cast<int32_t*>(match.p));
+    std::vector<int32_t> n_corr(np, 0);
+    if (geometry) {
+        std::vector<int32_t> h_src(b.rows);
+        for (size_t p = 0; p < np; ++p) {
+            const std::vector<int>& in = (*geometry)[p].inlier_rows;
+            if (in.size() > b.pair_rows(p)) throw std::runtime_error(b.who + ": more inlier rows than left descriptors");
+            std::copy(in.begin(), in.end(), h_src.begin() + b.start[p]);
+            n_corr[p] = (int32_t)in.size();
+        }
+        check(ps_host_to_dev(src.p, h_src.data(), h_src.size() * sizeof(int32_t)), b.who);
+    } else if (np > 0) {
+        DevBuf corr(nr * 4 * sizeof(float), b.who);
+        check(ps_match_correspondences(b.dev, (int)sets.size(), b.feat.data(), b.rev.data(), b.n_desc.data(), (int)np, b.flat.data(),
+                                       static_cast<const int32_t*>(match.p), static_cast<float*>(corr.p), static_cast<int32_t*>(src.p),
+                                       n_corr.data()),
+              b.who);
+    }
+    std::vector<int32_t> n_feat(sets.size());
+    std::vector<size_t> off(sets.size() + 1, 0);
+    for (size_t i = 0; i < sets.size(); ++i) {
+        n_feat[i] = sets[i]->getFeatureCount();
+        off[i + 1] = off[i] + (size_t)std::max(n_feat[i], 0);
+    }
+    const size_t N = off.back();
+    DevBuf track_of(N * sizeof(int32_t), b.who), track_start((N / std::max(min_length, 2) + 1) * sizeof(int32_t), b.who),
+        members(N * sizeof(int32_t), b.who);
+    ps_track_counts c;
+    check(ps_tracks_from_matches(b.dev, (int)sets.size(), n_feat.data(), b.rev.data(), b.n_desc.data(), (int)np, b.flat.data(),
+                                 static_cast<const int32_t*>(match.p), static_cast<const int32_t*>(src.p), n_corr.data(), nullptr,
+                                 min_length, static_cast<int32_t*>(track_of.p), static_cast<int32_t*>(track_start.p),
+                                 static_cast<int32_t*>(members.p), &c),
+          b.who, "ps_tracks_from_matches");
+    Tracks t;
+    t.start.resize((size_t)c.n_tracks + 1);
+    std::vector<int32_t> mem((size_t)c.n_members), of(N);
+    check(ps_dev_to_host(t.start.data(), track_start.p, t.start.size() * sizeof(int32_t)), b.who);
+    check(ps_dev_to_host(mem.data(), members.p, mem.size() * sizeof(int32_t)), b.who);
+    check(ps_dev_to_host(of.data(), track_of.p, of.size() * sizeof(int32_t)), b.who);
+    for (const int32_t g : mem) {
+        const size_t s = (size_t)(std::upper_bound(off.begin(), off.end(), (size_t)g) - off.begin()) - 1;
+        t.set.push_back((int)s);
+        t.feature.push_back((int)(g - off[s]));
+    }
+    for (size_t i = 0; i < sets.size(); ++i) t.track_of.emplace_back(of.begin() + off[i], of.begin() + off[i + 1]);
+    t.n_components = c.n_components;
+    t.n_conflicting = c.n_conflicting;
+    t.n_short = c.n_short;
+    return t;
+}
+
+} // namespace
+
+Tracks buildTracks(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                   const std::vector<std::vector<int>>& matches, const std::vector<PairGeometry>& geometry, int min_length)
+{
+    return build_tracks(sets, pairs, matches, &geometry, min_length);
+}
+
+Tracks buildTracks(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                   const std::vector<std::vector<int>>& matches, int min_length)
+{
+    return build_tracks(sets, pairs, matches, nullptr, min_length);
 }
 
 } // namespace popsift

@@ -10,6 +10,7 @@
 #include "ps_internal.h"
 #include "popsift_b200_guided.h"
 #include "popsift_b200_retrieval.h"
+#include "popsift_b200_tracks.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1278,6 +1279,77 @@ extern "C" int ps_retrieve_pairs(int device, int n, const float* d_vec, int dim,
     const char* err = nullptr;
     const int r = run_retrieve_pairs(n, d_vec, dim, m, d_nbr, d_score, nullptr, &err);
     return finish("ps_retrieve_pairs", r, err);
+}
+
+// both track entry points: the feature counts (none negative, N < 2^31), min_length, counts and the outputs; *N = the
+// number of features
+static bool check_tracks(int device, int n_sets, const int32_t* n_feat, int min_length, const int32_t* d_track_of,
+                         const int32_t* d_track_start, const int32_t* d_members, const ps_track_counts* counts, int64_t* N)
+{
+    if (n_sets < 0 || (n_sets > 0 && !n_feat) || min_length < 2 || !counts) return false;
+    *N = 0;
+    for (int i = 0; i < n_sets; ++i) {
+        if (n_feat[i] < 0) return false;
+        *N += n_feat[i];
+    }
+    if (*N >= 0x80000000LL) return false;
+    if (ps_pointer_device(d_track_start) != device) return false;
+    return *N == 0 || (ps_pointer_device(d_track_of) == device && ps_pointer_device(d_members) == device);
+}
+
+// the tail of both track entry points: an out-of-range endpoint is an argument error
+static int finish_tracks(const char* name, int launched, bool bad_edge, const char* err)
+{
+    if (launched >= 0 && bad_edge) { g_create_error = std::string(name) + ": an edge endpoint is out of range"; return PS_ERR_ARG; }
+    return finish(name, launched, err);
+}
+
+extern "C" int ps_tracks_from_edges(int device, int n_sets, const int32_t* n_feat, int n_edges, const int32_t* d_edges, int min_length,
+                                    int32_t* d_track_of, int32_t* d_track_start, int32_t* d_members, ps_track_counts* counts)
+{
+    if (n_edges < 0 || (n_edges > 0 && !d_edges)) return PS_ERR_ARG;
+    if (!set_device(device)) return PS_ERR_CUDA;
+    int64_t N = 0;
+    if (!check_tracks(device, n_sets, n_feat, min_length, d_track_of, d_track_start, d_members, counts, &N)) return PS_ERR_ARG;
+    if (n_edges > 0 && ps_pointer_device(d_edges) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    bool bad = false;
+    const int n = run_tracks_from_edges(n_sets, n_feat, n_edges, d_edges, min_length, d_track_of, d_track_start, d_members, counts,
+                                        &bad, nullptr, &err);
+    return finish_tracks("ps_tracks_from_edges", n, bad, err);
+}
+
+extern "C" int ps_tracks_from_matches(int device, int n_sets, const int32_t* n_feat, const int32_t* const* d_rev, const int32_t* n_desc,
+                                      int n_pairs, const int32_t* pairs, const int32_t* d_match, const int32_t* d_src, const int32_t* n_corr,
+                                      const uint8_t* d_inlier_mask, int min_length, int32_t* d_track_of, int32_t* d_track_start,
+                                      int32_t* d_members, ps_track_counts* counts)
+{
+    if (n_sets < 0 || n_pairs < 0 || (n_sets > 0 && (!d_rev || !n_desc)) || (n_pairs > 0 && (!pairs || !n_corr))) return PS_ERR_ARG;
+    if (!set_device(device)) return PS_ERR_CUDA;
+    int64_t N = 0, rows = 0;
+    if (!check_tracks(device, n_sets, n_feat, min_length, d_track_of, d_track_start, d_members, counts, &N) ||
+        !check_sets(device, n_sets, n_desc, d_rev, 0) || !check_pairs(n_sets, n_desc, pairs, n_pairs, &rows))
+        return PS_ERR_ARG;
+    if (rows > 0x7fffffff) return PS_ERR_ARG;
+    std::vector<int32_t> off(n_sets + 1, 0);
+    for (int i = 0; i < n_sets; ++i) off[i + 1] = off[i] + n_feat[i];
+    std::vector<TrackPair> tp(n_pairs);
+    int64_t row0 = 0, corr = 0;
+    for (int p = 0; p < n_pairs; ++p) {
+        const int l = pairs[2 * p], r = pairs[2 * p + 1];
+        if (n_corr[p] < 0 || n_corr[p] > n_desc[l]) return PS_ERR_ARG;
+        tp[p] = TrackPair{0, row0, d_rev[l], d_rev[r], off[l], off[r], n_desc[l], n_desc[r], n_feat[l], n_feat[r], n_corr[p], 0};
+        row0 += n_desc[l];
+        corr += n_corr[p];
+    }
+    if (corr > 0 && (ps_pointer_device(d_match) != device || ps_pointer_device(d_src) != device ||
+                     (d_inlier_mask && ps_pointer_device(d_inlier_mask) != device)))
+        return PS_ERR_ARG;
+    const char* err = nullptr;
+    bool bad = false;
+    const int n = run_tracks_from_matches(n_sets, n_feat, tp, d_match, d_src, d_inlier_mask, min_length, d_track_of, d_track_start,
+                                          d_members, counts, &bad, nullptr, &err);
+    return finish_tracks("ps_tracks_from_matches", n, bad, err);
 }
 
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)

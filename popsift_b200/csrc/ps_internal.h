@@ -1,10 +1,12 @@
 // Internal (device + host) structures shared by the kernels and the C-ABI layer.
 #pragma once
 #include "popsift_b200.h"
+#include "popsift_b200_tracks.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstdint>
+#include <vector>
 
 namespace psb {
 
@@ -247,5 +249,26 @@ int run_vlad_train(const ps_descriptor* const* sets, const int32_t* n_desc, int 
 int run_vlad_encode(const ps_descriptor* const* sets, const int32_t* n_desc, int n_sets, int k, const float* centroids,
                     float* vlad, int32_t* assign, int flags, cudaStream_t st, const char** err);
 int run_retrieve_pairs(int n, const float* vec, int dim, int m, int32_t* nbr, float* score, cudaStream_t st, const char** err);
+
+// feature tracks (include/popsift_b200_tracks.h, k_tracks.cu), arguments already validated except the edges' endpoints:
+// an endpoint outside its range sets *bad_edge, and the call returns before writing any output.  Synchronous on `st` (the
+// flag and the counts are read back); return the number of kernels launched or -1 (*err set).
+// One pair of ps_tracks_from_matches: first is filled in by the run.
+struct TrackPair {
+    long long first;                  // the pair's first correspondence in the concatenation of all pairs' correspondences
+    long long row0;                   // its first row of d_match / d_src / d_inlier_mask
+    const int32_t* rev_l;
+    const int32_t* rev_r;
+    int32_t off_l, off_r;             // global id of feature 0 of the left / right set
+    int32_t n_l, n_r;                 // descriptors
+    int32_t nf_l, nf_r;               // features
+    int32_t n_corr, pad_;
+};
+int run_tracks_from_edges(int n_sets, const int32_t* n_feat, int n_edges, const int32_t* edges, int min_length, int32_t* track_of,
+                          int32_t* track_start, int32_t* members, ps_track_counts* counts, bool* bad_edge, cudaStream_t st,
+                          const char** err);
+int run_tracks_from_matches(int n_sets, const int32_t* n_feat, const std::vector<TrackPair>& pairs, const int32_t* match,
+                            const int32_t* src, const uint8_t* mask, int min_length, int32_t* track_of, int32_t* track_start,
+                            int32_t* members, ps_track_counts* counts, bool* bad_edge, cudaStream_t st, const char** err);
 
 } // namespace psb

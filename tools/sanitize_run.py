@@ -123,3 +123,24 @@ if only in ("all", "retrieval"):
     for n, dim, m in ((300, 260, 7), (20, 36, 30), (1, 4, 1)):
         nbr, sc = api.retrieve(rng.normal(size=(n, dim)).astype(np.float32), m)
         print("retrieve", n, dim, m, int(nbr[0, 0]), flush=True)
+if only in ("all", "tracks"):
+    # feature tracks: the edge entry on a ragged graph (empty sets, self-loops, duplicates, forks) over more than one scan
+    # block and radix tile, then the chain entry on real match rows with a self pair, verified and guided
+    rng = np.random.default_rng(6)
+    n_feat = [0, 3000, 2500, 0, 4000, 1]
+    e = rng.integers(0, 9501, size=(6000, 2))
+    e[:50, 1] = e[:50, 0]
+    edges = np.c_[np.searchsorted(np.cumsum([0] + n_feat), e[:, 0], side="right") - 1, e[:, 0], np.zeros(len(e), int), e[:, 1]]
+    off = np.cumsum([0] + n_feat)
+    edges[:, 1] -= off[edges[:, 0]]
+    edges[:, 2] = np.searchsorted(off, e[:, 1], side="right") - 1
+    edges[:, 3] = e[:, 1] - off[edges[:, 2]]
+    t = api.build_tracks(n_feat, np.concatenate([edges, edges[:100]]), min_length=3)
+    print("tracks edges", len(t.start) - 1, t.n_conflicting, t.n_short, flush=True)
+    frames = [make_frame(320, 240, 18), make_frame(320, 240, 18)[:, ::-1].copy(), make_frame(320, 240, 19)]
+    ps = api.PopSift(api.Config(), mode=api.Config.MatchingMode, max_width=320, max_height=240, slots=1)
+    sets = [ps.enqueue(320, 240, im).getDev() for im in frames]
+    for guided in (False, True):
+        t = api.tracks(sets, [(0, 1), (1, 2), (0, 2), (2, 2)], guided=guided, n_samples=100)
+        print("tracks chain", "guided" if guided else "verified", len(t.start) - 1, t.n_conflicting, flush=True)
+    ps.uninit()
