@@ -158,6 +158,39 @@ struct PairGeometry
 std::vector<PairGeometry> verifyPairs(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
                                       const std::vector<std::vector<int>>& matches, const VerifyParams& params = VerifyParams());
 
+/// Pinhole intrinsics of one image in pixels (ps_camera in popsift_b200_pose.h); points must be undistorted.
+struct Camera
+{
+    float fx = 0.0f, fy = 0.0f, cx = 0.0f, cy = 0.0f;
+};
+
+/// RANSAC settings of relativePoses (same fields and rules as ps_pose_params in popsift_b200_pose.h).
+struct PoseParams
+{
+    int                n_samples = 1024;    // minimal samples per pair, 1 .. 65536 (fixed; no early exit)
+    float              threshold = 4.0f;    // pixels (Sampson distance, tested in calibrated coordinates)
+    bool               refine = true;       // one least-squares refit on the winner's inliers
+    unsigned long long seed = 0;
+};
+
+/// The calibrated two-view geometry of one pair (ps_two_view): E in calibrated coordinates, F in pixels (a model for
+/// matchPairsGuided with VerifyParams::Fundamental), R and unit t with X_r = R X_l + t, all row-major and zero when none
+/// was found.  inlier_rows / front_rows are the left descriptor indices of the inlier correspondences and of those also
+/// in front of both cameras, ascending.
+struct TwoViewPose
+{
+    float            E[9], F[9], R[9], t[3];
+    int              n_inliers, n_front;
+    std::vector<int> inlier_rows, front_rows;
+};
+
+/// Relative poses of matched calibrated pairs on the device (an addition to the reference's interface; C ABI
+/// ps_match_correspondences + ps_relative_pose_batch): `matches` is the output of matchPairs / matchPairsU8 on the same
+/// sets and pairs, `cameras` one per set.  Throws like verifyPairs, and when cameras.size() != sets.size().
+std::vector<TwoViewPose> relativePoses(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                       const std::vector<std::vector<int>>& matches, const std::vector<Camera>& cameras,
+                                       const PoseParams& params = PoseParams());
+
 /// Guided matching (an addition to the reference's interface; C ABI ps_match_guided_batch in popsift_b200_guided.h): matchPairs
 /// again with only the right descriptors whose keypoints pass the pair's model as candidates.  `geometry` is what
 /// verifyPairs gave for the same sets and pairs; params.model and params.threshold select the test (the other fields are

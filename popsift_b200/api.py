@@ -75,7 +75,23 @@ class PsTrackCounts(C.Structure):
                 ("n_short", C.c_int32)]
 
 
+class PsCamera(C.Structure):
+    """ps_camera (16 bytes): pinhole intrinsics in pixels"""
+    _fields_ = [("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float)]
+
+
+class PsPoseParams(C.Structure):
+    """ps_pose_params (24 bytes)"""
+    _fields_ = [("n_samples", C.c_int32), ("threshold", C.c_float), ("refine", C.c_int32), ("pad_", C.c_int32),
+                ("seed", C.c_uint64)]
+
+
+# ps_two_view (128 bytes): the per-pair output of ps_relative_pose_batch
+TWO_VIEW_DTYPE = np.dtype([("E", "<f4", (3, 3)), ("F", "<f4", (3, 3)), ("R", "<f4", (3, 3)), ("t", "<f4", 3),
+                           ("n_inliers", "<i4"), ("n_front", "<i4")])
+
 assert C.sizeof(PsVerifyParams) == 24 and C.sizeof(PsTrackCounts) == 20
+assert C.sizeof(PsCamera) == 16 and C.sizeof(PsPoseParams) == 24 and TWO_VIEW_DTYPE.itemsize == 128
 
 EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps_geometry", "ps_create", "ps_destroy",
            "ps_last_error", "ps_submit_u8", "ps_submit_f32", "ps_submit_dev_u8", "ps_counts", "ps_download",
@@ -90,6 +106,8 @@ GUIDED_EXPORTS = ["ps_match_guided_batch", "ps_match_u8_guided_batch"]
 RETRIEVAL_EXPORTS = ["ps_vlad_train", "ps_vlad_encode", "ps_retrieve_pairs"]
 # feature tracks, declared in popsift_b200_tracks.h (same library)
 TRACKS_EXPORTS = ["ps_tracks_from_edges", "ps_tracks_from_matches"]
+# calibrated two-view geometry, declared in popsift_b200_pose.h (same library)
+POSE_EXPORTS = ["ps_relative_pose_batch"]
 
 _lib = None
 
@@ -147,6 +165,9 @@ def load_library():
         L.ps_tracks_from_matches.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.POINTER(PsTrackCounts)]
+    if hasattr(L, "ps_relative_pose_batch"):
+        L.ps_relative_pose_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.POINTER(PsPoseParams), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsVerifyTaps)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -752,11 +773,10 @@ def verify_pairs(sets, pairs, matches=None, flags=0, u8=False, device=None, guid
 _Chain = namedtuple("_Chain", "device rows d_match d_src start n_corr d_mask models n_in mask")
 
 
-def _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, prm) -> _Chain:
-    """verify_pairs' device chain: match_pairs (match_pairs_u8) unless `matches` is given, ps_match_correspondences,
-    ps_verify_batch, and with guided=True guided matching and the correspondences again.  Device arrays in bufs: d_match,
-    the rows the final correspondences came from; d_src, start, n_corr, those correspondences; d_mask, the verification's
-    inlier mask, or None after guided matching (every guided correspondence passed the model).  Host: models, n_in, mask."""
+def _matched_rows(lib, bufs, sets, pairs, matches, flags, u8, device, u8_copies):
+    """The front of the device chains: match_pairs (match_pairs_u8) unless `matches` is given, then
+    ps_match_correspondences.  Returns (descs, device, rows, d_match, d_corr, d_src, start, n_corr): descs as _desc_sets
+    gave them (8-bit copies only with u8_copies), the device match rows and the correspondences."""
     counts = [s.getDescriptorCount() for s in sets]
     for l, r in pairs:
         if not (0 <= l < len(sets) and 0 <= r < len(sets)):
@@ -764,8 +784,7 @@ def _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, pr
     if matches is not None and len(matches) != len(pairs):
         raise PopSiftError("one match array per pair expected")
     rows = sum(counts[l] for l, _ in pairs)
-    # the 8-bit copies are made only when matching uses them
-    descs = _desc_sets(lib, bufs, sets, device, u8 and (matches is None or guided))
+    descs = _desc_sets(lib, bufs, sets, device, u8_copies)
     c_sets, c_n, _, device = descs
     if matches is not None:
         m = np.concatenate([np.asarray(r, np.int32).reshape(-1, 3) for r in matches]) if matches else np.zeros((0, 3), np.int32)
@@ -775,6 +794,17 @@ def _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, pr
         fn = lib.ps_match_u8_batch if u8 else lib.ps_match_batch
         _check(lib, fn(device, len(sets), c_sets, c_n, len(pairs), _c_pairs(pairs), d_match, flags), "matching")
     d_corr, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_match, device)
+    return descs, device, rows, d_match, d_corr, d_src, start, n_corr
+
+
+def _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, prm) -> _Chain:
+    """verify_pairs' device chain: _matched_rows, ps_verify_batch, and with guided=True guided matching and the
+    correspondences again.  Device arrays in bufs: d_match, the rows the final correspondences came from; d_src, start,
+    n_corr, those correspondences; d_mask, the verification's inlier mask, or None after guided matching (every guided
+    correspondence passed the model).  Host: models, n_in, mask."""
+    # the 8-bit copies are made only when matching uses them
+    descs, device, rows, d_match, d_corr, d_src, start, n_corr = _matched_rows(
+        lib, bufs, sets, pairs, matches, flags, u8, device, u8 and (matches is None or guided))
     d_models, d_mask = bufs.alloc(len(pairs) * 36), bufs.alloc(rows)
     models, n_in, mask = _verify_dev(lib, bufs, device, d_corr, start, n_corr, prm, d_models=d_models, d_mask=d_mask)
     if guided:
@@ -782,6 +812,110 @@ def _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, pr
         _, d_src, start, n_corr = _correspondences_dev(lib, bufs, sets, pairs, d_match, device)
         d_mask = mask = None
     return _Chain(device, rows, d_match, d_src, start, n_corr, d_mask, models, n_in, mask)
+
+
+TwoView = namedtuple("TwoView", "E F R t n_inliers n_front mask points")
+TwoView.__doc__ = """One pair's calibrated two-view geometry (ps_relative_pose_batch, popsift_b200_pose.h): E (3, 3) in calibrated
+coordinates, F (3, 3) in pixels, R (3, 3) and unit t with X_r = R X_l + t, the two counts, the (n,) uint8 mask (bit 0
+inlier, bit 1 also in front of both cameras) and the (n, 4) float32 points (X, Y, Z, 1) in the left frame with unit baseline,
+zero for rows without bit 1 (None unless asked for)."""
+
+
+def _pose_params(threshold=4.0, n_samples=1024, seed=0, refine=True) -> PsPoseParams:
+    return PsPoseParams(int(n_samples), float(threshold), 1 if refine else 0, 0, int(seed) & ((1 << 64) - 1))
+
+
+def _c_cameras(cams) -> np.ndarray:
+    """(fx, fy, cx, cy) rows as a contiguous float32 array of ps_camera"""
+    return np.ascontiguousarray(np.asarray(cams, np.float32).reshape(-1, 4))
+
+
+def _pose_dev(lib, bufs, device, d_corr, start, n_corr, cams, prm: PsPoseParams, points=False, taps=False):
+    """ps_relative_pose_batch: (d_out, d_mask, host two-view records, mask (rows,) uint8, points or None[, tap counts,
+    tap models])"""
+    P = len(start)
+    rows = int(max((int(a) + int(b) for a, b in zip(start, n_corr)), default=0))
+    d_out, d_mask = bufs.alloc(P * 128), bufs.alloc(rows)
+    d_pts = bufs.alloc(rows * 16) if points else None
+    tp = None
+    if taps:
+        nh = P * 10 * prm.n_samples
+        tp = PsVerifyTaps(bufs.alloc(nh * 4), bufs.alloc(nh * 36))
+    c_start = np.ascontiguousarray(start, np.int32)
+    c_n = np.ascontiguousarray(n_corr, np.int32)
+    rc = lib.ps_relative_pose_batch(device, P, d_corr, c_start.ctypes.data, c_n.ctypes.data, cams.ctypes.data, C.byref(prm), d_out,
+                                    d_mask, d_pts, C.byref(tp) if tp is not None else None)
+    _check(lib, rc, "ps_relative_pose_batch")
+    out = [d_out, d_mask, bufs.download(d_out, P, TWO_VIEW_DTYPE), bufs.download(d_mask, rows, np.uint8),
+           bufs.download(d_pts, (rows, 4), np.float32) if points else None]
+    if taps:
+        nh = 10 * prm.n_samples
+        out += [bufs.download(tp.d_counts, (P, nh), np.int32), bufs.download(tp.d_models, (P, nh, 3, 3), np.float32)]
+    return out
+
+
+def relative_pose_correspondences(corrs, cameras, threshold=4.0, n_samples=1024, seed=0, refine=True, points=False, taps=False,
+                                  device=0):
+    """Batched five-point RANSAC, relative pose and triangulation on host correspondences (C ABI ps_relative_pose_batch in
+    popsift_b200_pose.h; an addition to the reference's interface).  `corrs` is a list of (n, 4) arrays x_l, y_l, x_r, y_r
+    in undistorted pixels and `cameras` one (left, right) pair of (fx, fy, cx, cy) per array.  Returns a TwoView per pair;
+    with taps=True also (counts, models): every hypothesis's inlier count (P, 10 * n_samples; -1 invalid) and calibrated
+    E (P, 10 * n_samples, 3, 3)."""
+    lib = load_library()
+    prm = _pose_params(threshold, n_samples, seed, refine)
+    arrs = [np.ascontiguousarray(c, np.float32).reshape(-1, 4) for c in corrs]
+    cams = np.asarray(cameras, np.float32)
+    if cams.shape != (len(arrs), 2, 4):
+        raise PopSiftError("one (left, right) pair of (fx, fy, cx, cy) per correspondence array expected")
+    cams = _c_cameras(cams)
+    n_corr = np.array([len(a) for a in arrs], np.int32)
+    start = np.concatenate([[0], np.cumsum(n_corr)])[:len(arrs)].astype(np.int32)
+    bufs = _DevBuffers(lib)
+    try:
+        allc = np.concatenate(arrs) if arrs else np.zeros((0, 4), np.float32)
+        out = _pose_dev(lib, bufs, device, bufs.upload(allc), start, n_corr, cams, prm, points, taps)
+    finally:
+        bufs.free()
+    tv, mask, pts = out[2:5]
+    res = []
+    for p in range(len(arrs)):
+        a, n = int(start[p]), int(n_corr[p])
+        r = tv[p]
+        res.append(TwoView(r["E"].copy(), r["F"].copy(), r["R"].copy(), r["t"].copy(), int(r["n_inliers"]), int(r["n_front"]),
+                           mask[a:a + n].copy(), pts[a:a + n].copy() if points else None))
+    return (res, (out[5], out[6])) if taps else res
+
+
+def relative_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=None, points=False, **params):
+    """Calibrated two-view geometry of matched pairs without leaving the device: match_pairs (match_pairs_u8 with u8=True)
+    unless `matches` is given, ps_match_correspondences, then ps_relative_pose_batch.  `sets` are FeaturesDev objects,
+    `cameras` one (fx, fy, cx, cy) per set, params relative_pose_correspondences' (threshold, n_samples, seed, refine).
+    Returns per pair (TwoView, int32 left descriptor rows of the inliers (bit 0), int32 left descriptor rows of the rows
+    in front (bit 1))."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    prm = _pose_params(**params)
+    cam = np.asarray(cameras, np.float32).reshape(-1, 4)
+    if len(cam) != len(sets):
+        raise PopSiftError("one camera per set expected")
+    bufs = _DevBuffers(lib)
+    try:
+        _, device, rows, _, d_corr, d_src, start, n_corr = _matched_rows(lib, bufs, sets, pairs, matches, flags, u8, device,
+                                                                        u8 and matches is None)
+        cams = _c_cameras([cam[i] for lr in pairs for i in lr])
+        out = _pose_dev(lib, bufs, device, d_corr, start, n_corr, cams, prm, points)
+        src = bufs.download(d_src, rows, np.int32)
+    finally:
+        bufs.free()
+    tv, mask, pts = out[2:5]
+    res = []
+    for p in range(len(pairs)):
+        a, n = int(start[p]), int(n_corr[p])
+        r, m, sr = tv[p], mask[a:a + n], src[a:a + n]
+        two = TwoView(r["E"].copy(), r["F"].copy(), r["R"].copy(), r["t"].copy(), int(r["n_inliers"]), int(r["n_front"]), m.copy(),
+                      pts[a:a + n].copy() if points else None)
+        res.append((two, sr[(m & 1) != 0].copy(), sr[(m & 2) != 0].copy()))
+    return res
 
 
 Tracks = namedtuple("Tracks", "start set feature track_of n_components n_conflicting n_short")

@@ -5,6 +5,7 @@
 #include "pinned_pool.h"
 #include "popsift_b200.h"
 #include "popsift_b200_guided.h"
+#include "popsift_b200_pose.h"
 #include "popsift_b200_retrieval.h"
 #include "popsift_b200_tracks.h"
 
@@ -328,6 +329,62 @@ std::vector<PairGeometry> verifyPairs(const std::vector<FeaturesDev*>& sets, con
         out[p].n_inliers = h_counts[p];
         for (int k = 0; k < n_corr[p]; ++k)
             if (h_mask[b.start[p] + k]) out[p].inlier_rows.push_back(h_src[b.start[p] + k]);
+    }
+    return out;
+}
+
+std::vector<TwoViewPose> relativePoses(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                       const std::vector<std::vector<int>>& matches, const std::vector<Camera>& cameras,
+                                       const PoseParams& params)
+{
+    if (matches.size() != pairs.size()) throw std::runtime_error("popsift::relativePoses: one match list per pair expected");
+    if (cameras.size() != sets.size()) throw std::runtime_error("popsift::relativePoses: one camera per set expected");
+    const Batch b("relativePoses", sets, pairs);
+    std::vector<TwoViewPose> out(pairs.size());
+    for (TwoViewPose& g : out) {
+        std::fill(g.E, g.E + 9, 0.0f); std::fill(g.F, g.F + 9, 0.0f); std::fill(g.R, g.R + 9, 0.0f); std::fill(g.t, g.t + 3, 0.0f);
+        g.n_inliers = g.n_front = 0;
+    }
+    const size_t nr = std::max<size_t>(b.rows, 1), np = pairs.size();
+    DevBuf match(nr * 3 * sizeof(int32_t), b.who);
+    b.upload(matches, static_cast<int32_t*>(match.p));
+    if (pairs.empty()) return out;
+    DevBuf corr(nr * 4 * sizeof(float), b.who), src(nr * sizeof(int32_t), b.who), mask(nr, b.who), two(np * sizeof(ps_two_view), b.who);
+    std::vector<int32_t> start(b.start.begin(), b.start.end()), n_corr(np, 0);
+    check(ps_match_correspondences(b.dev, (int)sets.size(), b.feat.data(), b.rev.data(), b.n_desc.data(), (int)np, b.flat.data(),
+                                   static_cast<const int32_t*>(match.p), static_cast<float*>(corr.p), static_cast<int32_t*>(src.p), n_corr.data()),
+          b.who);
+    std::vector<ps_camera> cams(2 * np);
+    for (size_t p = 0; p < np; ++p)
+        for (int k = 0; k < 2; ++k) {
+            const Camera& c = cameras[k ? pairs[p].second : pairs[p].first];
+            cams[2 * p + k] = ps_camera{c.fx, c.fy, c.cx, c.cy};
+        }
+    ps_pose_params prm{};
+    prm.n_samples = params.n_samples;
+    prm.threshold = params.threshold;
+    prm.refine = params.refine ? 1 : 0;
+    prm.seed = params.seed;
+    check(ps_relative_pose_batch(b.dev, (int)np, static_cast<const float*>(corr.p), start.data(), n_corr.data(), cams.data(), &prm,
+                                 static_cast<ps_two_view*>(two.p), static_cast<uint8_t*>(mask.p), nullptr, nullptr),
+          b.who);
+    std::vector<ps_two_view> h_two(np);
+    std::vector<int32_t> h_src(b.rows);
+    std::vector<uint8_t> h_mask(b.rows);
+    check(ps_dev_to_host(h_two.data(), two.p, np * sizeof(ps_two_view)), b.who);
+    check(ps_dev_to_host(h_src.data(), src.p, b.rows * sizeof(int32_t)), b.who);
+    check(ps_dev_to_host(h_mask.data(), mask.p, b.rows), b.who);
+    for (size_t p = 0; p < np; ++p) {
+        const ps_two_view& v = h_two[p];
+        TwoViewPose& g = out[p];
+        std::copy(v.E, v.E + 9, g.E); std::copy(v.F, v.F + 9, g.F); std::copy(v.R, v.R + 9, g.R); std::copy(v.t, v.t + 3, g.t);
+        g.n_inliers = v.n_inliers;
+        g.n_front = v.n_front;
+        for (int k = 0; k < n_corr[p]; ++k) {
+            const uint8_t m = h_mask[b.start[p] + k];
+            if (m & 1) g.inlier_rows.push_back(h_src[b.start[p] + k]);
+            if (m & 2) g.front_rows.push_back(h_src[b.start[p] + k]);
+        }
     }
     return out;
 }

@@ -10,6 +10,7 @@
 #include "ps_internal.h"
 #include "popsift_b200_guided.h"
 #include "popsift_b200_retrieval.h"
+#include "popsift_b200_pose.h"
 #include "popsift_b200_tracks.h"
 
 #include <algorithm>
@@ -1195,6 +1196,37 @@ extern "C" int ps_verify_batch(int device, int n_pairs, const float* d_corr, con
     const char* err = nullptr;
     const int n = run_verify_batch(n_pairs, d_corr, corr_start, n_corr, *prm, d_models, d_n_inliers, d_inlier_mask, taps, nullptr, &err);
     return finish("ps_verify_batch", n, err);
+}
+
+extern "C" int ps_relative_pose_batch(int device, int n_pairs, const float* d_corr, const int32_t* corr_start, const int32_t* n_corr,
+                                      const ps_camera* cams, const ps_pose_params* prm, ps_two_view* d_out, uint8_t* d_inlier_mask,
+                                      float* d_points, const ps_verify_taps* taps)
+{
+    if (n_pairs < 0 || !prm) return PS_ERR_ARG;
+    if (prm->n_samples < 1 || prm->n_samples > 65536) return PS_ERR_ARG;
+    if (!std::isfinite(prm->threshold) || !(prm->threshold > 0.0f)) return PS_ERR_ARG;
+    if (prm->refine != 0 && prm->refine != 1) return PS_ERR_ARG;
+    if (n_pairs == 0) return PS_OK;
+    if (!corr_start || !n_corr || !cams) return PS_ERR_ARG;
+    int64_t rows = 0;
+    for (int p = 0; p < n_pairs; ++p) {
+        if (corr_start[p] < 0 || n_corr[p] < 0) return PS_ERR_ARG;
+        rows = std::max<int64_t>(rows, (int64_t)corr_start[p] + n_corr[p]);
+    }
+    for (int k = 0; k < 2 * n_pairs; ++k) {
+        const ps_camera& c = cams[k];
+        if (!std::isfinite(c.fx) || !(c.fx > 0.0f) || !std::isfinite(c.fy) || !(c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
+            return PS_ERR_ARG;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (ps_pointer_device(d_out) != device) return PS_ERR_ARG;
+    if (d_points && ps_pointer_device(d_points) != device) return PS_ERR_ARG;
+    if (rows > 0 && (ps_pointer_device(d_corr) != device || ps_pointer_device(d_inlier_mask) != device)) return PS_ERR_ARG;
+    if (rows > 0 && (reinterpret_cast<uintptr_t>(d_corr) & 15u)) return PS_ERR_ARG;
+    if (taps && (ps_pointer_device(taps->d_counts) != device || ps_pointer_device(taps->d_models) != device)) return PS_ERR_ARG;
+    const char* err = nullptr;
+    const int n = run_relative_pose_batch(n_pairs, d_corr, corr_start, n_corr, cams, *prm, d_out, d_inlier_mask, d_points, taps, nullptr, &err);
+    return finish("ps_relative_pose_batch", n, err);
 }
 
 // both guided entry points: the argument checks of ps_match_batch / ps_match_u8_batch and ps_match_correspondences, the

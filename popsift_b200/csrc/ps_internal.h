@@ -1,6 +1,7 @@
 // Internal (device + host) structures shared by the kernels and the C-ABI layer.
 #pragma once
 #include "popsift_b200.h"
+#include "popsift_b200_pose.h"
 #include "popsift_b200_tracks.h"
 
 #include <cuda_runtime.h>
@@ -229,6 +230,11 @@ int run_match_correspondences(const ps_feature* const* feat, const int32_t* cons
 // batched RANSAC (normalise, solve, score, select / refit, taps); asynchronous on `st`
 int run_verify_batch(int n_pairs, const float* corr, const int32_t* corr_start, const int32_t* n_corr, const ps_verify_params& prm,
                      float* d_models, int32_t* d_n, uint8_t* d_mask, const ps_verify_taps* taps, cudaStream_t st, const char** err);
+// calibrated two-view geometry (include/popsift_b200_pose.h, k_pose.cu), arguments already validated: calibrate, solve,
+// compact, score, select / pose, taps.  Synchronises `st` once, to plan the scoring on each pair's valid hypotheses.
+int run_relative_pose_batch(int n_pairs, const float* corr, const int32_t* corr_start, const int32_t* n_corr, const ps_camera* cams,
+                            const ps_pose_params& prm, ps_two_view* d_out, uint8_t* d_mask, float* d_points, const ps_verify_taps* taps,
+                            cudaStream_t st, const char** err);
 
 // guided matching (include/popsift_b200_guided.h), arguments already validated: run_match_batch / run_match_u8_batch with
 // right descriptor j of pair p eligible for left descriptor i only when their keypoints pass the test of k_guided.h under

@@ -144,3 +144,19 @@ if only in ("all", "tracks"):
         t = api.tracks(sets, [(0, 1), (1, 2), (0, 2), (2, 2)], guided=guided, n_samples=100)
         print("tracks chain", "guided" if guided else "verified", len(t.start) - 1, t.n_conflicting, flush=True)
     ps.uninit()
+if only in ("all", "pose"):
+    # calibrated two-view geometry: empty, tiny (< 5) and multi-tile pairs with taps and points, then the device chain on
+    # real match rows with a self pair
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import pose_oracle as po
+    rng = np.random.default_rng(7)
+    sc = [po.planted_pose(rng, n, 0.6) for n in (0, 3, 5, 40, 2500)]
+    res, taps = api.relative_pose_correspondences([s[0] for s in sc], [s[1] for s in sc], threshold=2.0, n_samples=150,
+                                                  points=True, taps=True)
+    print("pose", [r.n_inliers for r in res], int((taps[0] >= 0).sum()), flush=True)
+    frames = [make_frame(320, 240, 18), make_frame(320, 240, 18)[:, ::-1].copy()]
+    ps = api.PopSift(api.Config(), mode=api.Config.MatchingMode, max_width=320, max_height=240, slots=1)
+    sets = [ps.enqueue(320, 240, im).getDev() for im in frames]
+    out = api.relative_poses(sets, [(0, 1), (1, 1)], [(300, 300, 160, 120)] * 2, n_samples=100, points=True)
+    print("pose chain", [o[0].n_inliers for o in out], flush=True)
+    ps.uninit()
