@@ -3,6 +3,7 @@
 // Feature = 72 bytes with host pointers into the owning FeaturesHost's descriptor array.
 #pragma once
 
+#include <cstdint>
 #include <iostream>
 #include <utility>
 #include <vector>
@@ -240,5 +241,47 @@ Tracks buildTracks(const std::vector<FeaturesDev*>& sets, const std::vector<std:
 /// Tracks of every correspondence of `matches`: the rows of matchPairsGuided(U8), which already passed the model.
 Tracks buildTracks(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
                    const std::vector<std::vector<int>>& matches, int min_length = 2);
+
+/// A camera pose, world to camera: X_cam = R X_world + t, R row-major (ps_rigid in popsift_b200_triangulate.h).
+struct Rigid
+{
+    double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    double t[3] = {0, 0, 0};
+};
+
+/// Settings of triangulateTracks (same fields and rules as ps_triangulate_params).
+struct TriangulateParams
+{
+    float              max_error = 4.0f;     // pixels
+    float              min_angle = 1.5f;     // degrees, [0, 90)
+    int                min_views = 2;        // >= 2
+    int                n_samples = 256;      // hypotheses per track when not every pair is tried, 1 .. 65536
+    int                refine_iters = 10;    // Gauss-Newton steps, 0 .. 32
+    unsigned long long seed = 0;
+};
+
+/// One point per track (ps_track_point) and one entry per member of Tracks::set / Tracks::feature: the inlier mask and
+/// the pixel reprojection error (+inf behind the camera or without a point).  n_status[s] counts the tracks of status s
+/// (PS_TRI_OK .. PS_TRI_SMALL_ANGLE).
+struct TrackPoint
+{
+    double X[3];
+    float  error, angle;
+    int    n_inliers, status;
+};
+struct TrackPoints
+{
+    std::vector<TrackPoint>   points;
+    std::vector<std::uint8_t> mask;
+    std::vector<float>        obs_error;
+    int                       n_status[5] = {0, 0, 0, 0, 0};
+    int                       n_inlier_obs = 0;
+};
+
+/// Multi-view triangulation of `tracks` (what buildTracks gave for `sets`) from known poses on the device (an addition to
+/// the reference's interface; C ABI ps_triangulate_tracks): `cameras` and `poses` one per set.  Throws like
+/// relativePoses, and when poses.size() != sets.size().
+TrackPoints triangulateTracks(const std::vector<FeaturesDev*>& sets, const Tracks& tracks, const std::vector<Camera>& cameras,
+                              const std::vector<Rigid>& poses, const TriangulateParams& params = TriangulateParams());
 
 } // namespace popsift

@@ -93,6 +93,29 @@ TWO_VIEW_DTYPE = np.dtype([("E", "<f4", (3, 3)), ("F", "<f4", (3, 3)), ("R", "<f
 assert C.sizeof(PsVerifyParams) == 24 and C.sizeof(PsTrackCounts) == 20
 assert C.sizeof(PsCamera) == 16 and C.sizeof(PsPoseParams) == 24 and TWO_VIEW_DTYPE.itemsize == 128
 
+
+class PsRigid(C.Structure):
+    """ps_rigid (96 bytes): X_cam = R X_world + t, R row-major"""
+    _fields_ = [("R", C.c_double * 9), ("t", C.c_double * 3)]
+
+
+class PsTriangulateParams(C.Structure):
+    """ps_triangulate_params (32 bytes)"""
+    _fields_ = [("max_error", C.c_float), ("min_angle", C.c_float), ("min_views", C.c_int32), ("n_samples", C.c_int32),
+                ("refine_iters", C.c_int32), ("pad_", C.c_int32), ("seed", C.c_uint64)]
+
+
+class PsTriangulateCounts(C.Structure):
+    """ps_triangulate_counts (24 bytes)"""
+    _fields_ = [("n_status", C.c_int32 * 5), ("n_inlier_obs", C.c_int32)]
+
+
+# ps_track_point (40 bytes): the per-track output of ps_triangulate_tracks; status codes PS_TRI_*
+TRACK_POINT_DTYPE = np.dtype([("X", "<f8", 3), ("error", "<f4"), ("angle", "<f4"), ("n_inliers", "<i4"), ("status", "<i4")])
+TRI_STATUS = ("ok", "too_few_obs", "no_hypothesis", "too_few_inliers", "small_angle")
+assert C.sizeof(PsRigid) == 96 and C.sizeof(PsTriangulateParams) == 32 and C.sizeof(PsTriangulateCounts) == 24
+assert TRACK_POINT_DTYPE.itemsize == 40
+
 EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps_geometry", "ps_create", "ps_destroy",
            "ps_last_error", "ps_submit_u8", "ps_submit_f32", "ps_submit_dev_u8", "ps_counts", "ps_download",
            "ps_sync", "ps_debug_plane", "ps_debug_extrema", "ps_slot_geometry", "ps_set_timing", "ps_stage_ms",
@@ -108,6 +131,8 @@ RETRIEVAL_EXPORTS = ["ps_vlad_train", "ps_vlad_encode", "ps_retrieve_pairs"]
 TRACKS_EXPORTS = ["ps_tracks_from_edges", "ps_tracks_from_matches"]
 # calibrated two-view geometry, declared in popsift_b200_pose.h (same library)
 POSE_EXPORTS = ["ps_relative_pose_batch"]
+# multi-view triangulation, declared in popsift_b200_triangulate.h (same library)
+TRIANGULATE_EXPORTS = ["ps_triangulate_tracks"]
 
 _lib = None
 
@@ -168,6 +193,10 @@ def load_library():
     if hasattr(L, "ps_relative_pose_batch"):
         L.ps_relative_pose_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.POINTER(PsPoseParams), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsVerifyTaps)]
+    if hasattr(L, "ps_triangulate_tracks"):
+        L.ps_triangulate_tracks.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                            C.c_void_p, C.c_int, C.POINTER(PsTriangulateParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.POINTER(PsTriangulateCounts)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -925,6 +954,11 @@ Tracks.__doc__ = """Feature tracks: track t's members are set[start[t]:start[t +
 
 def _tracks_dev(lib, bufs, n_feat, min_length, call) -> Tracks:
     """the outputs of a track entry point: `call(d_track_of, d_track_start, d_members, counts)` returns its code"""
+    return _tracks_run(lib, bufs, n_feat, min_length, call)[0]
+
+
+def _tracks_run(lib, bufs, n_feat, min_length, call):
+    """_tracks_dev's Tracks with the device arrays d_track_start and d_members they were read from (they stay in bufs)"""
     n_feat = [int(n) for n in n_feat]
     off = np.concatenate([[0], np.cumsum(n_feat, dtype=np.int64)]).astype(np.int64)
     N = int(off[-1])
@@ -937,7 +971,7 @@ def _tracks_dev(lib, bufs, n_feat, min_length, call) -> Tracks:
     of = bufs.download(d_of, N, np.int32)
     s = (np.searchsorted(off, mem, side="right") - 1).astype(np.int32)
     return Tracks(start, s, (mem - off[s]).astype(np.int32), [of[off[i]:off[i + 1]] for i in range(len(n_feat))],
-                  cnt.n_components, cnt.n_conflicting, cnt.n_short)
+                  cnt.n_components, cnt.n_conflicting, cnt.n_short), d_start, d_mem
 
 
 def build_tracks(n_feat, edges, min_length=2, device=0) -> Tracks:
@@ -974,18 +1008,120 @@ def tracks(sets, pairs, matches=None, min_length=2, guided=False, u8=False, flag
     prm = _verify_params(**verify_params)
     bufs = _DevBuffers(lib)
     try:
-        ch = _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, prm)
-        n = max(len(sets), 1)
-        n_feat = [s.getFeatureCount() for s in sets]
-        c_nf = (C.c_int32 * n)(*n_feat)
-        c_rev = (C.c_void_p * n)(*[s.getReverseMap() for s in sets])
-        c_nd = (C.c_int32 * n)(*[s.getDescriptorCount() for s in sets])
-        c_corr = np.ascontiguousarray(ch.n_corr, np.int32)
-        return _tracks_dev(lib, bufs, n_feat, min_length, lambda of, st, mem, cnt: lib.ps_tracks_from_matches(
-            ch.device, len(sets), c_nf, c_rev, c_nd, len(pairs), _c_pairs(pairs), ch.d_match, ch.d_src, c_corr.ctypes.data,
-            ch.d_mask, int(min_length), of, st, mem, C.byref(cnt)))
+        return _tracks_chain(lib, bufs, sets, pairs, matches, min_length, guided, u8, flags, device, prm)[0]
     finally:
         bufs.free()
+
+
+def _tracks_chain(lib, bufs, sets, pairs, matches, min_length, guided, u8, flags, device, prm):
+    """tracks()' device chain: _verify_chain, then ps_tracks_from_matches on its arrays.  Returns (Tracks, device,
+    d_track_start, d_members), the device arrays in bufs"""
+    ch = _verify_chain(lib, bufs, sets, pairs, matches, flags, u8, device, guided, prm)
+    n = max(len(sets), 1)
+    n_feat = [s.getFeatureCount() for s in sets]
+    c_nf = (C.c_int32 * n)(*n_feat)
+    c_rev = (C.c_void_p * n)(*[s.getReverseMap() for s in sets])
+    c_nd = (C.c_int32 * n)(*[s.getDescriptorCount() for s in sets])
+    c_corr = np.ascontiguousarray(ch.n_corr, np.int32)
+    tr, d_start, d_mem = _tracks_run(lib, bufs, n_feat, min_length, lambda of, st, mem, cnt: lib.ps_tracks_from_matches(
+        ch.device, len(sets), c_nf, c_rev, c_nd, len(pairs), _c_pairs(pairs), ch.d_match, ch.d_src, c_corr.ctypes.data,
+        ch.d_mask, int(min_length), of, st, mem, C.byref(cnt)))
+    return tr, ch.device, d_start, d_mem
+
+
+TrackPoints = namedtuple("TrackPoints", "X error angle n_inliers status mask obs_error counts")
+TrackPoints.__doc__ = """Multi-view triangulation of tracks (ps_triangulate_tracks, popsift_b200_triangulate.h): per track X (T, 3)
+float64 in world coordinates, the mean pixel reprojection error over the inliers, the triangulation angle in degrees, the
+inlier count and the status (an index into TRI_STATUS, 0 = ok); per member (aligned with Tracks.set / Tracks.feature) the
+uint8 inlier mask and the float32 pixel error (+inf behind the camera or without a point); counts: tracks per status name
+and 'inlier_obs'."""
+
+
+def _tri_params(max_error=4.0, min_angle=1.5, min_views=2, n_samples=256, refine_iters=10, seed=0) -> PsTriangulateParams:
+    return PsTriangulateParams(float(max_error), float(min_angle), int(min_views), int(n_samples), int(refine_iters), 0,
+                               int(seed) & ((1 << 64) - 1))
+
+
+def _c_rigids(poses):
+    """ps_rigid array of poses given as (R (3, 3), t (3,)) or as [R | t] (3, 4), world to camera"""
+    out = (PsRigid * max(len(poses), 1))()
+    for i, p in enumerate(poses):
+        if isinstance(p, (tuple, list)) and len(p) == 2:
+            R, t = np.asarray(p[0], np.float64).reshape(3, 3), np.asarray(p[1], np.float64).reshape(3)
+        else:
+            m = np.asarray(p, np.float64).reshape(3, 4)
+            R, t = m[:, :3], m[:, 3]
+        out[i].R[:] = [float(v) for v in R.ravel()]
+        out[i].t[:] = [float(v) for v in t]
+    return out
+
+
+def _triangulate_dev(lib, bufs, device, n_feat, c_feat, cameras, poses, n_tracks, d_start, d_mem, n_members, prm) -> TrackPoints:
+    """ps_triangulate_tracks on device track arrays; Feature records at c_feat (a C array of device pointers)"""
+    cam = _c_cameras(cameras)
+    if len(cam) != len(n_feat) or len(poses) != len(n_feat):
+        raise PopSiftError("one camera and one pose per set expected")
+    n = max(len(n_feat), 1)
+    d_pts, d_mask, d_err = bufs.alloc(n_tracks * 40), bufs.alloc(n_members), bufs.alloc(n_members * 4)
+    cnt = PsTriangulateCounts()
+    rc = lib.ps_triangulate_tracks(device, len(n_feat), (C.c_int32 * n)(*n_feat), c_feat, cam.ctypes.data, _c_rigids(poses), n_tracks,
+                                   d_start, d_mem, n_members, C.byref(prm), d_pts, d_mask, d_err, C.byref(cnt))
+    _check(lib, rc, "ps_triangulate_tracks")
+    pts = bufs.download(d_pts, n_tracks, TRACK_POINT_DTYPE)
+    counts = dict(zip(TRI_STATUS, [int(v) for v in cnt.n_status]))
+    counts["inlier_obs"] = int(cnt.n_inlier_obs)
+    return TrackPoints(pts["X"].copy(), pts["error"].copy(), pts["angle"].copy(), pts["n_inliers"].copy(), pts["status"].copy(),
+                       bufs.download(d_mask, n_members, np.uint8), bufs.download(d_err, n_members, np.float32), counts)
+
+
+def triangulate(sets, tracks, cameras, poses, device=None, **params) -> TrackPoints:
+    """Multi-view triangulation of feature tracks from known poses (C ABI ps_triangulate_tracks in
+    popsift_b200_triangulate.h; an addition to the reference's interface): a RANSAC over pairs of each track's
+    observations, then a Gauss-Newton refinement, for every track in one call.  `sets` are FeaturesDev objects or host
+    Features (their records are uploaded), `tracks` a Tracks over them (tracks() / build_tracks()), `cameras` one (fx, fy,
+    cx, cy) per set and `poses` one world-to-camera pose per set, (R, t) or [R | t].  params: max_error (px, 4.0),
+    min_angle (degrees, 1.5), min_views (2), n_samples (256), refine_iters (10), seed (0)."""
+    lib = load_library()
+    prm = _tri_params(**params)
+    bufs = _DevBuffers(lib)
+    try:
+        ptrs, n_feat = [], []
+        for s in sets:
+            if isinstance(s, FeaturesDev):
+                ptrs.append(s.getFeatures()); n_feat.append(s.getFeatureCount())
+            else:
+                f = np.ascontiguousarray(s.feat if isinstance(s, Features) else s, FEATURE_DTYPE)
+                ptrs.append(bufs.upload(f)); n_feat.append(len(f))
+        if device is None:
+            device = next((max(0, lib.ps_pointer_device(p)) for p, k in zip(ptrs, n_feat) if k > 0), 0)
+        off = np.concatenate([[0], np.cumsum(n_feat, dtype=np.int64)])
+        st = np.ascontiguousarray(tracks.start, np.int32)
+        mem = (off[np.asarray(tracks.set, np.int64)] + np.asarray(tracks.feature, np.int64)).astype(np.int32)
+        c_feat = (C.c_void_p * max(len(sets), 1))(*ptrs)
+        return _triangulate_dev(lib, bufs, device, n_feat, c_feat, cameras, poses, len(st) - 1, bufs.upload(st), bufs.upload(mem),
+                                len(mem), prm)
+    finally:
+        bufs.free()
+
+
+def triangulated_tracks(sets, pairs, cameras, poses, matches=None, min_length=2, guided=False, u8=False, flags=0, device=None,
+                        verify=None, **params):
+    """tracks() and triangulate() in one device chain: verify_pairs' chain on FeaturesDev `sets` and `pairs` with the
+    verify_pairs parameters in the dict `verify`, ps_tracks_from_matches, then ps_triangulate_tracks on the same device
+    arrays.  cameras, poses and params are triangulate()'s.  Returns (Tracks, TrackPoints)."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    vprm = _verify_params(**(verify or {}))
+    prm = _tri_params(**params)
+    bufs = _DevBuffers(lib)
+    try:
+        tr, device, d_start, d_mem = _tracks_chain(lib, bufs, sets, pairs, matches, min_length, guided, u8, flags, device, vprm)
+        c_feat = (C.c_void_p * max(len(sets), 1))(*[s.getFeatures() for s in sets])
+        pts = _triangulate_dev(lib, bufs, device, [s.getFeatureCount() for s in sets], c_feat, cameras, poses, len(tr.start) - 1,
+                               d_start, d_mem, len(tr.set), prm)
+    finally:
+        bufs.free()
+    return tr, pts
 
 
 def _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, model, threshold, flags, u8) -> int:

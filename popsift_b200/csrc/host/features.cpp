@@ -8,6 +8,7 @@
 #include "popsift_b200_pose.h"
 #include "popsift_b200_retrieval.h"
 #include "popsift_b200_tracks.h"
+#include "popsift_b200_triangulate.h"
 
 #include <algorithm>
 #include <cmath>
@@ -550,6 +551,71 @@ Tracks buildTracks(const std::vector<FeaturesDev*>& sets, const std::vector<std:
                    const std::vector<std::vector<int>>& matches, int min_length)
 {
     return build_tracks(sets, pairs, matches, nullptr, min_length);
+}
+
+TrackPoints triangulateTracks(const std::vector<FeaturesDev*>& sets, const Tracks& tracks, const std::vector<Camera>& cameras,
+                              const std::vector<Rigid>& poses, const TriangulateParams& params)
+{
+    const Batch b("triangulateTracks", sets, {});
+    if (cameras.size() != sets.size()) throw std::runtime_error(b.who + ": one camera per set expected");
+    if (poses.size() != sets.size()) throw std::runtime_error(b.who + ": one pose per set expected");
+    if (tracks.start.empty() || tracks.set.size() != tracks.feature.size() || (size_t)tracks.start.back() != tracks.set.size())
+        throw std::runtime_error(b.who + ": malformed tracks");
+    std::vector<int32_t> n_feat(sets.size());
+    std::vector<int64_t> off(sets.size() + 1, 0);
+    for (size_t i = 0; i < sets.size(); ++i) {
+        n_feat[i] = sets[i]->getFeatureCount();
+        off[i + 1] = off[i] + std::max(n_feat[i], 0);
+    }
+    const size_t nt = tracks.start.size() - 1, nm = tracks.set.size();
+    std::vector<int32_t> mem(nm);
+    for (size_t k = 0; k < nm; ++k) {
+        const int s = tracks.set[k], f = tracks.feature[k];
+        if (s < 0 || (size_t)s >= sets.size() || f < 0 || f >= n_feat[s]) throw std::runtime_error(b.who + ": track member out of range");
+        mem[k] = (int32_t)(off[s] + f);
+    }
+    std::vector<ps_camera> cams(sets.size());
+    std::vector<ps_rigid> rig(sets.size());
+    for (size_t i = 0; i < sets.size(); ++i) {
+        cams[i] = ps_camera{cameras[i].fx, cameras[i].fy, cameras[i].cx, cameras[i].cy};
+        std::copy(poses[i].R, poses[i].R + 9, rig[i].R);
+        std::copy(poses[i].t, poses[i].t + 3, rig[i].t);
+    }
+    ps_triangulate_params prm{};
+    prm.max_error = params.max_error;
+    prm.min_angle = params.min_angle;
+    prm.min_views = params.min_views;
+    prm.n_samples = params.n_samples;
+    prm.refine_iters = params.refine_iters;
+    prm.seed = params.seed;
+    DevBuf start(tracks.start.size() * sizeof(int32_t), b.who), members(nm * sizeof(int32_t), b.who);
+    DevBuf pts(std::max<size_t>(nt, 1) * sizeof(ps_track_point), b.who), mask(nm, b.who), err(nm * sizeof(float), b.who);
+    check(ps_host_to_dev(start.p, tracks.start.data(), tracks.start.size() * sizeof(int32_t)), b.who);
+    check(ps_host_to_dev(members.p, mem.data(), nm * sizeof(int32_t)), b.who);
+    ps_triangulate_counts c;
+    check(ps_triangulate_tracks(b.dev, (int)sets.size(), n_feat.data(), b.feat.data(), cams.data(), rig.data(), (int)nt,
+                                static_cast<const int32_t*>(start.p), static_cast<const int32_t*>(members.p), (int)nm, &prm,
+                                static_cast<ps_track_point*>(pts.p), static_cast<uint8_t*>(mask.p), static_cast<float*>(err.p), &c),
+          b.who, "ps_triangulate_tracks");
+    TrackPoints out;
+    std::vector<ps_track_point> h(nt);
+    out.mask.resize(nm);
+    out.obs_error.resize(nm);
+    check(ps_dev_to_host(h.data(), pts.p, nt * sizeof(ps_track_point)), b.who);
+    check(ps_dev_to_host(out.mask.data(), mask.p, nm), b.who);
+    check(ps_dev_to_host(out.obs_error.data(), err.p, nm * sizeof(float)), b.who);
+    out.points.resize(nt);
+    for (size_t t = 0; t < nt; ++t) {
+        TrackPoint& p = out.points[t];
+        std::copy(h[t].X, h[t].X + 3, p.X);
+        p.error = h[t].error;
+        p.angle = h[t].angle;
+        p.n_inliers = h[t].n_inliers;
+        p.status = h[t].status;
+    }
+    std::copy(c.n_status, c.n_status + 5, out.n_status);
+    out.n_inlier_obs = c.n_inlier_obs;
+    return out;
 }
 
 } // namespace popsift

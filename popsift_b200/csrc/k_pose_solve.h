@@ -468,18 +468,30 @@ PSV_HD void pose_candidates(const double (&U)[3][3], const double (&V)[3][3], do
     }
 }
 
-// Triangulation of one calibrated row under (R, t), X_r = R X_l + t: a = R (x_l, y_l, 1), b = (x_r, y_r, 1), the
-// minimiser of |d_l a + t - d_r b|^2 by the 2 x 2 normal equations (Cramer).  In front when det > 1e-12 (a.a)(b.b),
-// d_l > 0 and d_r > 0.  *X (optional) = the midpoint (d_l x_l + R^T (d_r b - t)) / 2 in the left frame.
-PSV_HD bool pose_front(const double* R, const double* t, double xl, double yl, double xr, double yr, double* X = nullptr)
+// The two-ray rule of triangulation: (d_l, d_r) minimising |d_l a + t - d_r b|^2 by the 2 x 2 normal equations (Cramer),
+// for rays d_l a from t and d_r b from the origin.  True when det = (a.a)(b.b) - (a.b)^2 > 1e-12 (a.a)(b.b), d_l > 0 and
+// d_r > 0.  Shared by ps_relative_pose_batch (pose_front) and ps_triangulate_tracks (k_triangulate.cu).
+PSV_HD bool pose_two_rays(const double* a, const double* b, const double* t, double& dl, double& dr)
 {
-    const double a0 = R[0] * xl + R[1] * yl + R[2], a1 = R[3] * xl + R[4] * yl + R[5], a2 = R[6] * xl + R[7] * yl + R[8];
-    const double aa = a0 * a0 + a1 * a1 + a2 * a2, bb = xr * xr + yr * yr + 1.0, ab = a0 * xr + a1 * yr + a2;
-    const double at = a0 * t[0] + a1 * t[1] + a2 * t[2], bt = xr * t[0] + yr * t[1] + t[2];
+    const double aa = a[0] * a[0] + a[1] * a[1] + a[2] * a[2], bb = b[0] * b[0] + b[1] * b[1] + b[2] * b[2];
+    const double ab = a[0] * b[0] + a[1] * b[1] + a[2] * b[2];
+    const double at = a[0] * t[0] + a[1] * t[1] + a[2] * t[2], bt = b[0] * t[0] + b[1] * t[1] + b[2] * t[2];
     const double det = aa * bb - ab * ab;
     if (!(det > 1e-12 * (aa * bb))) return false;
-    const double dl = (ab * bt - at * bb) / det, dr = (aa * bt - ab * at) / det;
-    if (!(dl > 0.0 && dr > 0.0)) return false;
+    dl = (ab * bt - at * bb) / det;
+    dr = (aa * bt - ab * at) / det;
+    return dl > 0.0 && dr > 0.0;
+}
+
+// Triangulation of one calibrated row under (R, t), X_r = R X_l + t: pose_two_rays with a = R (x_l, y_l, 1), b = (x_r,
+// y_r, 1) (b's unit third entry enters every product exactly).  In front when it holds.  *X (optional) = the midpoint
+// (d_l x_l + R^T (d_r b - t)) / 2 in the left frame.
+PSV_HD bool pose_front(const double* R, const double* t, double xl, double yl, double xr, double yr, double* X = nullptr)
+{
+    const double a[3] = {R[0] * xl + R[1] * yl + R[2], R[3] * xl + R[4] * yl + R[5], R[6] * xl + R[7] * yl + R[8]};
+    const double b[3] = {xr, yr, 1.0};
+    double dl, dr;
+    if (!pose_two_rays(a, b, t, dl, dr)) return false;
     if (X) {
         const double c0 = dr * xr - t[0], c1 = dr * yr - t[1], c2 = dr - t[2];
         X[0] = 0.5 * (dl * xl + R[0] * c0 + R[3] * c1 + R[6] * c2);

@@ -12,6 +12,7 @@
 #include "popsift_b200_retrieval.h"
 #include "popsift_b200_pose.h"
 #include "popsift_b200_tracks.h"
+#include "popsift_b200_triangulate.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1382,6 +1383,58 @@ extern "C" int ps_tracks_from_matches(int device, int n_sets, const int32_t* n_f
     const int n = run_tracks_from_matches(n_sets, n_feat, tp, d_match, d_src, d_inlier_mask, min_length, d_track_of, d_track_start,
                                           d_members, counts, &bad, nullptr, &err);
     return finish_tracks("ps_tracks_from_matches", n, bad, err);
+}
+
+// a pose ps_triangulate_tracks takes: finite entries, max |R^T R - I| <= 1e-6 and det R > 0
+static bool rigid_ok(const ps_rigid& p)
+{
+    for (double v : p.R) if (!std::isfinite(v)) return false;
+    for (double v : p.t) if (!std::isfinite(v)) return false;
+    const double* R = p.R;
+    for (int a = 0; a < 3; ++a)
+        for (int b = 0; b < 3; ++b) {
+            const double d = R[a] * R[b] + R[3 + a] * R[3 + b] + R[6 + a] * R[6 + b] - (a == b ? 1.0 : 0.0);
+            if (!(std::fabs(d) <= 1e-6)) return false;
+        }
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) + R[2] * (R[3] * R[7] - R[4] * R[6]);
+    return det > 0.0;
+}
+
+extern "C" int ps_triangulate_tracks(int device, int n_sets, const int32_t* n_feat, const ps_feature* const* d_feat, const ps_camera* cams,
+                                     const ps_rigid* poses, int n_tracks, const int32_t* d_track_start, const int32_t* d_members, int n_members,
+                                     const ps_triangulate_params* prm, ps_track_point* d_points, uint8_t* d_obs_mask, float* d_obs_error,
+                                     ps_triangulate_counts* counts)
+{
+    if (n_sets < 0 || n_tracks < 0 || n_members < 0 || !prm || !counts) return PS_ERR_ARG;
+    if (!std::isfinite(prm->max_error) || !(prm->max_error > 0.0f)) return PS_ERR_ARG;
+    if (!(prm->min_angle >= 0.0f && prm->min_angle < 90.0f)) return PS_ERR_ARG;
+    if (prm->min_views < 2 || prm->n_samples < 1 || prm->n_samples > 65536 || prm->refine_iters < 0 || prm->refine_iters > 32) return PS_ERR_ARG;
+    if (n_sets > 0 && (!n_feat || !d_feat || !cams || !poses)) return PS_ERR_ARG;
+    for (int i = 0; i < n_sets; ++i) {
+        const ps_camera& c = cams[i];
+        if (!std::isfinite(c.fx) || !(c.fx > 0.0f) || !std::isfinite(c.fy) || !(c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
+            return PS_ERR_ARG;
+        if (!rigid_ok(poses[i])) return PS_ERR_ARG;
+    }
+    if (n_tracks == 0) {
+        std::memset(counts, 0, sizeof(*counts));
+        return PS_OK;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    int64_t N = 0;
+    if (!check_sets(device, n_sets, n_feat, d_feat, 0, &N) || N >= 0x80000000LL) return PS_ERR_ARG;
+    if (ps_pointer_device(d_track_start) != device || ps_pointer_device(d_points) != device) return PS_ERR_ARG;
+    if (n_members > 0 && (ps_pointer_device(d_members) != device || ps_pointer_device(d_obs_mask) != device)) return PS_ERR_ARG;
+    if (d_obs_error && ps_pointer_device(d_obs_error) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    bool bad = false;
+    const int n = run_triangulate_tracks(n_sets, n_feat, d_feat, cams, poses, n_tracks, d_track_start, d_members, n_members, *prm, d_points,
+                                         d_obs_mask, d_obs_error, counts, &bad, nullptr, &err);
+    if (n >= 0 && bad) {
+        g_create_error = "ps_triangulate_tracks: a member id or d_track_start is out of range";
+        return PS_ERR_ARG;
+    }
+    return finish("ps_triangulate_tracks", n, err);
 }
 
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)

@@ -3,6 +3,7 @@
 #include "popsift_b200.h"
 #include "popsift_b200_pose.h"
 #include "popsift_b200_tracks.h"
+#include "popsift_b200_triangulate.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
@@ -276,5 +277,13 @@ int run_tracks_from_edges(int n_sets, const int32_t* n_feat, int n_edges, const 
 int run_tracks_from_matches(int n_sets, const int32_t* n_feat, const std::vector<TrackPair>& pairs, const int32_t* match,
                             const int32_t* src, const uint8_t* mask, int min_length, int32_t* track_of, int32_t* track_start,
                             int32_t* members, ps_track_counts* counts, bool* bad_edge, cudaStream_t st, const char** err);
+
+// multi-view triangulation (include/popsift_b200_triangulate.h, k_triangulate.cu), arguments already validated except the
+// member ids and d_track_start, which the ray pass checks: a bad one sets *bad, and the call returns before writing any
+// output.  Synchronous on `st` (the flag and the counts are read back); returns the number of kernels launched or -1.
+int run_triangulate_tracks(int n_sets, const int32_t* n_feat, const ps_feature* const* feat, const ps_camera* cams, const ps_rigid* poses,
+                           int n_tracks, const int32_t* track_start, const int32_t* members, int n_members,
+                           const ps_triangulate_params& prm, ps_track_point* points, uint8_t* obs_mask, float* obs_error,
+                           ps_triangulate_counts* counts, bool* bad, cudaStream_t st, const char** err);
 
 } // namespace psb

@@ -160,3 +160,27 @@ if only in ("all", "pose"):
     out = api.relative_poses(sets, [(0, 1), (1, 1)], [(300, 300, 160, 120)] * 2, n_samples=100, points=True)
     print("pose chain", [o[0].n_inliers for o in out], flush=True)
     ps.uninit()
+if only in ("all", "triangulate"):
+    # multi-view triangulation: tracks of length 1 (too few), 2, across the exhaustive / sampled boundary and of 200 members,
+    # an empty set, outliers; then the device chain on real match rows
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import triangulate_oracle as tro
+    rng = np.random.default_rng(8)
+    sc = tro.planted_scene(rng, 220, [1, 2, 2, 3, 9, 10, 11, 40, 200] * 3, noise=0.5, outliers=0.2)
+    off =np.cumsum([0] + [len(f) for f in sc["feats"]])
+    sets_of = np.searchsorted(off, sc["members"], side="right") - 1
+    tr = api.Tracks(sc["start"], sets_of, sc["members"] - off[sets_of], None, 0, 0, 0)
+    feats = []
+    for f in sc["feats"]:
+        r = np.zeros(len(f), api.FEATURE_DTYPE)
+        r["x"], r["y"] = f[:, 0], f[:, 1]
+        feats.append(r)
+    p = api.triangulate(feats, tr, sc["cams"], sc["poses"], max_error=3.0, n_samples=45, seed=1)
+    print("triangulate", p.counts, flush=True)
+    frames = [make_frame(320, 240, 18), make_frame(320, 240, 18)[:, ::-1].copy(), make_frame(320, 240, 19)]
+    ps = api.PopSift(api.Config(), mode=api.Config.MatchingMode, max_width=320, max_height=240, slots=1)
+    sets = [ps.enqueue(320, 240, im).getDev() for im in frames]
+    poses = [(np.eye(3), np.array([0.1 * k, 0.0, 0.0])) for k in range(3)]
+    t, p = api.triangulated_tracks(sets, [(0, 1), (1, 2), (0, 2)], [(300, 300, 160, 120)] * 3, poses, verify=dict(n_samples=100))
+    print("triangulate chain", len(t.start) - 1, p.counts, flush=True)
+    ps.uninit()
