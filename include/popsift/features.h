@@ -284,4 +284,37 @@ struct TrackPoints
 TrackPoints triangulateTracks(const std::vector<FeaturesDev*>& sets, const Tracks& tracks, const std::vector<Camera>& cameras,
                               const std::vector<Rigid>& poses, const TriangulateParams& params = TriangulateParams());
 
+/// Settings of bundleAdjust (same fields and rules as ps_bundle_params in popsift_b200_bundle.h).
+struct BundleParams
+{
+    enum Loss { Squared = 0, Huber = 1, Cauchy = 2 };
+    int    loss = Squared;
+    double loss_scale = 1.0;         // pixels
+    int    max_iters = 50;           // LM iterations, 0 .. 10000
+    double function_tol = 1e-6;      // relative cost decrease of an accepted step that stops
+    int    cg_max_iters = 100;       // CG iterations per LM iteration, 1 .. 10000
+    double cg_tol = 1e-6;            // relative residual that stops CG, [0, 1)
+    double initial_lambda = 1e-4;
+    int    scale_set = -1;           // -1, or the set one of whose translation components is held
+    int    scale_axis = 0;           // that component, 0 .. 2
+};
+
+/// What bundleAdjust did (ps_bundle_report); termination is PS_BA_MAX_ITERS .. PS_BA_NONFINITE_START.
+struct BundleReport
+{
+    double initial_cost = 0, final_cost = 0;
+    int    iterations = 0, accepted = 0, cg_iterations = 0, termination = 0;
+    int    n_obs = 0, n_points = 0, n_free_cams = 0;
+};
+
+/// Bundle adjustment on the device (an addition to the reference's interface; C ABI ps_bundle_adjust): the poses of the
+/// sets with fixed[i] == false and the points of the OK tracks of `points` (what triangulateTracks gave for `tracks`;
+/// its mask selects the observations) refined by Levenberg-Marquardt.  Returns the refined poses and the report, and
+/// updates points (X, error, angle of the OK tracks, obs_error of every member).  Throws like triangulateTracks, and for
+/// the arguments ps_bundle_adjust refuses.
+std::pair<std::vector<Rigid>, BundleReport> bundleAdjust(const std::vector<FeaturesDev*>& sets, const Tracks& tracks,
+                                                         const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+                                                         const std::vector<bool>& fixed, TrackPoints& points,
+                                                         const BundleParams& params = BundleParams());
+
 } // namespace popsift

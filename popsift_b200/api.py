@@ -116,6 +116,25 @@ TRI_STATUS = ("ok", "too_few_obs", "no_hypothesis", "too_few_inliers", "small_an
 assert C.sizeof(PsRigid) == 96 and C.sizeof(PsTriangulateParams) == 32 and C.sizeof(PsTriangulateCounts) == 24
 assert TRACK_POINT_DTYPE.itemsize == 40
 
+
+class PsBundleParams(C.Structure):
+    """ps_bundle_params (56 bytes)"""
+    _fields_ = [("loss", C.c_int32), ("max_iters", C.c_int32), ("cg_max_iters", C.c_int32), ("scale_set", C.c_int32),
+                ("scale_axis", C.c_int32), ("pad_", C.c_int32), ("loss_scale", C.c_double), ("function_tol", C.c_double),
+                ("cg_tol", C.c_double), ("initial_lambda", C.c_double)]
+
+
+class PsBundleReport(C.Structure):
+    """ps_bundle_report (48 bytes)"""
+    _fields_ = [("initial_cost", C.c_double), ("final_cost", C.c_double), ("iterations", C.c_int32), ("accepted", C.c_int32),
+                ("cg_iterations", C.c_int32), ("termination", C.c_int32), ("n_obs", C.c_int32), ("n_points", C.c_int32),
+                ("n_free_cams", C.c_int32), ("pad_", C.c_int32)]
+
+
+BA_LOSS = ("squared", "huber", "cauchy")
+BA_TERMINATION = ("max_iters", "function_tol", "lambda", "no_observations", "nonfinite_start")
+assert C.sizeof(PsBundleParams) == 56 and C.sizeof(PsBundleReport) == 48
+
 EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps_geometry", "ps_create", "ps_destroy",
            "ps_last_error", "ps_submit_u8", "ps_submit_f32", "ps_submit_dev_u8", "ps_counts", "ps_download",
            "ps_sync", "ps_debug_plane", "ps_debug_extrema", "ps_slot_geometry", "ps_set_timing", "ps_stage_ms",
@@ -133,6 +152,8 @@ TRACKS_EXPORTS = ["ps_tracks_from_edges", "ps_tracks_from_matches"]
 POSE_EXPORTS = ["ps_relative_pose_batch"]
 # multi-view triangulation, declared in popsift_b200_triangulate.h (same library)
 TRIANGULATE_EXPORTS = ["ps_triangulate_tracks"]
+# bundle adjustment, declared in popsift_b200_bundle.h (same library)
+BUNDLE_EXPORTS = ["ps_bundle_adjust"]
 
 _lib = None
 
@@ -197,6 +218,10 @@ def load_library():
         L.ps_triangulate_tracks.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                             C.c_void_p, C.c_int, C.POINTER(PsTriangulateParams), C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.POINTER(PsTriangulateCounts)]
+    if hasattr(L, "ps_bundle_adjust"):
+        L.ps_bundle_adjust.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                       C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsBundleParams), C.c_void_p, C.c_void_p,
+                                       C.POINTER(PsBundleReport)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -1122,6 +1147,78 @@ def triangulated_tracks(sets, pairs, cameras, poses, matches=None, min_length=2,
     finally:
         bufs.free()
     return tr, pts
+
+
+BundleReport = namedtuple("BundleReport", "initial_cost final_cost iterations accepted cg_iterations termination n_obs n_points "
+                                          "n_free_cams")
+BundleReport.__doc__ = """ps_bundle_report of ps_bundle_adjust (popsift_b200_bundle.h); termination is a name of BA_TERMINATION."""
+
+
+def _bundle_params(loss="squared", loss_scale=1.0, max_iters=50, function_tol=1e-6, cg_max_iters=100, cg_tol=1e-6,
+                   initial_lambda=1e-4, scale_set=-1, scale_axis=0) -> PsBundleParams:
+    if loss not in BA_LOSS:
+        raise PopSiftError("loss must be one of %s" % (BA_LOSS,))
+    return PsBundleParams(BA_LOSS.index(loss), int(max_iters), int(cg_max_iters), int(scale_set), int(scale_axis), 0,
+                          float(loss_scale), float(function_tol), float(cg_tol), float(initial_lambda))
+
+
+def _bundle_report(r) -> BundleReport:
+    return BundleReport(float(r.initial_cost), float(r.final_cost), int(r.iterations), int(r.accepted), int(r.cg_iterations),
+                        BA_TERMINATION[r.termination], int(r.n_obs), int(r.n_points), int(r.n_free_cams))
+
+
+def bundle_adjust(sets, tracks, points, cameras, poses, fixed, loss="squared", loss_scale=1.0, max_iters=50, function_tol=1e-6,
+                  cg_max_iters=100, cg_tol=1e-6, initial_lambda=1e-4, scale_set=-1, scale_axis=0, device=None):
+    """Bundle adjustment on the device (C ABI ps_bundle_adjust in popsift_b200_bundle.h; an addition to the reference's
+    interface): Levenberg-Marquardt on the poses of the free sets and the points of the OK tracks, with a Schur-complement
+    PCG solve.  `sets`, `tracks`, `cameras` and `poses` are triangulate()'s; `points` the TrackPoints triangulate() gave
+    (the OK tracks' members with mask 1 are the observations); `fixed` one bool per set (at least one True).  loss is
+    "squared", "huber" or "cauchy" at loss_scale pixels; scale_set / scale_axis hold one translation component of a free
+    set.  Returns (poses as a list of (R, t), TrackPoints with the refined X, error and angle and the final per-member
+    pixel errors, BundleReport)."""
+    lib = load_library()
+    prm = _bundle_params(loss, loss_scale, max_iters, function_tol, cg_max_iters, cg_tol, initial_lambda, scale_set, scale_axis)
+    bufs = _DevBuffers(lib)
+    try:
+        ptrs, n_feat = [], []
+        for s in sets:
+            if isinstance(s, FeaturesDev):
+                ptrs.append(s.getFeatures()); n_feat.append(s.getFeatureCount())
+            else:
+                f = np.ascontiguousarray(s.feat if isinstance(s, Features) else s, FEATURE_DTYPE)
+                ptrs.append(bufs.upload(f)); n_feat.append(len(f))
+        if device is None:
+            device = next((max(0, lib.ps_pointer_device(p)) for p, k in zip(ptrs, n_feat) if k > 0), 0)
+        cam = _c_cameras(cameras)
+        if len(cam) != len(n_feat) or len(poses) != len(n_feat) or len(fixed) != len(n_feat):
+            raise PopSiftError("one camera, one pose and one fixed flag per set expected")
+        off = np.concatenate([[0], np.cumsum(n_feat, dtype=np.int64)])
+        st = np.ascontiguousarray(tracks.start, np.int32)
+        mem = (off[np.asarray(tracks.set, np.int64)] + np.asarray(tracks.feature, np.int64)).astype(np.int32)
+        T, M = len(st) - 1, len(mem)
+        rec = np.zeros(T, TRACK_POINT_DTYPE)
+        for f in ("X", "error", "angle", "n_inliers", "status"):
+            rec[f] = getattr(points, f)
+        d_pts = bufs.upload(rec) if T else None
+        d_mask = bufs.upload(np.ascontiguousarray(points.mask, np.uint8)) if M else None
+        d_err = bufs.alloc(M * 4) if M else None
+        n = max(len(n_feat), 1)
+        c_fix = (C.c_uint8 * n)(*[1 if f else 0 for f in fixed])
+        rig_in = _c_rigids(poses)
+        rig_out = (PsRigid * n)()
+        rep = PsBundleReport()
+        rc = lib.ps_bundle_adjust(device, len(n_feat), (C.c_int32 * n)(*n_feat), (C.c_void_p * n)(*ptrs), cam.ctypes.data, rig_in, T,
+                                  bufs.upload(st) if T else None, bufs.upload(mem) if M else None, M, d_pts, d_mask, c_fix,
+                                  C.byref(prm), rig_out, d_err, C.byref(rep))
+        _check(lib, rc, "ps_bundle_adjust")
+        out = bufs.download(d_pts, T, TRACK_POINT_DTYPE) if T else rec
+        err = bufs.download(d_err, M, np.float32) if M else np.zeros(0, np.float32)
+    finally:
+        bufs.free()
+    new_poses = [(np.array(rig_out[i].R[:], np.float64).reshape(3, 3), np.array(rig_out[i].t[:], np.float64)) for i in range(len(n_feat))]
+    tp = TrackPoints(out["X"].copy(), out["error"].copy(), out["angle"].copy(), out["n_inliers"].copy(), out["status"].copy(),
+                     np.asarray(points.mask, np.uint8).copy(), err, dict(points.counts) if points.counts is not None else None)
+    return new_poses, tp, _bundle_report(rep)
 
 
 def _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, model, threshold, flags, u8) -> int:

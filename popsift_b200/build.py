@@ -26,7 +26,7 @@ NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "--fmad=false",   # no implicit contraction anywhere; every fma in the kernels is explicit
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu", "k_pose.cu", "k_retrieval.cu", "k_tracks.cu", "k_triangulate.cu",
+LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu", "k_pose.cu", "k_retrieval.cu", "k_tracks.cu", "k_triangulate.cu", "k_bundle.cu",
                "host/sift_conf.cpp", "host/features.cpp", "host/popsift.cpp", "host/device_prop.cpp", "host/log_dump.cpp"]
 DEMO_SOURCES = ["app/popsift_demo.cpp", "app/pgmread.cpp"]
 MATCH_SOURCES = ["app/popsift_match.cpp"]            # + app/pgmread.cpp
@@ -71,6 +71,10 @@ TRIANGULATE_MATH_CHECK = os.path.join(BIN_DIR, "triangulate_math_check")
 TRIANGULATE_MATH_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "triangulate_math_check.cpp")
 TRIANGULATE_CHECK = os.path.join(BIN_DIR, "triangulate_check")
 TRIANGULATE_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "triangulate_check.cpp")
+BUNDLE_MATH_CHECK = os.path.join(BIN_DIR, "bundle_math_check")
+BUNDLE_MATH_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "bundle_math_check.cpp")
+BUNDLE_CHECK = os.path.join(BIN_DIR, "bundle_check")
+BUNDLE_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "bundle_check.cpp")
 
 
 def _newer(target: str, deps) -> bool:
@@ -208,6 +212,16 @@ def build(verbose: bool = False, force: bool = False) -> str:
         # popsift::triangulateTracks against the C ABI (popsift_b200_triangulate.h)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), TRIANGULATE_CHECK_SRC, "-o",
                                TRIANGULATE_CHECK, "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
+    ba_hdrs = [os.path.join(CSRC, "k_bundle.h")] + tri_hdrs
+    if os.path.exists(BUNDLE_MATH_CHECK_SRC) and (force or _newer(BUNDLE_MATH_CHECK, [BUNDLE_MATH_CHECK_SRC] + ba_hdrs)):
+        # host-only: the Jacobians, loss, Rodrigues update and small solves of bundle adjustment, the same __host__
+        # __device__ functions the kernels use (no CUDA, no library); no contraction, as in the kernels
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-I" + CSRC, BUNDLE_MATH_CHECK_SRC, "-o",
+                               BUNDLE_MATH_CHECK])
+    if os.path.exists(BUNDLE_CHECK_SRC) and (force or _newer(BUNDLE_CHECK, [BUNDLE_CHECK_SRC, LIB] + hdrs)):
+        # popsift::bundleAdjust against the C ABI (popsift_b200_bundle.h)
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), BUNDLE_CHECK_SRC, "-o",
+                               BUNDLE_CHECK, "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
     pgm_src = os.path.join(CSRC, "app", "pgmread.cpp")
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):
         # host-only check of popsift-demo's image reader

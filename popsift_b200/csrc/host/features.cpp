@@ -9,6 +9,7 @@
 #include "popsift_b200_retrieval.h"
 #include "popsift_b200_tracks.h"
 #include "popsift_b200_triangulate.h"
+#include "popsift_b200_bundle.h"
 
 #include <algorithm>
 #include <cmath>
@@ -616,6 +617,98 @@ TrackPoints triangulateTracks(const std::vector<FeaturesDev*>& sets, const Track
     std::copy(c.n_status, c.n_status + 5, out.n_status);
     out.n_inlier_obs = c.n_inlier_obs;
     return out;
+}
+
+std::pair<std::vector<Rigid>, BundleReport> bundleAdjust(const std::vector<FeaturesDev*>& sets, const Tracks& tracks,
+                                                         const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+                                                         const std::vector<bool>& fixed, TrackPoints& points, const BundleParams& params)
+{
+    const Batch b("bundleAdjust", sets, {});
+    if (cameras.size() != sets.size()) throw std::runtime_error(b.who + ": one camera per set expected");
+    if (poses.size() != sets.size()) throw std::runtime_error(b.who + ": one pose per set expected");
+    if (fixed.size() != sets.size()) throw std::runtime_error(b.who + ": one fixed flag per set expected");
+    if (tracks.start.empty() || tracks.set.size() != tracks.feature.size() || (size_t)tracks.start.back() != tracks.set.size())
+        throw std::runtime_error(b.who + ": malformed tracks");
+    const size_t nt = tracks.start.size() - 1, nm = tracks.set.size();
+    if (points.points.size() != nt || points.mask.size() != nm) throw std::runtime_error(b.who + ": points do not match the tracks");
+    std::vector<int32_t> n_feat(sets.size());
+    std::vector<int64_t> off(sets.size() + 1, 0);
+    for (size_t i = 0; i < sets.size(); ++i) {
+        n_feat[i] = sets[i]->getFeatureCount();
+        off[i + 1] = off[i] + std::max(n_feat[i], 0);
+    }
+    std::vector<int32_t> mem(nm);
+    for (size_t k = 0; k < nm; ++k) {
+        const int s = tracks.set[k], f = tracks.feature[k];
+        if (s < 0 || (size_t)s >= sets.size() || f < 0 || f >= n_feat[s]) throw std::runtime_error(b.who + ": track member out of range");
+        mem[k] = (int32_t)(off[s] + f);
+    }
+    std::vector<ps_camera> cams(sets.size());
+    std::vector<ps_rigid> rig(sets.size()), out(sets.size());
+    std::vector<uint8_t> fix(sets.size());
+    for (size_t i = 0; i < sets.size(); ++i) {
+        cams[i] = ps_camera{cameras[i].fx, cameras[i].fy, cameras[i].cx, cameras[i].cy};
+        std::copy(poses[i].R, poses[i].R + 9, rig[i].R);
+        std::copy(poses[i].t, poses[i].t + 3, rig[i].t);
+        fix[i] = fixed[i] ? 1 : 0;
+    }
+    std::vector<ps_track_point> h(nt);
+    for (size_t t = 0; t < nt; ++t) {
+        const TrackPoint& p = points.points[t];
+        std::copy(p.X, p.X + 3, h[t].X);
+        h[t].error = p.error;
+        h[t].angle = p.angle;
+        h[t].n_inliers = p.n_inliers;
+        h[t].status = p.status;
+    }
+    ps_bundle_params prm{};
+    prm.loss = params.loss;
+    prm.max_iters = params.max_iters;
+    prm.cg_max_iters = params.cg_max_iters;
+    prm.scale_set = params.scale_set;
+    prm.scale_axis = params.scale_axis;
+    prm.loss_scale = params.loss_scale;
+    prm.function_tol = params.function_tol;
+    prm.cg_tol = params.cg_tol;
+    prm.initial_lambda = params.initial_lambda;
+    DevBuf start(tracks.start.size() * sizeof(int32_t), b.who), members(nm * sizeof(int32_t), b.who);
+    DevBuf pts(std::max<size_t>(nt, 1) * sizeof(ps_track_point), b.who), mask(nm, b.who), err(nm * sizeof(float), b.who);
+    check(ps_host_to_dev(start.p, tracks.start.data(), tracks.start.size() * sizeof(int32_t)), b.who);
+    check(ps_host_to_dev(members.p, mem.data(), nm * sizeof(int32_t)), b.who);
+    check(ps_host_to_dev(pts.p, h.data(), nt * sizeof(ps_track_point)), b.who);
+    check(ps_host_to_dev(mask.p, points.mask.data(), nm), b.who);
+    ps_bundle_report r;
+    check(ps_bundle_adjust(b.dev, (int)sets.size(), n_feat.data(), b.feat.data(), cams.data(), rig.data(), (int)nt,
+                           static_cast<const int32_t*>(start.p), static_cast<const int32_t*>(members.p), (int)nm,
+                           static_cast<ps_track_point*>(pts.p), static_cast<const uint8_t*>(mask.p), fix.data(), &prm, out.data(),
+                           static_cast<float*>(err.p), &r),
+          b.who, "ps_bundle_adjust");
+    check(ps_dev_to_host(h.data(), pts.p, nt * sizeof(ps_track_point)), b.who);
+    points.obs_error.resize(nm);
+    check(ps_dev_to_host(points.obs_error.data(), err.p, nm * sizeof(float)), b.who);
+    for (size_t t = 0; t < nt; ++t) {
+        TrackPoint& p = points.points[t];
+        std::copy(h[t].X, h[t].X + 3, p.X);
+        p.error = h[t].error;
+        p.angle = h[t].angle;
+    }
+    std::pair<std::vector<Rigid>, BundleReport> res;
+    res.first.resize(sets.size());
+    for (size_t i = 0; i < sets.size(); ++i) {
+        std::copy(out[i].R, out[i].R + 9, res.first[i].R);
+        std::copy(out[i].t, out[i].t + 3, res.first[i].t);
+    }
+    BundleReport& R = res.second;
+    R.initial_cost = r.initial_cost;
+    R.final_cost = r.final_cost;
+    R.iterations = r.iterations;
+    R.accepted = r.accepted;
+    R.cg_iterations = r.cg_iterations;
+    R.termination = r.termination;
+    R.n_obs = r.n_obs;
+    R.n_points = r.n_points;
+    R.n_free_cams = r.n_free_cams;
+    return res;
 }
 
 } // namespace popsift

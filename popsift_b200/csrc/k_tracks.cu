@@ -14,9 +14,10 @@
 //   emit      an exclusive scan over the segment heads (the head of a segment is its root, its smallest gid) packs
 //             (track index, member position) into one uint64; the heads write d_track_start, the members d_members and
 //             d_track_of
-// No library sort or scan: both are here.
+// No library sort or scan: both are in k_scan.h.
 #include "ps_internal.h"
 #include "k_match_common.h"
+#include "k_scan.h"
 #include "popsift_b200_tracks.h"
 
 #include <algorithm>
@@ -28,11 +29,6 @@ namespace psb {
 namespace {
 
 constexpr int kT = 256;                 // threads of the element-wise kernels
-constexpr int kScanT = 1024;            // threads of a scan block
-constexpr int kScanPer = 4;             // consecutive elements per scan thread
-constexpr long long kScanChunk = (long long)kScanT * kScanPer;
-constexpr int kRadixRounds = 16;        // rounds of kT elements per radix tile
-constexpr long long kRadixTile = (long long)kT * kRadixRounds;
 constexpr uint32_t kConflict = 0x80000000u;
 
 __device__ __forceinline__ long long gtid() { return (long long)blockIdx.x * blockDim.x + threadIdx.x; }
@@ -170,139 +166,11 @@ __global__ void __launch_bounds__(kT) tracks_gather_kernel(const int* __restrict
     if (cnt[parent[v]] >= 2) out[pos[v]] = (int)v;
 }
 
-// ---- device-wide exclusive scan: blocks of kScanChunk elements, the block sums scanned recursively, then added back
-
-template <class T>
-__global__ void __launch_bounds__(kScanT) scan_block_kernel(T* data, long long n, T* __restrict__ sums)
-{
-    __shared__ T warp_sum[kScanT / 32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const long long base = blockIdx.x * kScanChunk + (long long)threadIdx.x * kScanPer;
-    T v[kScanPer];
-    T own = 0;
-#pragma unroll
-    for (int k = 0; k < kScanPer; ++k) {
-        const T x = base + k < n ? data[base + k] : T(0);
-        v[k] = own;
-        own += x;
-    }
-    T inc = own;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const T y = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += y;
-    }
-    if (lane == 31) warp_sum[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-        const T x = warp_sum[lane];
-        T xi = x;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const T y = __shfl_up_sync(0xffffffffu, xi, o);
-            if (lane >= o) xi += y;
-        }
-        warp_sum[lane] = xi - x;
-    }
-    __syncthreads();
-    const T off = warp_sum[w] + inc - own;
-#pragma unroll
-    for (int k = 0; k < kScanPer; ++k)
-        if (base + k < n) data[base + k] = v[k] + off;
-    if (threadIdx.x == kScanT - 1) sums[blockIdx.x] = off + own;
-}
-
-template <class T>
-__global__ void __launch_bounds__(kScanT) scan_add_kernel(T* __restrict__ data, long long n, const T* __restrict__ sums)
-{
-    const T s = sums[blockIdx.x];
-    const long long base = blockIdx.x * kScanChunk + (long long)threadIdx.x * kScanPer;
-#pragma unroll
-    for (int k = 0; k < kScanPer; ++k)
-        if (base + k < n) data[base + k] += s;
-}
-
-// elements of partial sums every level of a scan of n elements needs
-long long scan_partials(long long n)
-{
-    long long total = 0;
-    do {
-        n = (n + kScanChunk - 1) / kScanChunk;
-        total += n;
-    } while (n > 1);
-    return total;
-}
-
-// data[0, n) becomes its exclusive prefix sum; *total (device) the sum of all; partial: scan_partials(n) elements
-template <class T>
-int scan_exclusive(T* data, long long n, T* partial, T* total, cudaStream_t st)
-{
-    const unsigned nb = blocks_for(n, kScanChunk);
-    if (nb == 1) {
-        scan_block_kernel<T><<<1, kScanT, 0, st>>>(data, n, total);
-        return 1;
-    }
-    scan_block_kernel<T><<<nb, kScanT, 0, st>>>(data, n, partial);
-    const int launches = scan_exclusive(partial, (long long)nb, partial + nb, total, st);
-    scan_add_kernel<T><<<nb, kScanT, 0, st>>>(data, n, partial);
-    return launches + 2;
-}
-
-// ---- stable LSD radix sort of the active gids by root, 8 bits per pass
-
-__global__ void __launch_bounds__(kT) radix_hist_kernel(const int* __restrict__ vals, int A, const int* __restrict__ parent,
-                                                        int shift, int* __restrict__ hist, int nb)
-{
-    __shared__ int h[256];
-    h[threadIdx.x] = 0;
-    __syncthreads();
-    const long long base = blockIdx.x * kRadixTile;
-    for (int r = 0; r < kRadixRounds; ++r) {
-        const long long i = base + r * kT + threadIdx.x;
-        if (i < A) atomicAdd(&h[(parent[vals[i]] >> shift) & 255], 1);
-    }
-    __syncthreads();
-    hist[(size_t)threadIdx.x * nb + blockIdx.x] = h[threadIdx.x];
-}
-
-// hist: the exclusive scan of the histograms, digit-major, so hist[d * nb + b] is where tile b's first digit-d entry goes.
-// Each round of kT entries ranks its entries per digit in index order (warp match + per-warp counts), so the pass is
-// stable.
-__global__ void __launch_bounds__(kT) radix_scatter_kernel(const int* __restrict__ vin, int* __restrict__ vout, int A,
-                                                           const int* __restrict__ parent, int shift, const int* __restrict__ hist,
-                                                           int nb)
-{
-    constexpr int W = kT / 32;
-    __shared__ int next[256];      // the next output position of each digit
-    __shared__ int wpos[W][256];   // per round: the entries of warp w with digit d, then their first position
-    const int t = threadIdx.x, lane = t & 31, w = t >> 5;
-    next[t] = hist[(size_t)t * nb + blockIdx.x];
-    const unsigned lt = (1u << lane) - 1u;
-    const long long base = blockIdx.x * kRadixTile;
-    for (int r = 0; r < kRadixRounds; ++r) {
-        for (int k = t; k < W * 256; k += kT) (&wpos[0][0])[k] = 0;
-        __syncthreads();
-        const long long i = base + r * kT + t;
-        const bool valid = i < A;
-        const int v = valid ? vin[i] : 0;
-        const int d = valid ? (parent[v] >> shift) & 255 : -1;
-        const unsigned peers = __match_any_sync(0xffffffffu, d);
-        const int rank = __popc(peers & lt);
-        if (valid && rank == 0) wpos[w][d] = __popc(peers);
-        __syncthreads();
-        int run = next[t];
-#pragma unroll
-        for (int q = 0; q < W; ++q) {
-            const int c = wpos[q][t];
-            wpos[q][t] = run;
-            run += c;
-        }
-        next[t] = run;
-        __syncthreads();
-        if (valid) vout[wpos[w][d] + rank] = v;
-        __syncthreads();
-    }
-}
+// the radix sort's key of an active gid: its root
+struct RootKey {
+    const int* parent;
+    __device__ __forceinline__ int operator()(int v) const { return parent[v]; }
+};
 
 // ---- classify and emit
 
@@ -483,9 +351,9 @@ int run_tracks(int n_sets, const int32_t* n_feat, long long n_items, const std::
         int* src = va;
         int* dst = vb;
         for (int p = 0; p < passes; ++p) {
-            radix_hist_kernel<<<nb, kT, 0, st>>>(src, A, parent, 8 * p, hist, nb);
+            radix_hist_kernel<<<nb, kRadixT, 0, st>>>(src, A, RootKey{parent}, 8 * p, hist, nb);
             launches += 1 + scan_exclusive(hist, 256ll * nb, static_cast<int*>(part), &stat->hist_total, st);
-            radix_scatter_kernel<<<nb, kT, 0, st>>>(src, dst, A, parent, 8 * p, hist, nb);
+            radix_scatter_kernel<<<nb, kRadixT, 0, st>>>(src, dst, A, RootKey{parent}, 8 * p, hist, nb);
             ++launches;
             std::swap(src, dst);
         }

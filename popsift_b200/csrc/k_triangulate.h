@@ -42,12 +42,15 @@ PSV_HD bool tri_hypothesis(const double* Ca, const double* da, const double* Cb,
 }
 
 // The pixel residual of pixel (x, y) under X: X_c = R X + t, false unless z = X_c[2] > 0; iz = 1 / z,
-// e_x = fx (X_c[0] iz) + cx - x, e_y = fy (X_c[1] iz) + cy - y.  Jx / Jy (optional): d e_x / dX, d e_y / dX.
+// e_x = fx (X_c[0] iz) + cx - x, e_y = fy (X_c[1] iz) + cy - y.  Jx / Jy (optional): d e_x / dX, d e_y / dX.  Xc_out
+// (optional): X_c, written whether or not z > 0 (bundle adjustment's pose Jacobian, k_bundle.h).
 PSV_HD bool tri_residual(const TriCam& K, const double* X, double x, double y, double& ex, double& ey, double* Jx = nullptr,
-                         double* Jy = nullptr)
+                         double* Jy = nullptr, double* Xc_out = nullptr)
 {
     double Xc[3];
     for (int r = 0; r < 3; ++r) Xc[r] = K.R[3 * r] * X[0] + K.R[3 * r + 1] * X[1] + K.R[3 * r + 2] * X[2] + K.t[r];
+    if (Xc_out)
+        for (int r = 0; r < 3; ++r) Xc_out[r] = Xc[r];
     if (!(Xc[2] > 0.0)) return false;
     const double iz = 1.0 / Xc[2];
     const double p = Xc[0] * iz, q = Xc[1] * iz;

@@ -13,6 +13,7 @@
 #include "popsift_b200_pose.h"
 #include "popsift_b200_tracks.h"
 #include "popsift_b200_triangulate.h"
+#include "popsift_b200_bundle.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1400,22 +1401,30 @@ static bool rigid_ok(const ps_rigid& p)
     return det > 0.0;
 }
 
+// the host checks ps_triangulate_tracks and ps_bundle_adjust share: the counts, the cameras and the poses
+static bool check_tracks_call(int n_sets, const int32_t* n_feat, const ps_feature* const* d_feat, const ps_camera* cams,
+                              const ps_rigid* poses, int n_tracks, int n_members)
+{
+    if (n_sets < 0 || n_tracks < 0 || n_members < 0) return false;
+    if (n_sets > 0 && (!n_feat || !d_feat || !cams || !poses)) return false;
+    for (int i = 0; i < n_sets; ++i) {
+        const ps_camera& c = cams[i];
+        if (!std::isfinite(c.fx) || !(c.fx > 0.0f) || !std::isfinite(c.fy) || !(c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
+            return false;
+        if (!rigid_ok(poses[i])) return false;
+    }
+    return true;
+}
+
 extern "C" int ps_triangulate_tracks(int device, int n_sets, const int32_t* n_feat, const ps_feature* const* d_feat, const ps_camera* cams,
                                      const ps_rigid* poses, int n_tracks, const int32_t* d_track_start, const int32_t* d_members, int n_members,
                                      const ps_triangulate_params* prm, ps_track_point* d_points, uint8_t* d_obs_mask, float* d_obs_error,
                                      ps_triangulate_counts* counts)
 {
-    if (n_sets < 0 || n_tracks < 0 || n_members < 0 || !prm || !counts) return PS_ERR_ARG;
+    if (!prm || !counts || !check_tracks_call(n_sets, n_feat, d_feat, cams, poses, n_tracks, n_members)) return PS_ERR_ARG;
     if (!std::isfinite(prm->max_error) || !(prm->max_error > 0.0f)) return PS_ERR_ARG;
     if (!(prm->min_angle >= 0.0f && prm->min_angle < 90.0f)) return PS_ERR_ARG;
     if (prm->min_views < 2 || prm->n_samples < 1 || prm->n_samples > 65536 || prm->refine_iters < 0 || prm->refine_iters > 32) return PS_ERR_ARG;
-    if (n_sets > 0 && (!n_feat || !d_feat || !cams || !poses)) return PS_ERR_ARG;
-    for (int i = 0; i < n_sets; ++i) {
-        const ps_camera& c = cams[i];
-        if (!std::isfinite(c.fx) || !(c.fx > 0.0f) || !std::isfinite(c.fy) || !(c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
-            return PS_ERR_ARG;
-        if (!rigid_ok(poses[i])) return PS_ERR_ARG;
-    }
     if (n_tracks == 0) {
         std::memset(counts, 0, sizeof(*counts));
         return PS_OK;
@@ -1435,6 +1444,56 @@ extern "C" int ps_triangulate_tracks(int device, int n_sets, const int32_t* n_fe
         return PS_ERR_ARG;
     }
     return finish("ps_triangulate_tracks", n, err);
+}
+
+extern "C" int ps_bundle_adjust(int device, int n_sets, const int32_t* n_feat, const ps_feature* const* d_feat, const ps_camera* cams,
+                                const ps_rigid* poses_in, int n_tracks, const int32_t* d_track_start, const int32_t* d_members, int n_members,
+                                ps_track_point* d_points, const uint8_t* d_obs_mask, const uint8_t* fixed, const ps_bundle_params* prm,
+                                ps_rigid* poses_out, float* d_obs_error, ps_bundle_report* report)
+{
+    if (!prm || !report || !poses_out || !fixed) return PS_ERR_ARG;
+    if (!check_tracks_call(n_sets, n_feat, d_feat, cams, poses_in, n_tracks, n_members)) return PS_ERR_ARG;
+    if (prm->loss < PS_LOSS_SQUARED || prm->loss > PS_LOSS_CAUCHY) return PS_ERR_ARG;
+    if (prm->max_iters < 0 || prm->max_iters > 10000 || prm->cg_max_iters < 1 || prm->cg_max_iters > 10000) return PS_ERR_ARG;
+    if (!std::isfinite(prm->loss_scale) || !(prm->loss_scale > 0.0)) return PS_ERR_ARG;
+    if (!std::isfinite(prm->function_tol) || !(prm->function_tol >= 0.0)) return PS_ERR_ARG;
+    if (!(prm->cg_tol >= 0.0 && prm->cg_tol < 1.0)) return PS_ERR_ARG;
+    if (!(prm->initial_lambda > 0.0 && prm->initial_lambda <= 1e32)) return PS_ERR_ARG;
+    if (prm->scale_set < -1 || prm->scale_set >= n_sets || prm->scale_axis < 0 || prm->scale_axis > 2) return PS_ERR_ARG;
+    bool any_fixed = false;
+    for (int i = 0; i < n_sets; ++i) {
+        if (fixed[i] > 1) return PS_ERR_ARG;
+        any_fixed |= fixed[i] == 1;
+    }
+    if (!any_fixed) return PS_ERR_ARG;
+    if (n_tracks == 0) {
+        std::memset(report, 0, sizeof(*report));
+        report->termination = PS_BA_NO_OBSERVATIONS;
+        if (poses_out != poses_in) std::memcpy(poses_out, poses_in, (size_t)n_sets * sizeof(ps_rigid));
+        return PS_OK;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    int64_t N = 0;
+    if (!check_sets(device, n_sets, n_feat, d_feat, 0, &N) || N >= 0x80000000LL) return PS_ERR_ARG;
+    if (ps_pointer_device(d_track_start) != device || ps_pointer_device(d_points) != device) return PS_ERR_ARG;
+    if (n_members > 0 && (ps_pointer_device(d_members) != device || ps_pointer_device(d_obs_mask) != device)) return PS_ERR_ARG;
+    if (d_obs_error && ps_pointer_device(d_obs_error) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    bool bad = false;
+    std::vector<ps_rigid> out(n_sets);
+    ps_bundle_report rep{};
+    const int n = run_bundle_adjust(n_sets, n_feat, d_feat, cams, poses_in, n_tracks, d_track_start, d_members, n_members, d_points, d_obs_mask,
+                                    fixed, *prm, out.data(), d_obs_error, &rep, &bad, nullptr, &err);
+    if (n >= 0 && bad) {
+        g_create_error = "ps_bundle_adjust: a member id or d_track_start is out of range";
+        return PS_ERR_ARG;
+    }
+    const int rc = finish("ps_bundle_adjust", n, err);
+    if (rc == PS_OK) {
+        std::memcpy(poses_out, out.data(), (size_t)n_sets * sizeof(ps_rigid));
+        *report = rep;
+    }
+    return rc;
 }
 
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)

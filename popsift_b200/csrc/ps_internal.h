@@ -4,6 +4,7 @@
 #include "popsift_b200_pose.h"
 #include "popsift_b200_tracks.h"
 #include "popsift_b200_triangulate.h"
+#include "popsift_b200_bundle.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
@@ -285,5 +286,14 @@ int run_triangulate_tracks(int n_sets, const int32_t* n_feat, const ps_feature* 
                            int n_tracks, const int32_t* track_start, const int32_t* members, int n_members,
                            const ps_triangulate_params& prm, ps_track_point* points, uint8_t* obs_mask, float* obs_error,
                            ps_triangulate_counts* counts, bool* bad, cudaStream_t st, const char** err);
+
+// bundle adjustment (include/popsift_b200_bundle.h, k_bundle.cu), arguments already validated except the member ids and
+// d_track_start, which the first pass checks: a bad one sets *bad, and the call returns before writing any output.
+// Synchronous on `st` (one small read-back per LM iteration); *report and poses_out are written when it returns >= 0 with
+// *bad false.  Returns the number of kernels launched or -1 (*err set).
+int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const* feat, const ps_camera* cams, const ps_rigid* poses_in,
+                      int n_tracks, const int32_t* track_start, const int32_t* members, int n_members, ps_track_point* points,
+                      const uint8_t* obs_mask, const uint8_t* fixed, const ps_bundle_params& prm, ps_rigid* poses_out, float* obs_error,
+                      ps_bundle_report* report, bool* bad, cudaStream_t st, const char** err);
 
 } // namespace psb

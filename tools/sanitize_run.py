@@ -184,3 +184,38 @@ if only in ("all", "triangulate"):
     t, p = api.triangulated_tracks(sets, [(0, 1), (1, 2), (0, 2)], [(300, 300, 160, 120)] * 3, poses, verify=dict(n_samples=100))
     print("triangulate chain", len(t.start) - 1, p.counts, flush=True)
     ps.uninit()
+if only in ("all", "bundle"):
+    # bundle adjustment: each loss on a planted scene with a fixed set, a held scale component, a set without features,
+    # masked members and non-OK tracks; a non-finite start; structure only
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import bundle_oracle as bo
+    rng = np.random.default_rng(9)
+    sc = bo.planted(rng, 12, [2, 3, 5, 9, 12] * 20, noise=0.5, outliers=0.1)
+    sc["feats"] = list(sc["feats"]) + [np.zeros((0, 2), np.float32)]
+    sc["cams"] = np.concatenate([sc["cams"], sc["cams"][:1]])
+    sc["poses"] = list(sc["poses"]) + [sc["poses"][0]]
+    off = np.cumsum([0] + [len(f) for f in sc["feats"]])
+    sets_of = np.searchsorted(off, sc["members"], side="right") - 1
+    tr = api.Tracks(sc["start"], sets_of, sc["members"] - off[sets_of], None, 0, 0, 0)
+    feats = []
+    for f in sc["feats"]:
+        r = np.zeros(len(f), api.FEATURE_DTYPE)
+        r["x"], r["y"] = f[:, 0], f[:, 1]
+        feats.append(r)
+    status = sc["status"].copy()
+    status[::7] = 3
+    mask = sc["mask"].copy()
+    mask[::5] = 0
+    tp = api.TrackPoints(sc["X0"], np.zeros(100, np.float32), np.zeros(100, np.float32), np.diff(sc["start"]).astype(np.int32), status, mask,
+                         None, None)
+    fixed = [True] + [False] * 12
+    for loss in ("squared", "huber", "cauchy"):
+        _, _, rep = api.bundle_adjust(feats, tr, tp, sc["cams"], sc["poses"], fixed, loss=loss, max_iters=5, scale_set=1, scale_axis=2)
+        print("bundle", loss, rep, flush=True)
+    _, _, rep = api.bundle_adjust(feats, tr, tp, sc["cams"], sc["poses"], [True] * 13, max_iters=3)
+    print("bundle structure only", rep, flush=True)
+    R, t = sc["poses"][4]
+    bad = list(sc["poses"])
+    bad[4] = (np.diag([-1.0, 1.0, -1.0]) @ R, np.diag([-1.0, 1.0, -1.0]) @ t)
+    _, _, rep = api.bundle_adjust(feats, tr, tp, sc["cams"], bad, fixed)
+    print("bundle non-finite start", rep, flush=True)
