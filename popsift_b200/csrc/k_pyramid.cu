@@ -445,6 +445,18 @@ int launch_level0_any(const PIX* img, size_t img_pitch, int w, int h, float upsc
 
 } // namespace
 
+int launch_level01_u8(const uint8_t* img, size_t img_pitch, int w, int h, float upscale, int sift_mode,
+                      const OctaveView& o0, const GaussRow& dd, const GaussRow& inc0, const GaussRow& g1, cudaStream_t st)
+{
+    if (!use_march()) return 0;
+    // as launch_level0_any for octave 0
+    float shift = 0.5f;
+    if (sift_mode == PS_MODE_POPSIFT || sift_mode == PS_MODE_VLFEAT) shift = 0.5f * powf(2.0f, upscale);
+    const int R = (dd.span > inc0.span ? dd.span : inc0.span) - 1;
+    return march_level01_u8(img, img_pitch, w, h, shift, o0, make_taps(dd), make_taps(inc0), R, make_taps(g1), g1.span - 1,
+                            level0_plan(w, h, o0.w, o0.h, shift, R), st);
+}
+
 int level0_plan_for(int w, int h, int W, int H, float shift, int R) { return level0_plan(w, h, W, H, shift, R); }
 
 int launch_level0_u8(const uint8_t* img, size_t img_pitch, int w, int h, float upscale, int sift_mode,

@@ -43,6 +43,10 @@ enum { LEVEL0_IDEAL_X2 = 0,   // exactly 2x: every fetch has fraction 0 or 1/2 a
        LEVEL0_PER_TAP  = 2 }; // neither: every tap is fetched at its own coordinate
 int march_level0_u8(const uint8_t* img, size_t img_pitch, int w, int h, float shift, const OctaveView& o0,
                     const Taps& dd, const Taps& inc0, int R, int plan, cudaStream_t st);
+// levels 0 and 1 of octave 0 in one launch (march_level01x2_kernel): the exact-2x 8-bit path with R0 == R1 == 5; returns 0
+// (nothing launched) anywhere else
+int march_level01_u8(const uint8_t* img, size_t img_pitch, int w, int h, float shift, const OctaveView& o0,
+                     const Taps& dd, const Taps& inc0, int R0, const Taps& t1, int R1, int plan, cudaStream_t st);
 int march_level0_f32(const float* img, size_t img_pitch, int w, int h, float shift, const OctaveView& o0,
                      const Taps& dd, const Taps& inc0, int R, int plan, cudaStream_t st);
 

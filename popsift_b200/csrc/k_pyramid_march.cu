@@ -154,7 +154,8 @@ __device__ __forceinline__ void patch_halo(float* __restrict__ S, int x0, int W)
 
 // ---- row pass: stage -> ring ------------------------------------------------------------------
 
-template <int R, bool LEVEL0>
+// SWP: stage row stride, HS: ring row stride (the defaults are the level kernels' layout)
+template <int R, bool LEVEL0, int SWP = Geo<R>::SWP, int HS = HBW>
 __device__ __forceinline__ void row_pass(const float* __restrict__ S, float* __restrict__ HB, int slot0, const Taps& t)
 {
     using G = Geo<R>;
@@ -162,7 +163,7 @@ __device__ __forceinline__ void row_pass(const float* __restrict__ S, float* __r
     const int g = threadIdx.x >> 4;             // 16-column group (0..7)
     constexpr int WIN = 16 + 2 * G::RP;
     float w[WIN];
-    const float* p = S + j * G::SWP + 16 * g;
+    const float* p = S + j * SWP + 16 * g;
 #pragma unroll
     for (int m = 0; m < WIN / 4; ++m) {
         const float4 v = *reinterpret_cast<const float4*>(p + 4 * m);
@@ -170,7 +171,7 @@ __device__ __forceinline__ void row_pass(const float* __restrict__ S, float* __r
     }
     int slot = slot0 + j;
     if (slot >= G::RING) slot -= G::RING;
-    float* o = HB + slot * HBW + 16 * g;
+    float* o = HB + slot * HS + 16 * g;
 #pragma unroll
     for (int q4 = 0; q4 < 4; ++q4) {
         float r[4];
@@ -206,6 +207,44 @@ __device__ __forceinline__ f32x2 fma2(f32x2 a, float g, f32x2 c) { return make_f
 
 constexpr int QH = Q / 2;   // output rows per thread in the column pass
 
+// one output row jj of a column pair from its window of ring lines
+template <int R>
+__device__ __forceinline__ f32x2 col_sum(const f32x2 (&win)[QH + 2 * R], int jj, const Taps& t)
+{
+    f32x2 acc = make_float2(0.0f, 0.0f);
+#pragma unroll
+    for (int off = R; off > 0; --off) {
+        acc = fma2(win[jj + R - off], t.g[off], acc);
+        acc = fma2(win[jj + R + off], t.g[off], acc);
+    }
+    return fma2(win[jj + R], t.g[0], acc);
+}
+
+// the QH + 2R ring lines of ring column c (even) that rows jbase .. jbase+QH-1 of the chunk's output block need; HS is
+// the ring's row stride
+template <int R, int HS = HBW>
+__device__ __forceinline__ void col_window(const float* __restrict__ HB, int slot_oldest, int jbase, int c, f32x2 (&win)[QH + 2 * R])
+{
+    using G = Geo<R>;
+    int first = slot_oldest + jbase;                    // ring slot of the first window line (warp-uniform, a multiple of 8)
+    if (first >= G::RING) first -= G::RING;
+    // `first` is the line Q + 2R' lines before the newest (R' = R rounded so that the ring is a multiple of 8); the window
+    // proper starts PAD lines later.  It wraps around the ring at most once, and only between two blocks of 8 lines (RING,
+    // the chunk height and the half-chunk offset are multiples of 8): one base-pointer select per block, every line at a
+    // compile-time offset from it.
+    constexpr int PAD = G::RING - Q - 2 * R;
+    const int nb = (G::RING - first) >> 3;              // blocks before the wrap
+    const float* a0 = HB + first * HS + c;
+    const float* a1 = a0 - G::RING * HS;
+#pragma unroll
+    for (int b = 0; b < (PAD + QH + 2 * R + 7) / 8; ++b) {
+        const float* base = (b < nb) ? a0 : a1;
+#pragma unroll
+        for (int p = (8 * b > PAD ? 8 * b : PAD); p < 8 * b + 8 && p < PAD + QH + 2 * R; ++p)
+            win[p - PAD] = *reinterpret_cast<const f32x2*>(base + p * HS);
+    }
+}
+
 // Candidates (CandSink): a lane forms its two DoG samples (output - centre source row) in registers, notes
 // the rows in which one of them passes the peak threshold -- one compare pair and one predicated OR per row
 // in the hot loop -- and afterwards, if it has any, reserves entries of the block's list region with ONE
@@ -223,13 +262,7 @@ __device__ __forceinline__ void col_emit(const f32x2 (&win)[QH + 2 * R], const f
     unsigned pm = 0;
 #pragma unroll
     for (int jj = 0; jj < QH; ++jj) {
-        f32x2 acc = make_float2(0.0f, 0.0f);
-#pragma unroll
-        for (int off = R; off > 0; --off) {
-            acc = fma2(win[jj + R - off], t.g[off], acc);
-            acc = fma2(win[jj + R + off], t.g[off], acc);
-        }
-        acc = fma2(win[jj + R], t.g[0], acc);
+        const f32x2 acc = col_sum<R>(win, jj, t);
         const int j = jbase + jj;                       // row of the chunk's output block (0..Q-1)
         const bool ok = !GUARD || (col_in && y_first + j >= ys && y_first + j < ye);
         if (ok) {
@@ -269,27 +302,10 @@ __device__ __forceinline__ void col_pass(const float* __restrict__ HB, const flo
                                          float* __restrict__ next0, int pitch, int next_pitch, const Taps& t,
                                          const CandSink& sink = CandSink(), int* cand_n = nullptr)
 {
-    using G = Geo<R>;
     const int c2 = 2 * (threadIdx.x & 63);
     const int jbase = (threadIdx.x >> 6) * QH;          // 0 or Q/2 (warp-uniform)
     f32x2 win[QH + 2 * R];
-    int first = slot_oldest + jbase;                    // ring slot of the first window line (warp-uniform, a multiple of 8)
-    if (first >= G::RING) first -= G::RING;
-    // `first` is the line Q + 2R' lines before the newest (R' = R rounded so that the ring is a multiple of 8); the window
-    // proper starts PAD lines later.  It wraps around the ring at most once, and only between two blocks of 8 lines (RING,
-    // the chunk height and the half-chunk offset are multiples of 8): one base-pointer select per block, every line at a
-    // compile-time offset from it.
-    constexpr int PAD = G::RING - Q - 2 * R;
-    const int nb = (G::RING - first) >> 3;              // blocks before the wrap
-    const float* a0 = HB + first * HBW + c2;
-    const float* a1 = a0 - G::RING * HBW;
-#pragma unroll
-    for (int b = 0; b < (PAD + QH + 2 * R + 7) / 8; ++b) {
-        const float* base = (b < nb) ? a0 : a1;
-#pragma unroll
-        for (int p = (8 * b > PAD ? 8 * b : PAD); p < 8 * b + 8 && p < PAD + QH + 2 * R; ++p)
-            win[p - PAD] = *reinterpret_cast<const f32x2*>(base + p * HBW);
-    }
+    col_window<R>(HB, slot_oldest, jbase, c2, win);
     const int x = x0 + c2;
     const int yb = y_first + jbase;
     if (yb + QH <= ys || yb >= ye) return;                     // nothing of this half-block is inside the segment (warp-uniform)
@@ -477,22 +493,81 @@ march_level0_kernel(const PIX* __restrict__ img, size_t img_pitch, int w, int h,
 // r16 = (257*s4 + 2) >> 2, value = r16/65535.  Per chunk the CTA needs 9 source rows x (SW/2 + 1) bytes:
 // they are staged as raw bytes with 4-byte cp.async two chunks ahead (the tile is < 1 KB), then
 // "expanded" into the float staging buffer: thread = virtual column, the column's 9 row sums live in
-// registers and the row pairing is static because the chunk's first row has the parity of R.
-template <int R>
-struct Geo0 {
-    using G = Geo<R>;
+// registers and the row pairing is static because the parity of the chunk's first row is known (P below).
+//
+// Tile0<SW>: the raw byte tiles of SW staged virtual columns starting at X = x0 - RP (SW/2 + 1 source columns, rounded)
+template <int SW_>
+struct Tile0 {
+    static constexpr int SW = SW_;
     static constexpr int TROWS = Q / 2 + 2;             // source rows per tile (9 used away from the border)
-    static constexpr int TSW = G::SW / 2 + 4;           // bytes per tile row (multiple of 4)
+    static constexpr int TSW = SW / 2 + 4;              // bytes per tile row (multiple of 4)
     static constexpr int PIECES = TROWS * (TSW / 4);    // 4-byte pieces per tile
     static constexpr int NP = (PIECES + NT - 1) / NT;
     static constexpr int AHEAD = 2, NRAW = AHEAD + 2;
-    static constexpr int TAIL = G::SW - NT;             // staged columns beyond the first NT (= 2*RP)
-    // float staging buffer, ring, raw tiles
-    static constexpr size_t smem = sizeof(float) * (Q * G::SWP + G::RING * HBW) + (size_t)NRAW * TROWS * TSW;
+    static constexpr int TAIL = SW - NT;                // staged columns beyond the first NT
+    static constexpr size_t bytes = (size_t)NRAW * TROWS * TSW;
     static_assert(TAIL >= 0 && TAIL <= NT, "one extra expand pass covers the halo columns");
 };
 
+template <int R>
+struct Geo0 : Tile0<Geo<R>::SW> {
+    using G = Geo<R>;
+    // float staging buffer, ring, raw tiles
+    static constexpr size_t smem = sizeof(float) * (Q * G::SWP + G::RING * HBW) + Tile0<G::SW>::bytes;
+};
+
 __device__ __forceinline__ float s4_to_float(unsigned s4) { return unorm16_to_float((257u * s4 + 2u) >> 2); }
+
+// tile offsets of the two source columns of virtual column X; sx0 = source column of tile byte 0
+__device__ __forceinline__ void x2_cols(int X, int w, int sx0, int& o0, int& o1)
+{
+    o0 = clampi(X >> 1, 0, w - 1) - sx0;
+    o1 = clampi((X + 1) >> 1, 0, w - 1) - sx0;
+}
+
+// 4-byte cp.async of one tile: tile row r holds source row clamp(rbase + r); every thread issues its pieces
+template <class T0>
+__device__ __forceinline__ void x2_issue(const uint8_t* __restrict__ img, size_t img_pitch, int w, int h, uint8_t* Tk,
+                                         int sx0, int rbase)
+{
+#pragma unroll
+    for (int q = 0; q < T0::NP; ++q) {
+        const int e = threadIdx.x + q * NT;
+        const int r = e / (T0::TSW / 4);
+        const int c4 = 4 * (e - r * (T0::TSW / 4));
+        const int sc = sx0 + c4;
+        if (e < T0::PIECES && sc >= 0 && sc < w) {
+            const uint8_t* g = img + (size_t)clampi(rbase + r, 0, h - 1) * img_pitch + sc;
+            const unsigned sa = (unsigned)__cvta_generic_to_shared(Tk + r * T0::TSW + c4);
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" :: "r"(sa), "l"(g) : "memory");
+        }
+    }
+}
+
+// expand one virtual column of the chunk whose first row is iy (tile Tk, tile row 0 = source row iy >> 1): 16 staged samples
+// to out[j * SWP].  P is the parity of iy away from the border, which fixes the row pairing at compile time.
+template <class T0, int P, int SWP>
+__device__ __forceinline__ void x2_expand(const uint8_t* __restrict__ Tk, float* __restrict__ out, int iy, int o0, int o1,
+                                          int H, int h)
+{
+    if (iy >= 0 && iy + Q < H && (iy & 1) == P) {
+        unsigned hs[Q / 2 + 1];
+#pragma unroll
+        for (int r = 0; r < Q / 2 + 1; ++r) hs[r] = (unsigned)Tk[r * T0::TSW + o0] + (unsigned)Tk[r * T0::TSW + o1];
+#pragma unroll
+        for (int j = 0; j < Q; ++j) out[j * SWP] = s4_to_float(hs[(P + j) >> 1] + hs[(P + j + 1) >> 1]);
+    } else {
+        const int rbase = iy >> 1;
+        for (int j = 0; j < Q; ++j) {
+            const int vy = clampi(iy + j, 0, H - 1);
+            const int ra = clampi((vy >> 1) - rbase, 0, T0::TROWS - 1);
+            const int rb = clampi(min((vy + 1) >> 1, h - 1) - rbase, 0, T0::TROWS - 1);
+            const unsigned s4 = (unsigned)Tk[ra * T0::TSW + o0] + (unsigned)Tk[ra * T0::TSW + o1] +
+                                (unsigned)Tk[rb * T0::TSW + o0] + (unsigned)Tk[rb * T0::TSW + o1];
+            out[j * SWP] = s4_to_float(s4);
+        }
+    }
+}
 
 template <int R>
 __global__ void __launch_bounds__(NT, 6)
@@ -510,58 +585,17 @@ march_level0x2_kernel(const uint8_t* __restrict__ img, size_t img_pitch, int w, 
     uint8_t* T = reinterpret_cast<uint8_t*>(HB + G::RING * HBW);
     const int nchunks = (ye - ys + 2 * R + Q - 1) / Q;
     const int sx0 = ((x0 - G::RP) >> 1) & ~3;           // source column of tile byte 0 (may be negative)
+    auto tile = [&](int k) { return T + (k % G0::NRAW) * (G0::TROWS * G0::TSW); };
 
     // tile offsets of the two source columns of this thread's virtual columns (main + halo tail)
-    auto col_offsets = [&](int i, int& o0, int& o1) {
-        const int X = x0 - G::RP + i;
-        o0 = clampi(X >> 1, 0, w - 1) - sx0;
-        o1 = clampi((X + 1) >> 1, 0, w - 1) - sx0;
-    };
     int m0, m1, t0 = 0, t1 = 0;
-    col_offsets(threadIdx.x, m0, m1);
+    x2_cols(x0 - G::RP + threadIdx.x, w, sx0, m0, m1);
     const bool has_tail = threadIdx.x < G0::TAIL;
-    if (has_tail) col_offsets(NT + threadIdx.x, t0, t1);
+    if (has_tail) x2_cols(x0 - G::RP + NT + threadIdx.x, w, sx0, t0, t1);
 
-    auto issue = [&](int k) {
-        const int rbase = (ys - R + k * Q) >> 1;         // floor: tile row r holds source row clamp(rbase + r)
-        uint8_t* Tk = T + (k % G0::NRAW) * (G0::TROWS * G0::TSW);
-#pragma unroll
-        for (int q = 0; q < G0::NP; ++q) {
-            const int e = threadIdx.x + q * NT;
-            const int r = e / (G0::TSW / 4);
-            const int c4 = 4 * (e - r * (G0::TSW / 4));
-            const int sc = sx0 + c4;
-            if (e < G0::PIECES && sc >= 0 && sc < w) {
-                const uint8_t* g = img + (size_t)clampi(rbase + r, 0, h - 1) * img_pitch + sc;
-                const unsigned sa = (unsigned)__cvta_generic_to_shared(Tk + r * G0::TSW + c4);
-                asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" :: "r"(sa), "l"(g) : "memory");
-            }
-        }
-    };
-    // expand one virtual column of chunk k: 16 staged samples
-    auto expand = [&](int k, int i, int o0, int o1) {
-        const int iy = ys - R + k * Q;
-        const uint8_t* Tk = T + (k % G0::NRAW) * (G0::TROWS * G0::TSW);
-        float* out = S + i;
-        if (iy >= 0 && iy + Q < H && (iy & 1) == (R & 1)) {
-            constexpr int P = R & 1;
-            unsigned hs[Q / 2 + 1];
-#pragma unroll
-            for (int r = 0; r < Q / 2 + 1; ++r) hs[r] = (unsigned)Tk[r * G0::TSW + o0] + (unsigned)Tk[r * G0::TSW + o1];
-#pragma unroll
-            for (int j = 0; j < Q; ++j) out[j * G::SWP] = s4_to_float(hs[(P + j) >> 1] + hs[(P + j + 1) >> 1]);
-        } else {
-            const int rbase = iy >> 1;
-            for (int j = 0; j < Q; ++j) {
-                const int vy = clampi(iy + j, 0, H - 1);
-                const int ra = clampi((vy >> 1) - rbase, 0, G0::TROWS - 1);
-                const int rb = clampi(min((vy + 1) >> 1, h - 1) - rbase, 0, G0::TROWS - 1);
-                const unsigned s4 = (unsigned)Tk[ra * G0::TSW + o0] + (unsigned)Tk[ra * G0::TSW + o1] +
-                                    (unsigned)Tk[rb * G0::TSW + o0] + (unsigned)Tk[rb * G0::TSW + o1];
-                out[j * G::SWP] = s4_to_float(s4);
-            }
-        }
-    };
+    // the chunk's first row ys - R + kQ has the parity of R (ys is a multiple of Q)
+    auto issue = [&](int k) { x2_issue<G0>(img, img_pitch, w, h, tile(k), sx0, (ys - R + k * Q) >> 1); };
+    auto expand = [&](int k, int i, int o0, int o1) { x2_expand<G0, R & 1, G::SWP>(tile(k), S + i, ys - R + k * Q, o0, o1, H, h); };
 
 #pragma unroll
     for (int k = 0; k < G0::AHEAD; ++k) {
@@ -585,6 +619,159 @@ march_level0x2_kernel(const uint8_t* __restrict__ img, size_t img_pitch, int w, 
         if (slot_old >= G::RING) slot_old -= G::RING;
         col_pass<R, false>(HB, S, S, slot_old, ys - 2 * R + k * Q, ys, ye, x0, W, dst, nullptr, pitch, 0, inc0);
         slot_in = slot_old;
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+}
+
+// ---- octave 0, levels 0 and 1 in one launch (the default case above, level 1 with the same radius) --------------------
+//
+// Level 1 of octave 0 is the only consumer that reads all of G0, so the two levels are computed by the same CTA and G0
+// never comes back from HBM.  Per chunk of Q rows:
+//   stage A: the level-0 pipeline above (byte tiles, expand, row_pass with dd, column sums with inc0) for the strip's TW
+//            columns plus RP halo columns on each side.  The TW own columns are stored to G0 exactly as the level-0 kernel
+//            stores them; all TW + 2RP columns go to a staging buffer with the level kernels' layout (Geo<R>), where the
+//            rows and columns outside the plane are then clamped to the border of G0, as the TMA staging of the level
+//            kernel does (patch_halo for the columns, the border rows copied for the rows);
+//   stage B: the level kernel's row_pass and col_pass (no candidates: DoG[0] is not scanned) from that buffer to G1.
+// Stage B's chunk k reads G0 rows ys - R + kQ .. + Q - 1, which is what stage A's column sums of input chunk k produce
+// (rows ys + kQ ..): stage A runs one chunk ahead, starting at the input chunk ys - Q.  Every output sample is the
+// same instructions in the same order as in the two separate launches (the same row_pass, col_sum, x2_expand), so G0
+// and G1 are bit-identical to them.
+//
+// The CTA has NF = 160 threads, one per stage-A staged column: every stage-A phase (expand of 160 columns, row pass of
+// 9 x 16 column groups x rows, column sums of 72 pairs x 2 half-chunks) is one pass of at most one unit per thread.  With
+// the level kernels' 128 threads each of them would need a second pass on one or two warps, which the whole CTA then waits
+// for at the next barrier.  Stage B keeps the level kernel's 128-thread mapping; the fifth warp idles there.
+constexpr int NF = 160;
+
+template <int R>
+struct GeoF {
+    using G = Geo<R>;
+    static constexpr int CA = TW + 2 * G::RP;           // stage-A output columns = stage B's staged columns (x0 - RP ..)
+    static constexpr int SWA = CA + 2 * G::RP;          // stage-A staged virtual columns (x0 - 2RP ..)
+    static constexpr int SWPA = pad_odd4(SWA);          // stage-A staging row stride
+    static constexpr int HA = CA + ((4 - CA % 32) + 32) % 32;   // stage-A ring row stride (== 4 mod 32, like HBW)
+    using T0 = Tile0<SWA>;
+    // the stage-A staging buffer is dead once stage A's row pass has read it, and the stage-B staging buffer is written
+    // after that and read before the next expand: one buffer serves both
+    static constexpr int SBUF = (Q * SWPA > Q * G::SWP ? Q * SWPA : Q * G::SWP);
+    // staging, ring A, ring B, the last row of G0 (border rows below the plane), raw tiles
+    static constexpr size_t smem = sizeof(float) * (SBUF + G::RING * HA + G::RING * HBW + CA) + T0::bytes;
+    static_assert(CA == G::SW, "stage A produces exactly the level kernel's staged columns");
+    static_assert(SWA == NF, "one thread per staged column in the expand");
+    static_assert(CA % 16 == 0 && Q * (CA / 16) <= NF && CA <= NF, "one row-pass group and one column pair-half per thread");
+    // 4 resident CTAs per SM (the level kernels' residency, make_partition's default slots): 4 x (smem + 1 KB reserved
+    // per CTA) within the 228 KB of an H100 SM
+    static_assert(4 * (smem + 1024) <= 228 * 1024, "4 CTAs per SM");
+};
+
+// Stage A's column sums for one thread's column pair c, c+1 (stage-A output columns; c even): every row of the chunk to
+// the staging buffer Sb (layout Geo<R>), the strip's own columns of the rows in [ys, ye) also to G0.
+template <int R>
+__device__ __forceinline__ void col_pass_g0(const float* __restrict__ HA, float* __restrict__ Sb, int slot_oldest, int c,
+                                            int jbase, int y_first, int ys, int ye, int x0, int W, float* __restrict__ dst,
+                                            int pitch, const Taps& t)
+{
+    using G = Geo<R>;
+    f32x2 win[QH + 2 * R];
+    col_window<R, GeoF<R>::HA>(HA, slot_oldest, jbase, c, win);
+    const int x = x0 - G::RP + c;
+    const bool own = c >= G::RP && c < G::RP + TW && x < W;
+    float* pd = dst + (long long)(y_first + jbase) * pitch + x;   // dereferenced only for own columns inside the segment
+#pragma unroll
+    for (int jj = 0; jj < QH; ++jj) {
+        const f32x2 acc = col_sum<R>(win, jj, t);
+        const int j = jbase + jj;
+        *reinterpret_cast<f32x2*>(Sb + j * G::SWP + c) = acc;
+        if (own && y_first + j >= ys && y_first + j < ye) *reinterpret_cast<f32x2*>(pd) = acc;
+        pd += pitch;
+    }
+}
+
+template <int R>
+__global__ void __launch_bounds__(NF, 4)
+march_level01x2_kernel(const uint8_t* __restrict__ img, size_t img_pitch, int w, int h, float* __restrict__ g0,
+                       float* __restrict__ g1, int W, int H, int pitch, Partition part, Taps dd, Taps inc0, Taps inc1)
+{
+    using G = Geo<R>;
+    using F = GeoF<R>;
+    using T0 = typename F::T0;
+    extern __shared__ __align__(128) float smem[];
+    int strip, ys, ye;
+    if (!locate(part, blockIdx.x, H, Q, strip, ys, ye)) return;
+    const int x0 = strip * TW;
+    const bool edge = (x0 - G::RP < 0) || (x0 + TW + G::RP > W);
+    float* S = smem;                                     // stage-A staging (stride SWPA), then stage-B staging (stride SWP)
+    float* HA = S + F::SBUF;
+    float* HB = HA + G::RING * F::HA;
+    float* last = HB + G::RING * HBW;                    // G0 row H-1 (CA columns), once a chunk has produced it
+    uint8_t* T = reinterpret_cast<uint8_t*>(last + F::CA);
+    const int nchunks = (ye - ys + 2 * R + Q - 1) / Q;   // stage-B chunks; stage A runs nchunks + 1
+    const int sx0 = ((x0 - 2 * G::RP) >> 1) & ~3;       // source column of tile byte 0 (may be negative)
+    auto tile = [&](int kk) { return T + (kk % T0::NRAW) * (T0::TROWS * T0::TSW); };
+
+    const int tid = threadIdx.x;
+    const bool lvl = tid < NT;                           // a thread of the level kernels' 128-thread mappings
+    int m0, m1;
+    x2_cols(x0 - 2 * G::RP + tid, w, sx0, m0, m1);
+
+    // stage-A input chunk kk starts at row ys - Q + kk*Q: even, as ys is a multiple of Q.  The tile copies keep the
+    // 128-thread split of x2_issue.
+    auto issue = [&](int kk) { if (lvl) x2_issue<T0>(img, img_pitch, w, h, tile(kk), sx0, (ys - Q + kk * Q) >> 1); };
+
+    // stage-A column sums: pair p of the CA columns, half-chunk hc
+    const bool col_a = tid < F::CA;
+    const int pa = tid % (F::CA / 2), hc = tid / (F::CA / 2);
+
+#pragma unroll
+    for (int kk = 0; kk < T0::AHEAD; ++kk) {
+        issue(kk);
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    }
+    asm volatile("cp.async.wait_group %0;" :: "n"(T0::AHEAD - 1) : "memory");
+    __syncthreads();                                      // tile 0 visible
+    int slot_a = 0, slot_b = 0;
+    for (int kk = 0; kk <= nchunks; ++kk) {
+        // S was last read by stage B's row pass of the previous chunk (before the barrier ahead of its column pass)
+        x2_expand<T0, 0, F::SWPA>(tile(kk), S + tid, ys - Q + kk * Q, m0, m1, H, h);
+        if (kk + T0::AHEAD <= nchunks) issue(kk + T0::AHEAD);
+        asm volatile("cp.async.commit_group;" ::: "memory");
+        __syncthreads();                                  // chunk kk expanded; both column passes of kk-1 finished (rings free)
+        if (tid < Q * (F::CA / 16)) row_pass<R, true, F::SWPA, F::HA>(S, HA, slot_a, dd);
+        asm volatile("cp.async.wait_group %0;" :: "n"(T0::AHEAD - 1) : "memory");
+        __syncthreads();                                  // ring-A lines of chunk kk written; tile kk+1 visible
+        int old_a = slot_a + Q;
+        if (old_a >= G::RING) old_a -= G::RING;
+        slot_a = old_a;
+        if (kk == 0) continue;                            // warm-up: the ring holds no full window yet
+
+        const int k = kk - 1;                             // stage-B chunk
+        const int yb0 = ys - R + k * Q;                   // its first G0 row
+        if (col_a) col_pass_g0<R>(HA, S, old_a, 2 * pa, hc * QH, yb0, ys, ye, x0, W, g0, pitch, inc0);
+        __syncthreads();                                  // G0 rows of chunk k staged
+        if (yb0 < 0 || yb0 + Q >= H) {
+            // rows outside the plane take G0's border rows: row 0 is in this chunk whenever a row above the plane is (only
+            // the first chunk of the top segment has any), row H-1 is in this chunk or was kept from an earlier one
+            const int jl = H - 1 - yb0;                   // chunk row of G0 row H-1 (negative: an earlier chunk)
+            for (int e = tid; e < Q * F::CA; e += NF) {
+                const int j = e / F::CA, c = e - j * F::CA;
+                const int y = yb0 + j;
+                if (y < 0) S[j * G::SWP + c] = S[-yb0 * G::SWP + c];
+                else if (y >= H) S[j * G::SWP + c] = jl >= 0 ? S[jl * G::SWP + c] : last[c];
+                else if (y == H - 1) last[c] = S[j * G::SWP + c];
+            }
+            __syncthreads();
+        }
+        if (edge) {
+            if (lvl) patch_halo<R>(S, x0, W);
+            __syncthreads();
+        }
+        if (lvl) row_pass<R, false>(S, HB, slot_b, inc1);
+        __syncthreads();                                  // ring-B lines of chunk k written
+        int old_b = slot_b + Q;
+        if (old_b >= G::RING) old_b -= G::RING;
+        if (lvl) col_pass<R, false>(HB, S, S, old_b, ys - 2 * R + k * Q, ys, ye, x0, W, g1, nullptr, pitch, 0, inc1);
+        slot_b = old_b;
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
@@ -652,14 +839,19 @@ int run_march(const OctaveView& o, int level, const Taps& t, float* next0, int n
                 : launch_march<R, false, false>(part, src, dst, next0, o, next_pitch, t, cs, st);
 }
 
+// the exact-2x byte-tile path of level 0 applies (see march_level0x2_kernel)
+bool x2_geometry(const uint8_t* img, size_t img_pitch, int w, int h, float shift, const OctaveView& o0, int plan)
+{
+    return plan == LEVEL0_IDEAL_X2 && shift == 1.0f && o0.w == 2 * w && o0.h == 2 * h && (img_pitch & 3) == 0 &&
+           (reinterpret_cast<uintptr_t>(img) & 3) == 0;
+}
+
 template <int R, typename PIX>
 int run_march0(const PIX* img, size_t img_pitch, int w, int h, float shift, const OctaveView& o0, const Taps& dd,
                const Taps& inc0, int plan, cudaStream_t st)
 {
     if constexpr (sizeof(PIX) == 1) {
-        const bool x2 = plan == LEVEL0_IDEAL_X2 && shift == 1.0f && o0.w == 2 * w && o0.h == 2 * h && (img_pitch & 3) == 0 &&
-                        (reinterpret_cast<uintptr_t>(img) & 3) == 0;
-        if (x2) {
+        if (x2_geometry(img, img_pitch, w, h, shift, o0, plan)) {
             const Partition part = make_partition(o0.w, o0.h, level0_slots());
             ensure_smem(march_level0x2_kernel<R>, Geo0<R>::smem, true);
             march_level0x2_kernel<R><<<part.B, NT, Geo0<R>::smem, st>>>(img, img_pitch, w, h, o0.gauss, o0.w, o0.h, o0.pitch,
@@ -708,6 +900,17 @@ int march_level0_u8(const uint8_t* img, size_t img_pitch, int w, int h, float sh
 #undef PSB_CASE
         default: return -1;
     }
+}
+
+int march_level01_u8(const uint8_t* img, size_t img_pitch, int w, int h, float shift, const OctaveView& o0,
+                     const Taps& dd, const Taps& inc0, int R0, const Taps& t1, int R1, int plan, cudaStream_t st)
+{
+    if (R0 != 5 || R1 != 5 || !x2_geometry(img, img_pitch, w, h, shift, o0, plan)) return 0;
+    const Partition part = make_partition(o0.w, o0.h);
+    ensure_smem(march_level01x2_kernel<5>, GeoF<5>::smem, true);
+    march_level01x2_kernel<5><<<part.B, NF, GeoF<5>::smem, st>>>(img, img_pitch, w, h, o0.gauss, o0.gauss + o0.plane, o0.w, o0.h,
+                                                                 o0.pitch, part, dd, inc0, t1);
+    return 1;
 }
 
 int march_level0_f32(const float* img, size_t img_pitch, int w, int h, float shift, const OctaveView& o0,

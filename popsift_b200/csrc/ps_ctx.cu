@@ -107,6 +107,7 @@ struct ps_ctx {
     int max_octaves = 0;
     int levels = 3;
     bool timing = false;
+    bool fuse_l0 = true;             // levels 0 and 1 of octave 0 in one launch where possible (POPSIFT_B200_FUSE_L0=0: two)
     bool graph_broken = false;       // a stream capture failed once: direct launches from then on
     std::vector<Slot> slots;
     std::atomic<int64_t> launches{0};
@@ -286,6 +287,7 @@ int run_pyramid(ps_ctx* ctx, Slot& s)
     // --gauss-mode vlfeat-direct (VLFeat_Relative_All, s_pyramid_build.cu:543-546; under ScaleDirect the direct-scaling
     // arm comes first, :499): every level of octave 0 straight from the input image
     const bool abs_o0 = ctx->cfg.gauss_mode == PS_GAUSS_VLFEAT_RELATIVE_ALL && !direct;
+    bool fused01 = false;           // level 1 of octave 0 came with level 0
     bool collects = L <= kMaxLevels && !abs_o0;
     for (int l = 2; l <= L + 1 && collects; ++l) collects = blur_level_collects(ctx->rows[l]);
     for (int o = 0; o < s.num_octaves && collects; ++o) collects = s.view.oct[o].w <= 65535 && s.view.oct[o].h <= 65535;
@@ -303,7 +305,14 @@ int run_pyramid(ps_ctx* ctx, Slot& s)
         }
         if (s.num_octaves > 1) n += launch_decimate(s.view.oct[0], L, s.view.oct[1], s.stream);
     } else {
-    if (s.is_float)
+    // 8-bit input up-scaled exactly 2x: level 1 of octave 0 in the same launch as level 0, so that G0 is written once and
+    // never read back (not under direct scaling, and not when level 1 also writes the next octave, L == 1)
+    if (ctx->fuse_l0 && !s.is_float && !direct && L >= 2)
+        fused01 = launch_level01_u8(s.d_img, u8_pitch(s.w), s.w, s.h, ctx->cfg.upscale, ctx->cfg.sift_mode, s.view.oct[0],
+                                    ctx->dd0, ctx->rows[0], ctx->rows[1], s.stream) > 0;
+    if (fused01)
+        r = 1;
+    else if (s.is_float)
         r = launch_level0_f32(reinterpret_cast<const float*>(s.d_img), (size_t)s.w, s.w, s.h, ctx->cfg.upscale,
                               ctx->cfg.sift_mode, s.view.oct[0], ctx->dd0, ctx->rows[0], s.stream);
     else
@@ -325,7 +334,7 @@ int run_pyramid(ps_ctx* ctx, Slot& s)
             if (r < 0) return ctx->fail(PS_ERR_ARG, "unsupported level-0 filter span %d (octave %d)", ctx->dd[o].span, o);
             n += r;
         }
-        for (int l = 1; l < L + 3 && !(abs_o0 && o == 0); ++l) {
+        for (int l = (o == 0 && fused01) ? 2 : 1; l < L + 3 && !(abs_o0 && o == 0); ++l) {
             // Config::ScaleDirect (s_pyramid_build.cu:499-514): level 0 of EVERY octave comes straight from the input image
             // (rows: the dd table of the octave, columns: the level-0 table), nothing is decimated from the octave above
             const OctaveView* next = (l == L && !last && !direct) ? &s.view.oct[o + 1] : nullptr;
@@ -619,6 +628,7 @@ extern "C" ps_ctx* ps_create(int device, const ps_config* cfg, int max_w, int ma
         ctx->absn[l].span = ctx->tab.absn_span[l];
     }
     ctx->max_w = max_w; ctx->max_h = max_h;
+    if (const char* e = getenv("POPSIFT_B200_FUSE_L0")) ctx->fuse_l0 = e[0] != '0';
     int32_t W[kMaxOctaves], H[kMaxOctaves];
     ctx->max_octaves = ps_geometry(&ctx->cfg, max_w, max_h, W, H);
     if (ctx->max_octaves < 1) { delete ctx; return bail("ps_create: bad geometry", cudaSuccess); }

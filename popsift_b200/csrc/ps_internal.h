@@ -127,6 +127,10 @@ int level0_plan_for(int w, int h, int W, int H, float shift, int R);   // k_pyra
 // (octave > 0: Config::ScaleDirect, the same pass onto a smaller octave with that octave's dd row and shift 0.5)
 int launch_level0_u8(const uint8_t* img, size_t img_pitch, int w, int h, float upscale, int sift_mode,
                      const OctaveView& o0, const GaussRow& dd, const GaussRow& inc0, cudaStream_t st, int octave = 0);
+// levels 0 and 1 of octave 0 in one launch where the fused kernel applies (8-bit input up-scaled exactly 2x, both radii 5,
+// marching kernels); 0 (nothing launched) anywhere else
+int launch_level01_u8(const uint8_t* img, size_t img_pitch, int w, int h, float upscale, int sift_mode,
+                      const OctaveView& o0, const GaussRow& dd, const GaussRow& inc0, const GaussRow& g1, cudaStream_t st);
 int launch_level0_f32(const float* img, size_t img_pitch_floats, int w, int h, float upscale, int sift_mode,
                       const OctaveView& o0, const GaussRow& dd, const GaussRow& inc0, cudaStream_t st, int octave = 0);
 // --gauss-mode vlfeat-direct (VLFeat_Relative_All): one level of octave 0 straight from the input image; the next

@@ -43,7 +43,7 @@ def group(name: str):
     m = re.search(r"march_level_kernel<(\d+), (\w+), (\w+)>", name)
     if m:
         return "pyramid", "march_level_kernel R=%s next=%s cand=%s" % m.groups()
-    m = re.search(r"(march_level0x2_kernel|march_level0_kernel|level0_kernel|level0_generic_kernel)<([^>]*)>", name)
+    m = re.search(r"(march_level01x2_kernel|march_level0x2_kernel|march_level0_kernel|level0_kernel|level0_generic_kernel)<([^>]*)>", name)
     if m:
         return "pyramid", "level0 %s<%s>" % (m.group(1), m.group(2))
     m = re.search(r"(cand_extrema_kernel|find_extrema_kernel)<([^>]*)>", name)
