@@ -317,4 +317,72 @@ std::pair<std::vector<Rigid>, BundleReport> bundleAdjust(const std::vector<Featu
                                                          const std::vector<bool>& fixed, TrackPoints& points,
                                                          const BundleParams& params = BundleParams());
 
+/// Settings of rotationAveraging (same fields and rules as ps_rotation_params in popsift_b200_global.h).
+struct RotationParams
+{
+    int    loss = BundleParams::Cauchy;
+    double loss_scale = 5.0;         // degrees
+    int    max_iters = 100;          // IRLS iterations, 0 .. 10000
+    double step_tol = 1e-4;          // degrees: the largest update that stops
+    int    cg_max_iters = 100;       // 1 .. 10000
+    double cg_tol = 1e-8;            // [0, 1)
+    int    min_inliers = 15;         // a pair is used when its n_front reaches this
+};
+
+/// What rotationAveraging did (ps_rotation_report); termination is PS_RA_MAX_ITERS .. PS_RA_NO_PAIRS.
+struct RotationReport
+{
+    double initial_cost = 0, final_cost = 0;
+    int    iterations = 0, cg_iterations = 0, n_pairs = 0, n_registered = 0, termination = 0;
+};
+
+/// One world-to-camera rotation per set, registered flags and per-pair errors (degrees, +inf for pairs not used).
+struct Rotations
+{
+    std::vector<Rigid>  R;               // t is zero
+    std::vector<bool>   registered;
+    std::vector<float>  pair_error;
+    RotationReport      report;
+};
+
+/// Rotation averaging on device 0 (an addition to the reference's interface; C ABI ps_rotation_averaging): `poses` is
+/// what relativePoses gave for `pairs` (its R and n_front are uploaded).  Throws when poses.size() != pairs.size(), and
+/// for the arguments ps_rotation_averaging refuses.
+Rotations rotationAveraging(int n_sets, const std::vector<std::pair<int, int>>& pairs, const std::vector<TwoViewPose>& poses,
+                            const RotationParams& params = RotationParams());
+
+/// Settings of globalPositioning (same fields and rules as ps_position_params).
+struct PositionParams
+{
+    int    loss = BundleParams::Huber;
+    double loss_scale = 0.1;
+    int    max_iters = 100;
+    double function_tol = 1e-8;
+    int    cg_max_iters = 300;
+    double cg_tol = 1e-8;
+};
+
+/// What globalPositioning did (ps_position_report); termination is PS_GP_MAX_ITERS .. PS_GP_NO_OBSERVATIONS.
+struct PositionReport
+{
+    double initial_cost = 0, final_cost = 0;
+    int    iterations = 0, cg_iterations = 0, n_obs = 0, n_points = 0, n_cams = 0, termination = 0;
+};
+
+/// Camera poses (world to camera) and one point per track (0 for tracks that took no part).
+struct Positions
+{
+    std::vector<Rigid>   poses;
+    std::vector<bool>    positioned;
+    std::vector<double>  X;              // 3 per track
+    PositionReport       report;
+};
+
+/// Global positioning of camera centres and track points with rotations held (an addition to the reference's interface;
+/// C ABI ps_global_positioning): `tracks` as for triangulateTracks, `rotations` and `registered` what rotationAveraging
+/// gave (only R of each Rigid is read).  Throws like triangulateTracks, and for the arguments ps_global_positioning refuses.
+Positions globalPositioning(const std::vector<FeaturesDev*>& sets, const Tracks& tracks, const std::vector<Camera>& cameras,
+                            const std::vector<Rigid>& rotations, const std::vector<bool>& registered,
+                            const PositionParams& params = PositionParams());
+
 } // namespace popsift

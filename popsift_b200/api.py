@@ -135,6 +135,36 @@ BA_LOSS = ("squared", "huber", "cauchy")
 BA_TERMINATION = ("max_iters", "function_tol", "lambda", "no_observations", "nonfinite_start")
 assert C.sizeof(PsBundleParams) == 56 and C.sizeof(PsBundleReport) == 48
 
+
+class PsRotationParams(C.Structure):
+    """ps_rotation_params (40 bytes)"""
+    _fields_ = [("loss", C.c_int32), ("max_iters", C.c_int32), ("cg_max_iters", C.c_int32), ("min_inliers", C.c_int32),
+                ("loss_scale", C.c_double), ("step_tol", C.c_double), ("cg_tol", C.c_double)]
+
+
+class PsRotationReport(C.Structure):
+    """ps_rotation_report (40 bytes)"""
+    _fields_ = [("initial_cost", C.c_double), ("final_cost", C.c_double), ("iterations", C.c_int32), ("cg_iterations", C.c_int32),
+                ("n_pairs", C.c_int32), ("n_registered", C.c_int32), ("termination", C.c_int32), ("pad_", C.c_int32)]
+
+
+class PsPositionParams(C.Structure):
+    """ps_position_params (40 bytes)"""
+    _fields_ = [("loss", C.c_int32), ("max_iters", C.c_int32), ("cg_max_iters", C.c_int32), ("pad_", C.c_int32),
+                ("loss_scale", C.c_double), ("function_tol", C.c_double), ("cg_tol", C.c_double)]
+
+
+class PsPositionReport(C.Structure):
+    """ps_position_report (40 bytes)"""
+    _fields_ = [("initial_cost", C.c_double), ("final_cost", C.c_double), ("iterations", C.c_int32), ("cg_iterations", C.c_int32),
+                ("n_obs", C.c_int32), ("n_points", C.c_int32), ("n_cams", C.c_int32), ("termination", C.c_int32)]
+
+
+RA_TERMINATION = ("max_iters", "step_tol", "no_pairs")
+GP_TERMINATION = ("max_iters", "function_tol", "no_observations")
+assert C.sizeof(PsRotationParams) == 40 and C.sizeof(PsRotationReport) == 40
+assert C.sizeof(PsPositionParams) == 40 and C.sizeof(PsPositionReport) == 40
+
 EXPORTS = ["ps_abi_version", "ps_config_default", "ps_gauss_tables_compute", "ps_geometry", "ps_create", "ps_destroy",
            "ps_last_error", "ps_submit_u8", "ps_submit_f32", "ps_submit_dev_u8", "ps_counts", "ps_download",
            "ps_sync", "ps_debug_plane", "ps_debug_extrema", "ps_slot_geometry", "ps_set_timing", "ps_stage_ms",
@@ -154,6 +184,8 @@ POSE_EXPORTS = ["ps_relative_pose_batch"]
 TRIANGULATE_EXPORTS = ["ps_triangulate_tracks"]
 # bundle adjustment, declared in popsift_b200_bundle.h (same library)
 BUNDLE_EXPORTS = ["ps_bundle_adjust"]
+# global poses, declared in popsift_b200_global.h (same library)
+GLOBAL_EXPORTS = ["ps_rotation_averaging", "ps_global_positioning"]
 
 _lib = None
 
@@ -222,6 +254,12 @@ def load_library():
         L.ps_bundle_adjust.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                        C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsBundleParams), C.c_void_p, C.c_void_p,
                                        C.POINTER(PsBundleReport)]
+    if hasattr(L, "ps_rotation_averaging"):
+        L.ps_rotation_averaging.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(PsRotationParams), C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.POINTER(PsRotationReport)]
+        L.ps_global_positioning.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                            C.c_void_p, C.c_void_p, C.c_int, C.POINTER(PsPositionParams), C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.POINTER(PsPositionReport)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -1219,6 +1257,172 @@ def bundle_adjust(sets, tracks, points, cameras, poses, fixed, loss="squared", l
     tp = TrackPoints(out["X"].copy(), out["error"].copy(), out["angle"].copy(), out["n_inliers"].copy(), out["status"].copy(),
                      np.asarray(points.mask, np.uint8).copy(), err, dict(points.counts) if points.counts is not None else None)
     return new_poses, tp, _bundle_report(rep)
+
+
+RotationReport = namedtuple("RotationReport", "initial_cost final_cost iterations cg_iterations n_pairs n_registered termination")
+RotationReport.__doc__ = """ps_rotation_report of ps_rotation_averaging (popsift_b200_global.h); termination is a name of
+RA_TERMINATION."""
+PositionReport = namedtuple("PositionReport", "initial_cost final_cost iterations cg_iterations n_obs n_points n_cams termination")
+PositionReport.__doc__ = """ps_position_report of ps_global_positioning (popsift_b200_global.h); termination is a name of
+GP_TERMINATION."""
+GlobalPoses = namedtuple("GlobalPoses", "tracks poses registered positioned rotation_report position_report pair_error")
+GlobalPoses.__doc__ = """global_poses' result: the Tracks of the pairs kept, one world-to-camera (R, t) per set, the bool
+registered (rotation averaging) and positioned (global positioning) flags per set, both reports and the pairs' final
+rotation errors in degrees (+inf for pairs not used)."""
+
+
+def _loss_code(loss) -> int:
+    if loss not in BA_LOSS:
+        raise PopSiftError("loss must be one of %s" % (BA_LOSS,))
+    return BA_LOSS.index(loss)
+
+
+def _rotation_params(loss="cauchy", loss_scale=5.0, max_iters=100, step_tol=1e-4, cg_max_iters=100, cg_tol=1e-8,
+                     min_inliers=15) -> PsRotationParams:
+    return PsRotationParams(_loss_code(loss), int(max_iters), int(cg_max_iters), int(min_inliers), float(loss_scale), float(step_tol),
+                            float(cg_tol))
+
+
+def _position_params(loss="huber", loss_scale=0.1, max_iters=100, function_tol=1e-8, cg_max_iters=300, cg_tol=1e-8) -> PsPositionParams:
+    return PsPositionParams(_loss_code(loss), int(max_iters), int(cg_max_iters), 0, float(loss_scale), float(function_tol), float(cg_tol))
+
+
+def _rotation_dev(lib, device, n_sets, pairs, d_two_view, prm: PsRotationParams):
+    """ps_rotation_averaging on device two-view records: (R (S, 3, 3), registered bool (S,), pair_error (P,), RotationReport)"""
+    n, P = max(int(n_sets), 1), len(pairs)
+    R = np.zeros((n, 9), np.float64)
+    reg = np.zeros(n, np.uint8)
+    err = np.zeros(max(P, 1), np.float32)
+    rep = PsRotationReport()
+    rc = lib.ps_rotation_averaging(device, int(n_sets), P, _c_pairs(pairs), d_two_view if P else None, C.byref(prm), R.ctypes.data,
+                                   reg.ctypes.data, err.ctypes.data, C.byref(rep))
+    _check(lib, rc, "ps_rotation_averaging")
+    out = RotationReport(float(rep.initial_cost), float(rep.final_cost), int(rep.iterations), int(rep.cg_iterations), int(rep.n_pairs),
+                         int(rep.n_registered), RA_TERMINATION[rep.termination])
+    return R[:n_sets].reshape(-1, 3, 3), reg[:n_sets].astype(bool), err[:P].copy(), out
+
+
+def rotation_averaging(n_sets, pairs, two_view, device=0, **params):
+    """Robust rotation averaging over a view graph (C ABI ps_rotation_averaging in popsift_b200_global.h; an addition to the
+    reference's interface): a maximum-spanning-tree start, then IRLS on the device.  `pairs` is the (l, r) list and
+    `two_view` one relative pose per pair (X_r = R X_l + t) as TwoView tuples, ps_two_view records (TWO_VIEW_DTYPE) or
+    (R, n_front) tuples.  params: loss ("cauchy"), loss_scale (degrees, 5.0), max_iters (100), step_tol (degrees, 1e-4),
+    cg_max_iters (100), cg_tol (1e-8), min_inliers (n_front threshold, 15).  Returns (R (n_sets, 3, 3) world to camera,
+    registered bool (n_sets,), pair_error degrees (P,), RotationReport)."""
+    lib = load_library()
+    prm = _rotation_params(**params)
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    if isinstance(two_view, np.ndarray) and two_view.dtype == TWO_VIEW_DTYPE:
+        rec = np.ascontiguousarray(two_view)
+    else:
+        rec = np.zeros(len(two_view), TWO_VIEW_DTYPE)
+        for p, tv in enumerate(two_view):
+            if isinstance(tv, TwoView):
+                rec[p]["R"], rec[p]["t"], rec[p]["n_inliers"], rec[p]["n_front"] = tv.R, tv.t, tv.n_inliers, tv.n_front
+            else:
+                rec[p]["R"], rec[p]["n_front"] = np.asarray(tv[0], np.float32).reshape(3, 3), int(tv[1])
+    if len(rec) != len(pairs):
+        raise PopSiftError("one two-view record per pair expected")
+    bufs = _DevBuffers(lib)
+    try:
+        return _rotation_dev(lib, device, n_sets, pairs, bufs.upload(rec) if len(rec) else None, prm)
+    finally:
+        bufs.free()
+
+
+def _positioning_dev(lib, bufs, device, n_feat, c_feat, cameras, R, registered, n_tracks, d_start, d_mem, n_members, prm):
+    """ps_global_positioning on device track arrays: (poses [(R, t)], positioned bool (S,), X (T, 3), PositionReport)"""
+    cam = _c_cameras(cameras)
+    S = len(n_feat)
+    Rs = np.ascontiguousarray(np.asarray(R, np.float64).reshape(-1, 9))
+    reg = np.ascontiguousarray(np.asarray(registered).astype(np.uint8).reshape(-1))
+    if len(cam) != S or len(Rs) != S or len(reg) != S:
+        raise PopSiftError("one camera, one rotation and one registered flag per set expected")
+    n = max(S, 1)
+    out = (PsRigid * n)()
+    pos = np.zeros(n, np.uint8)
+    d_X = bufs.alloc(n_tracks * 24) if n_tracks else None
+    rep = PsPositionReport()
+    rc = lib.ps_global_positioning(device, S, (C.c_int32 * n)(*n_feat), c_feat, cam.ctypes.data, Rs.ctypes.data if S else None,
+                                   reg.ctypes.data if S else None, n_tracks, d_start, d_mem, n_members, C.byref(prm), out,
+                                   pos.ctypes.data, d_X, C.byref(rep))
+    _check(lib, rc, "ps_global_positioning")
+    X = bufs.download(d_X, (n_tracks, 3), np.float64) if n_tracks else np.zeros((0, 3))
+    poses = [(np.array(out[i].R[:], np.float64).reshape(3, 3), np.array(out[i].t[:], np.float64)) for i in range(S)]
+    r = PositionReport(float(rep.initial_cost), float(rep.final_cost), int(rep.iterations), int(rep.cg_iterations), int(rep.n_obs),
+                       int(rep.n_points), int(rep.n_cams), GP_TERMINATION[rep.termination])
+    return poses, pos[:S].astype(bool), X, r
+
+
+def global_positioning(sets, tracks, cameras, rotations, registered, device=None, **params):
+    """Global positioning of camera centres and track points from the tracks' viewing rays, rotations held (C ABI
+    ps_global_positioning in popsift_b200_global.h; an addition to the reference's interface).  `sets` are FeaturesDev
+    objects or host Features, `tracks` a Tracks over them, `cameras` one (fx, fy, cx, cy) per set, `rotations` one
+    world-to-camera R per set and `registered` one bool per set (rotation_averaging's).  params: loss ("huber"),
+    loss_scale (0.1), max_iters (100), function_tol (1e-8), cg_max_iters (300), cg_tol (1e-8).  Returns (poses as a list of
+    (R, t), positioned bool (n_sets,), X (T, 3) points (0 for tracks that took no part), PositionReport); the positioned
+    centres have an RMS distance of 1 from the root's."""
+    lib = load_library()
+    prm = _position_params(**params)
+    bufs = _DevBuffers(lib)
+    try:
+        ptrs, n_feat = [], []
+        for s in sets:
+            if isinstance(s, FeaturesDev):
+                ptrs.append(s.getFeatures()); n_feat.append(s.getFeatureCount())
+            else:
+                f = np.ascontiguousarray(s.feat if isinstance(s, Features) else s, FEATURE_DTYPE)
+                ptrs.append(bufs.upload(f)); n_feat.append(len(f))
+        if device is None:
+            device = next((max(0, lib.ps_pointer_device(p)) for p, k in zip(ptrs, n_feat) if k > 0), 0)
+        off = np.concatenate([[0], np.cumsum(n_feat, dtype=np.int64)])
+        st = np.ascontiguousarray(tracks.start, np.int32)
+        mem = (off[np.asarray(tracks.set, np.int64)] + np.asarray(tracks.feature, np.int64)).astype(np.int32)
+        c_feat = (C.c_void_p * max(len(sets), 1))(*ptrs)
+        return _positioning_dev(lib, bufs, device, n_feat, c_feat, cameras, rotations, registered, len(st) - 1, bufs.upload(st),
+                                bufs.upload(mem) if len(mem) else None, len(mem), prm)
+    finally:
+        bufs.free()
+
+
+def global_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=None, min_length=2, max_pair_error=5.0, pose=None,
+                 rotation=None, position=None) -> GlobalPoses:
+    """Poses for every image from images and intrinsics alone, without leaving the device: relative_poses' chain
+    (matching unless `matches` is given, correspondences, ps_relative_pose_batch with the parameters in the dict `pose`),
+    ps_rotation_averaging on its records (dict `rotation`: rotation_averaging's params), ps_tracks_from_matches on the
+    pose masks of the pairs that were used, are registered and have a final rotation error <= max_pair_error degrees
+    (the other pairs contribute no correspondence), then ps_global_positioning on those tracks (dict `position`:
+    global_positioning's params).  `sets` are FeaturesDev objects and `cameras` one (fx, fy, cx, cy) per set.  The
+    result feeds triangulate() and then bundle_adjust()."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    pprm = _pose_params(**(pose or {}))
+    rprm = _rotation_params(**(rotation or {}))
+    gprm = _position_params(**(position or {}))
+    cam = np.asarray(cameras, np.float32).reshape(-1, 4)
+    if len(cam) != len(sets):
+        raise PopSiftError("one camera per set expected")
+    bufs = _DevBuffers(lib)
+    try:
+        _, device, rows, d_match, d_corr, d_src, start, n_corr = _matched_rows(lib, bufs, sets, pairs, matches, flags, u8, device,
+                                                                              u8 and matches is None)
+        d_out, d_mask = _pose_dev(lib, bufs, device, d_corr, start, n_corr, _c_cameras([cam[i] for lr in pairs for i in lr]), pprm)[:2]
+        R, reg, perr, rrep = _rotation_dev(lib, device, len(sets), pairs, d_out, rprm)
+        keep = np.ascontiguousarray(np.where(perr <= float(max_pair_error), n_corr, 0), np.int32)
+        n = max(len(sets), 1)
+        n_feat = [s.getFeatureCount() for s in sets]
+        c_nf = (C.c_int32 * n)(*n_feat)
+        c_rev = (C.c_void_p * n)(*[s.getReverseMap() for s in sets])
+        c_nd = (C.c_int32 * n)(*[s.getDescriptorCount() for s in sets])
+        tr, d_start, d_mem = _tracks_run(lib, bufs, n_feat, min_length, lambda of, st, mem, cnt: lib.ps_tracks_from_matches(
+            device, len(sets), c_nf, c_rev, c_nd, len(pairs), _c_pairs(pairs), d_match, d_src, keep.ctypes.data, d_mask,
+            int(min_length), of, st, mem, C.byref(cnt)))
+        c_feat = (C.c_void_p * n)(*[s.getFeatures() for s in sets])
+        poses, positioned, _, grep = _positioning_dev(lib, bufs, device, n_feat, c_feat, cam, R, reg, len(tr.start) - 1, d_start,
+                                                      d_mem, len(tr.set), gprm)
+    finally:
+        bufs.free()
+    return GlobalPoses(tr, poses, reg, positioned, rrep, grep, perr)
 
 
 def _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, model, threshold, flags, u8) -> int:

@@ -10,6 +10,7 @@
 #include "popsift_b200_tracks.h"
 #include "popsift_b200_triangulate.h"
 #include "popsift_b200_bundle.h"
+#include "popsift_b200_global.h"
 
 #include <algorithm>
 #include <cmath>
@@ -709,6 +710,127 @@ std::pair<std::vector<Rigid>, BundleReport> bundleAdjust(const std::vector<Featu
     R.n_points = r.n_points;
     R.n_free_cams = r.n_free_cams;
     return res;
+}
+
+Rotations rotationAveraging(int n_sets, const std::vector<std::pair<int, int>>& pairs, const std::vector<TwoViewPose>& poses,
+                            const RotationParams& params)
+{
+    const std::string who = "popsift::rotationAveraging";
+    if (n_sets < 0) throw std::runtime_error(who + ": n_sets < 0");
+    if (poses.size() != pairs.size()) throw std::runtime_error(who + ": one relative pose per pair expected");
+    const size_t np = pairs.size();
+    std::vector<ps_two_view> rec(np);
+    std::vector<int32_t> flat(2 * np);
+    for (size_t p = 0; p < np; ++p) {
+        rec[p] = ps_two_view{};
+        std::copy(poses[p].R, poses[p].R + 9, rec[p].R);
+        std::copy(poses[p].t, poses[p].t + 3, rec[p].t);
+        rec[p].n_inliers = poses[p].n_inliers;
+        rec[p].n_front = poses[p].n_front;
+        flat[2 * p] = pairs[p].first;
+        flat[2 * p + 1] = pairs[p].second;
+    }
+    DevBuf d(std::max<size_t>(np, 1) * sizeof(ps_two_view), who);
+    if (np) check(ps_host_to_dev(d.p, rec.data(), np * sizeof(ps_two_view)), who);
+    ps_rotation_params prm{};
+    prm.loss = params.loss;
+    prm.max_iters = params.max_iters;
+    prm.cg_max_iters = params.cg_max_iters;
+    prm.min_inliers = params.min_inliers;
+    prm.loss_scale = params.loss_scale;
+    prm.step_tol = params.step_tol;
+    prm.cg_tol = params.cg_tol;
+    std::vector<double> R(9 * (size_t)std::max(n_sets, 1));
+    std::vector<uint8_t> reg(std::max(n_sets, 1));
+    Rotations out;
+    out.pair_error.resize(np);
+    ps_rotation_report r;
+    check(ps_rotation_averaging(0, n_sets, (int)np, flat.data(), static_cast<const ps_two_view*>(d.p), &prm, R.data(), reg.data(),
+                                out.pair_error.data(), &r),
+          who, "ps_rotation_averaging");
+    out.R.resize(n_sets);
+    out.registered.resize(n_sets);
+    for (int i = 0; i < n_sets; ++i) {
+        std::copy(&R[9 * (size_t)i], &R[9 * (size_t)i] + 9, out.R[i].R);
+        out.registered[i] = reg[i] != 0;
+    }
+    RotationReport& o = out.report;
+    o.initial_cost = r.initial_cost;
+    o.final_cost = r.final_cost;
+    o.iterations = r.iterations;
+    o.cg_iterations = r.cg_iterations;
+    o.n_pairs = r.n_pairs;
+    o.n_registered = r.n_registered;
+    o.termination = r.termination;
+    return out;
+}
+
+Positions globalPositioning(const std::vector<FeaturesDev*>& sets, const Tracks& tracks, const std::vector<Camera>& cameras,
+                            const std::vector<Rigid>& rotations, const std::vector<bool>& registered, const PositionParams& params)
+{
+    const Batch b("globalPositioning", sets, {});
+    if (cameras.size() != sets.size()) throw std::runtime_error(b.who + ": one camera per set expected");
+    if (rotations.size() != sets.size() || registered.size() != sets.size())
+        throw std::runtime_error(b.who + ": one rotation and one registered flag per set expected");
+    if (tracks.start.empty() || tracks.set.size() != tracks.feature.size() || (size_t)tracks.start.back() != tracks.set.size())
+        throw std::runtime_error(b.who + ": malformed tracks");
+    std::vector<int32_t> n_feat(sets.size());
+    std::vector<int64_t> off(sets.size() + 1, 0);
+    for (size_t i = 0; i < sets.size(); ++i) {
+        n_feat[i] = sets[i]->getFeatureCount();
+        off[i + 1] = off[i] + std::max(n_feat[i], 0);
+    }
+    const size_t nt = tracks.start.size() - 1, nm = tracks.set.size();
+    std::vector<int32_t> mem(nm);
+    for (size_t k = 0; k < nm; ++k) {
+        const int s = tracks.set[k], f = tracks.feature[k];
+        if (s < 0 || (size_t)s >= sets.size() || f < 0 || f >= n_feat[s]) throw std::runtime_error(b.who + ": track member out of range");
+        mem[k] = (int32_t)(off[s] + f);
+    }
+    std::vector<ps_camera> cams(sets.size());
+    std::vector<double> R(9 * std::max<size_t>(sets.size(), 1));
+    std::vector<uint8_t> reg(std::max<size_t>(sets.size(), 1)), pos(std::max<size_t>(sets.size(), 1));
+    std::vector<ps_rigid> rig(std::max<size_t>(sets.size(), 1));
+    for (size_t i = 0; i < sets.size(); ++i) {
+        cams[i] = ps_camera{cameras[i].fx, cameras[i].fy, cameras[i].cx, cameras[i].cy};
+        std::copy(rotations[i].R, rotations[i].R + 9, &R[9 * i]);
+        reg[i] = registered[i] ? 1 : 0;
+    }
+    ps_position_params prm{};
+    prm.loss = params.loss;
+    prm.max_iters = params.max_iters;
+    prm.cg_max_iters = params.cg_max_iters;
+    prm.loss_scale = params.loss_scale;
+    prm.function_tol = params.function_tol;
+    prm.cg_tol = params.cg_tol;
+    DevBuf start(tracks.start.size() * sizeof(int32_t), b.who), members(nm * sizeof(int32_t), b.who), X(nt * 3 * sizeof(double), b.who);
+    check(ps_host_to_dev(start.p, tracks.start.data(), tracks.start.size() * sizeof(int32_t)), b.who);
+    check(ps_host_to_dev(members.p, mem.data(), nm * sizeof(int32_t)), b.who);
+    ps_position_report r;
+    check(ps_global_positioning(b.dev, (int)sets.size(), n_feat.data(), b.feat.data(), cams.data(), R.data(), reg.data(), (int)nt,
+                                static_cast<const int32_t*>(start.p), static_cast<const int32_t*>(members.p), (int)nm, &prm, rig.data(),
+                                pos.data(), static_cast<double*>(X.p), &r),
+          b.who, "ps_global_positioning");
+    Positions out;
+    out.X.resize(3 * nt);
+    check(ps_dev_to_host(out.X.data(), X.p, 3 * nt * sizeof(double)), b.who);
+    out.poses.resize(sets.size());
+    out.positioned.resize(sets.size());
+    for (size_t i = 0; i < sets.size(); ++i) {
+        std::copy(rig[i].R, rig[i].R + 9, out.poses[i].R);
+        std::copy(rig[i].t, rig[i].t + 3, out.poses[i].t);
+        out.positioned[i] = pos[i] != 0;
+    }
+    PositionReport& o = out.report;
+    o.initial_cost = r.initial_cost;
+    o.final_cost = r.final_cost;
+    o.iterations = r.iterations;
+    o.cg_iterations = r.cg_iterations;
+    o.n_obs = r.n_obs;
+    o.n_points = r.n_points;
+    o.n_cams = r.n_cams;
+    o.termination = r.termination;
+    return out;
 }
 
 } // namespace popsift

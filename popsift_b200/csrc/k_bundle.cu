@@ -110,37 +110,6 @@ struct BaArgs {
     double s2;
 };
 
-__device__ __forceinline__ double warp_sum(double v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-    return v;
-}
-
-// N values summed over a CTA of NT threads: xor butterflies within warps, then the warps in index order; the result is
-// valid in thread 0
-template <int N, int NT>
-__device__ void cta_sum(double (&v)[N])
-{
-    __shared__ double part[NT / 32][N];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-        const double s = warp_sum(v[k]);
-        if (lane == 0) part[w][k] = s;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int k = 0; k < N; ++k) {
-            double s = part[0][k];
-            for (int q = 1; q < NT / 32; ++q) s += part[q][k];
-            v[k] = s;
-        }
-    }
-    __syncthreads();
-}
-
 __device__ __forceinline__ int ba_set_of(const int32_t* __restrict__ off, int n_sets, int g)
 {
     int lo = 0, hi = n_sets - 1;    // the last set with off[s] <= g (an empty set shares its offset with the next)

@@ -1,6 +1,7 @@
 // Device-wide exclusive scan and stable LSD radix sort (8-bit digits) without a library, shared by the track builder
-// (k_tracks.cu) and bundle adjustment's camera-major order (k_bundle.cu).  Both are deterministic: no floating point, and
-// every entry's output position depends only on the input.
+// (k_tracks.cu), bundle adjustment's camera-major order (k_bundle.cu) and global positioning's (k_global.cu).  Both are
+// deterministic: no floating point, and every entry's output position depends only on the input.  Also the CTA sum of
+// doubles the solvers use, in a fixed order.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -14,6 +15,39 @@ constexpr long long kScanChunk = (long long)kScanT * kScanPer;
 constexpr int kRadixT = 256;            // threads of a radix block: one per digit
 constexpr int kRadixRounds = 16;        // rounds of kRadixT elements per radix tile
 constexpr long long kRadixTile = (long long)kRadixT * kRadixRounds;
+
+// ---- deterministic CTA sums of doubles (bundle adjustment, global poses)
+
+__device__ __forceinline__ double warp_sum(double v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// N values summed over a CTA of NT threads: xor butterflies within warps, then the warps in index order; the result is
+// valid in thread 0
+template <int N, int NT>
+__device__ void cta_sum(double (&v)[N])
+{
+    __shared__ double part[NT / 32][N];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+        const double s = warp_sum(v[k]);
+        if (lane == 0) part[w][k] = s;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) {
+            double s = part[0][k];
+            for (int q = 1; q < NT / 32; ++q) s += part[q][k];
+            v[k] = s;
+        }
+    }
+    __syncthreads();
+}
 
 // ---- device-wide exclusive scan: blocks of kScanChunk elements, the block sums scanned recursively, then added back
 

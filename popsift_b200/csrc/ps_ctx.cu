@@ -14,6 +14,7 @@
 #include "popsift_b200_tracks.h"
 #include "popsift_b200_triangulate.h"
 #include "popsift_b200_bundle.h"
+#include "popsift_b200_global.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1501,6 +1502,98 @@ extern "C" int ps_bundle_adjust(int device, int n_sets, const int32_t* n_feat, c
     const int rc = finish("ps_bundle_adjust", n, err);
     if (rc == PS_OK) {
         std::memcpy(poses_out, out.data(), (size_t)n_sets * sizeof(ps_rigid));
+        *report = rep;
+    }
+    return rc;
+}
+
+// a rotation ps_global_positioning takes: ps_triangulate_tracks' check of a pose's rotation part
+static bool rotation_ok(const double* R)
+{
+    ps_rigid p{};
+    std::memcpy(p.R, R, sizeof(p.R));
+    return rigid_ok(p);
+}
+
+extern "C" int ps_rotation_averaging(int device, int n_sets, int n_pairs, const int32_t* pairs, const ps_two_view* d_two_view,
+                                     const ps_rotation_params* prm, double* R_out, uint8_t* registered, float* pair_error,
+                                     ps_rotation_report* report)
+{
+    if (n_sets < 0 || n_pairs < 0 || !prm || !R_out || !registered || !report || (n_pairs > 0 && !pairs)) return PS_ERR_ARG;
+    for (int p = 0; p < 2 * n_pairs; ++p)
+        if (pairs[p] < 0 || pairs[p] >= n_sets) return PS_ERR_ARG;
+    if (prm->loss < PS_LOSS_SQUARED || prm->loss > PS_LOSS_CAUCHY || prm->min_inliers < 0) return PS_ERR_ARG;
+    if (prm->max_iters < 0 || prm->max_iters > 10000 || prm->cg_max_iters < 1 || prm->cg_max_iters > 10000) return PS_ERR_ARG;
+    if (!std::isfinite(prm->loss_scale) || !(prm->loss_scale > 0.0)) return PS_ERR_ARG;
+    if (!std::isfinite(prm->step_tol) || !(prm->step_tol >= 0.0)) return PS_ERR_ARG;
+    if (!(prm->cg_tol >= 0.0 && prm->cg_tol < 1.0)) return PS_ERR_ARG;
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (n_pairs > 0 && ps_pointer_device(d_two_view) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    std::vector<double> R((size_t)n_sets * 9);
+    std::vector<uint8_t> reg(n_sets);
+    std::vector<float> perr(n_pairs);
+    ps_rotation_report rep{};
+    const int n = run_rotation_averaging(n_sets, n_pairs, pairs, d_two_view, *prm, R.data(), reg.data(), perr.data(), &rep, nullptr, &err);
+    const int rc = finish("ps_rotation_averaging", n, err);
+    if (rc == PS_OK) {
+        if (n_sets) std::memcpy(R_out, R.data(), R.size() * 8);
+        if (n_sets) std::memcpy(registered, reg.data(), reg.size());
+        if (pair_error && n_pairs) std::memcpy(pair_error, perr.data(), perr.size() * 4);
+        *report = rep;
+    }
+    return rc;
+}
+
+extern "C" int ps_global_positioning(int device, int n_sets, const int32_t* n_feat, const ps_feature* const* d_feat, const ps_camera* cams,
+                                     const double* R, const uint8_t* registered, int n_tracks, const int32_t* d_track_start,
+                                     const int32_t* d_members, int n_members, const ps_position_params* prm, ps_rigid* poses_out,
+                                     uint8_t* positioned, double* d_X, ps_position_report* report)
+{
+    if (!prm || !report || n_sets < 0 || n_tracks < 0 || n_members < 0) return PS_ERR_ARG;
+    if (n_sets > 0 && (!n_feat || !d_feat || !cams || !R || !registered || !poses_out || !positioned)) return PS_ERR_ARG;
+    for (int i = 0; i < n_sets; ++i) {
+        const ps_camera& c = cams[i];
+        if (!std::isfinite(c.fx) || !(c.fx > 0.0f) || !std::isfinite(c.fy) || !(c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
+            return PS_ERR_ARG;
+        if (!rotation_ok(R + 9 * (size_t)i) || registered[i] > 1) return PS_ERR_ARG;
+    }
+    if (prm->loss < PS_LOSS_SQUARED || prm->loss > PS_LOSS_CAUCHY) return PS_ERR_ARG;
+    if (prm->max_iters < 0 || prm->max_iters > 10000 || prm->cg_max_iters < 1 || prm->cg_max_iters > 10000) return PS_ERR_ARG;
+    if (!std::isfinite(prm->loss_scale) || !(prm->loss_scale > 0.0)) return PS_ERR_ARG;
+    if (!std::isfinite(prm->function_tol) || !(prm->function_tol >= 0.0)) return PS_ERR_ARG;
+    if (!(prm->cg_tol >= 0.0 && prm->cg_tol < 1.0)) return PS_ERR_ARG;
+    if (n_tracks == 0) {
+        std::memset(report, 0, sizeof(*report));
+        report->termination = PS_GP_NO_OBSERVATIONS;
+        for (int i = 0; i < n_sets; ++i) {
+            std::memcpy(poses_out[i].R, R + 9 * (size_t)i, sizeof(poses_out[i].R));
+            poses_out[i].t[0] = poses_out[i].t[1] = poses_out[i].t[2] = 0.0;
+            positioned[i] = 0;
+        }
+        return PS_OK;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    int64_t N = 0;
+    if (!check_sets(device, n_sets, n_feat, d_feat, 0, &N) || N >= 0x80000000LL) return PS_ERR_ARG;
+    if (ps_pointer_device(d_track_start) != device) return PS_ERR_ARG;
+    if (n_members > 0 && ps_pointer_device(d_members) != device) return PS_ERR_ARG;
+    if (d_X && ps_pointer_device(d_X) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    bool bad = false;
+    std::vector<ps_rigid> out(n_sets);
+    std::vector<uint8_t> pos(n_sets);
+    ps_position_report rep{};
+    const int n = run_global_positioning(n_sets, n_feat, d_feat, cams, R, registered, n_tracks, d_track_start, d_members, n_members, *prm,
+                                         out.data(), pos.data(), d_X, &rep, &bad, nullptr, &err);
+    if (n >= 0 && bad) {
+        g_create_error = "ps_global_positioning: a member id or d_track_start is out of range";
+        return PS_ERR_ARG;
+    }
+    const int rc = finish("ps_global_positioning", n, err);
+    if (rc == PS_OK) {
+        if (n_sets) std::memcpy(poses_out, out.data(), (size_t)n_sets * sizeof(ps_rigid));
+        if (n_sets) std::memcpy(positioned, pos.data(), pos.size());
         *report = rep;
     }
     return rc;

@@ -5,6 +5,7 @@
 #include "popsift_b200_tracks.h"
 #include "popsift_b200_triangulate.h"
 #include "popsift_b200_bundle.h"
+#include "popsift_b200_global.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
@@ -299,5 +300,17 @@ int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const
                       int n_tracks, const int32_t* track_start, const int32_t* members, int n_members, ps_track_point* points,
                       const uint8_t* obs_mask, const uint8_t* fixed, const ps_bundle_params& prm, ps_rigid* poses_out, float* obs_error,
                       ps_bundle_report* report, bool* bad, cudaStream_t st, const char** err);
+
+// global poses (include/popsift_b200_global.h, k_global.cu), arguments already validated.  Rotation averaging reads the
+// two-view records back once, starts on the host and writes every output when it returns >= 0.  Positioning: the member
+// ids and d_track_start are checked by the first pass (a bad one sets *bad, and the call returns before writing any
+// output); otherwise every output is written.  Synchronous on `st`; return the number of kernels launched or -1 (*err set).
+int run_rotation_averaging(int n_sets, int n_pairs, const int32_t* pairs, const ps_two_view* d_two_view, const ps_rotation_params& prm,
+                           double* R_out, uint8_t* registered, float* pair_error, ps_rotation_report* report, cudaStream_t st,
+                           const char** err);
+int run_global_positioning(int n_sets, const int32_t* n_feat, const ps_feature* const* feat, const ps_camera* cams, const double* R,
+                           const uint8_t* registered, int n_tracks, const int32_t* track_start, const int32_t* members, int n_members,
+                           const ps_position_params& prm, ps_rigid* poses_out, uint8_t* positioned, double* X_out,
+                           ps_position_report* report, bool* bad, cudaStream_t st, const char** err);
 
 } // namespace psb
