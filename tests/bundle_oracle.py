@@ -110,8 +110,8 @@ class Problem:
         self.n = col + 3 * len(self.points)
 
     def residuals(self, poses, X):
-        R = np.stack([np.asarray(poses[i][0], np.float64) for i in self.set])
-        t = np.stack([np.asarray(poses[i][1], np.float64) for i in self.set])
+        R = np.stack([np.asarray(p[0], np.float64) for p in poses])[self.set]
+        t = np.stack([np.asarray(p[1], np.float64) for p in poses])[self.set]
         return jacobian(self.cams[self.set], R, t, np.asarray(X, np.float64)[self.track], self.xy[:, 0], self.xy[:, 1])
 
     def cost(self, poses, X):
@@ -150,8 +150,7 @@ class Problem:
         for i, cols in self.cam_cols.items():
             di = np.array([d[c] if c >= 0 else 0.0 for c in cols])
             poses[i] = pose_update(poses[i][0], poses[i][1], di)
-        for j, c in self.pt_col.items():
-            X[j] = X[j] + d[c:c + 3]
+        X[self.points] = X[self.points] + np.asarray(d[self.n_cam:], np.float64).reshape(-1, 3)
         return poses, X
 
     def step(self, poses, X, lam, schur=False):
@@ -163,6 +162,102 @@ class Problem:
         d = schur_solve(Hd, -g, self.n_cam) if schur else np.linalg.solve(Hd, -g)
         pred = -(g @ d + 0.5 * d @ H @ d)
         return d, pred
+
+    def schur_step(self, poses, X, lam):
+        """step()'s damped step by the Schur complement onto the cameras, vectorised: (d, pred, ReducedSystem)"""
+        sys_ = ReducedSystem(self, poses, X, lam)
+        d = sys_.solve()
+        return d, sys_.pred(d), sys_
+
+
+class ReducedSystem:
+    """One LM step's reduced camera system S x = b (S = U + lambda D - sum_j W_j V_j^-1 W_j^T, the points eliminated),
+    assembled without a dense Jacobian: per-set blocks U_i and g_i, per-track blocks V_j and g_j with step()'s damping, and
+    S from every within-track pair of observations.  The columns are the problem's camera columns (a held component and
+    the fixed and unobserved sets have none)."""
+
+    def __init__(self, prob, poses, X, lam):
+        front, e, Jc, Jp = prob.residuals(poses, X)
+        _, w = loss(prob.loss, (e[:, 0] * e[:, 0] + e[:, 1] * e[:, 1]) / (prob.s * prob.s))
+        sw = np.sqrt(w)
+        e, Jc, Jp = e * sw[:, None], Jc * sw[:, None, None], Jp * sw[:, None, None]
+        # camera columns: cam[u, k] is the column of observation u's pose component k, or -1
+        colmap = np.full((prob.S, 6), -1, np.int64)
+        for i, cols in prob.cam_cols.items():
+            colmap[i] = cols
+        cam = colmap[prob.set]
+        Jc = np.where((cam >= 0)[:, None, :], Jc, 0.0)
+        self.prob, self.nc, self.cam = prob, prob.n_cam, cam
+        nc = self.nc
+        # points: k = the index of observation u's point among prob.points
+        pk = np.searchsorted(prob.points, prob.track)
+        nP = len(prob.points)
+        self.pk, self.Jc, self.Jp, self.e = pk, Jc, Jp, e
+        V = np.zeros((nP, 3, 3))
+        np.add.at(V, pk, np.einsum("ura,urb->uab", Jp, Jp))
+        self.gp = np.zeros((nP, 3))
+        np.add.at(self.gp, pk, np.einsum("ura,ur->ua", Jp, e))
+        Vd = V.copy()
+        for a in range(3):
+            Vd[:, a, a] = damp(V[:, a, a], lam)
+        self.Vi = np.linalg.inv(Vd)
+        # U and g over the camera columns (observation u's 6 x 6 block scattered to its columns)
+        Wu = np.einsum("ura,urb->uab", Jc, Jp)                 # (U, 6, 3): Jc^T Jp
+        self.Wu = Wu
+        gc_u = np.einsum("ura,ur->ua", Jc, e)
+        self.gc = np.bincount(cam[cam >= 0], weights=gc_u[cam >= 0], minlength=nc)
+        Uu = np.einsum("ura,urb->uab", Jc, Jc)
+        ok = (cam[:, :, None] >= 0) & (cam[:, None, :] >= 0)
+        flat = (cam[:, :, None] * nc + cam[:, None, :])[ok]
+        Uc = np.bincount(flat, weights=Uu[ok], minlength=nc * nc).reshape(nc, nc)
+        self.Ud = Uc.copy()
+        self.Ud[np.diag_indices(nc)] = damp(np.diag(Uc), lam)
+        self.Uc = Uc
+        # S = Ud - sum over within-track pairs (u, v) of W_u Vi W_v^T; b = -g_c + sum_u W_u Vi g_p
+        WVi = np.einsum("uab,ubc->uac", Wu, self.Vi[pk])      # (U, 6, 3)
+        self.WVi = WVi
+        bu = np.einsum("uab,ub->ua", WVi, self.gp[pk])
+        self.b = -self.gc + np.bincount(cam[cam >= 0], weights=bu[cam >= 0], minlength=nc)
+        start = np.searchsorted(pk, np.arange(nP + 1))          # observations are track-major, so each point's are a run
+        L = np.diff(start)
+        S = self.Ud.copy().reshape(-1)
+        for n in np.unique(L):                                  # tracks of one length at a time, in chunks
+            tr = np.flatnonzero(L == n)
+            for c0 in range(0, len(tr), max(1, 200000 // (n * n))):
+                base = start[tr[c0:c0 + max(1, 200000 // (n * n))]]
+                uu = (base[:, None, None] + np.arange(n)[None, :, None]).repeat(n, 2).reshape(-1)
+                vv = (base[:, None, None] + np.arange(n)[None, None, :]).repeat(n, 1).reshape(-1)
+                blk = np.einsum("pac,pbc->pab", WVi[uu], Wu[vv])
+                ca, cb = cam[uu][:, :, None], cam[vv][:, None, :]
+                m = (ca >= 0) & (cb >= 0)
+                S -= np.bincount((ca * nc + cb)[m], weights=blk[m], minlength=nc * nc)
+        self.S = S.reshape(nc, nc)
+        self.pstart = start
+
+    def solve(self):
+        """the damped step in the problem's columns: the cameras by Cholesky, then the points by back-substitution"""
+        from scipy.linalg import cho_factor, cho_solve
+        xc = cho_solve(cho_factor(self.S), self.b) if self.nc else np.zeros(0)
+        return np.concatenate([xc, self.back(xc).reshape(-1)])
+
+    def back(self, xc):
+        """the points' step for a camera step xc: dX_j = -Vi_j (g_j + sum_u W_u^T xc)"""
+        xu = np.where(self.cam >= 0, np.asarray(xc, np.float64)[np.maximum(self.cam, 0)], 0.0)
+        s = np.zeros((len(self.Vi), 3))
+        np.add.at(s, self.pk, np.einsum("uab,ua->ub", self.Wu, xu))
+        return -np.einsum("jab,jb->ja", self.Vi, self.gp + s)
+
+    def pred(self, d):
+        """-(g.d + 1/2 d^T H d) of the undamped H = J^T J"""
+        xc, dX = d[:self.nc], d[self.nc:].reshape(-1, 3)
+        xu = np.where(self.cam >= 0, np.asarray(xc, np.float64)[np.maximum(self.cam, 0)], 0.0)
+        Jd = np.einsum("ura,ua->ur", self.Jc, xu) + np.einsum("ura,ua->ur", self.Jp, dX[self.pk])
+        return -(self.gc @ xc + (self.gp * dX).sum() + 0.5 * (Jd * Jd).sum())
+
+
+def schur_step(prob, poses, X, lam):
+    """(d, pred) of Problem.schur_step, for lm(solve=...)"""
+    return prob.schur_step(poses, X, lam)[:2]
 
 
 def schur_solve(A, b, nc):
@@ -178,8 +273,10 @@ def schur_solve(A, b, nc):
     return np.concatenate([xc, xp])
 
 
-def lm(prob, poses, X, max_iters=50, function_tol=1e-6, initial_lambda=1e-4):
-    """the header's LM with dense solves: (poses, X, report dict)"""
+def lm(prob, poses, X, max_iters=50, function_tol=1e-6, initial_lambda=1e-4, solve=None):
+    """the header's LM, each step by solve(prob, poses, X, lambda) -> (d, pred) (default the dense Problem.step; schur_step
+    for large problems): (poses, X, report dict)"""
+    solve = solve or (lambda p, po, x, lam: p.step(po, x, lam))
     X = np.asarray(X, np.float64).copy()
     rep = dict(iterations=0, accepted=0, termination=MAX_ITERS)
     if len(prob.set) == 0:
@@ -192,7 +289,7 @@ def lm(prob, poses, X, max_iters=50, function_tol=1e-6, initial_lambda=1e-4):
         return poses, X, rep
     lam, nu = float(initial_lambda), 2.0
     for _ in range(max_iters):
-        d, pred = prob.step(poses, X, lam)
+        d, pred = solve(prob, poses, X, lam)
         pn, Xn = prob.apply(poses, X, d)
         nc = prob.cost(pn, Xn)
         rep["iterations"] += 1
@@ -227,7 +324,8 @@ def small_rotation(rng, deg):
 
 
 def planted(rng, n_cams, lengths, noise=0.5, outliers=0.0, rot_deg=1.0, trans=0.2, point_sigma=0.02, **kw):
-    """triangulate_oracle.planted_scene (cameras on a sphere of radius 10 around a cloud of spread 2) with every pose
+    """triangulate_oracle.planted_scene (cameras on a sphere of radius 10 around a cloud of spread 2; sets= gives every
+    track's cameras) with every pose
     turned by rot_deg about a random axis and its t moved by `trans` (about 2 % of the scene scale) in a random direction,
     and every point moved by point_sigma per axis.  Adds poses_true, X0 (the perturbed points), status (all OK) and mask
     (all 1)."""

@@ -133,8 +133,9 @@ def start(n_sets, pairs, Rp, n_front, min_inliers):
     return used, reg, root, R
 
 
-def laplacian_solve(n, ends, W, g, root):
-    """the weighted Laplacian (x) I3 system of the header with node `root` and the nodes of zero degree held: x (n, 3)"""
+def laplacian_solve(n, ends, W, g, root, n_cam=None):
+    """the weighted Laplacian (x) I3 system of the header with node `root` and the nodes of zero degree held: x (n, 3).
+    Dense; n_cam (where the point nodes start, see LaplacianSystem) is not needed here."""
     D = np.zeros(n)
     b = np.zeros((n, 3))
     for (a, c), w, ge in zip(ends, W, g):
@@ -161,8 +162,97 @@ def laplacian_solve(n, ends, W, g, root):
     return x
 
 
-def rotation_averaging(n_sets, pairs, Rp, n_front, loss="cauchy", loss_scale=5.0, max_iters=100, step_tol=1e-4, min_inliers=15):
-    """ps_rotation_averaging with dense solves: (R (S, 3, 3), registered, pair_error (deg), report dict)"""
+class LaplacianSystem:
+    """laplacian_solve's system with the point nodes (n_cam and up) eliminated, assembled with bincount.  A point node joins
+    only camera nodes, so its row is D_j x_j - sum_e w_e x_c(e) = b_j and x_j = (b_j + sum_e w_e x_c(e)) / D_j; putting that
+    into the camera rows leaves S x_c = b_c with S = L_cc - sum_j sum_{e, f at j} w_e w_f / D_j and
+    b_c = b_c + sum_j sum_{e at j} w_e b_j / D_j, over the free camera nodes (not the root, degree > 0)."""
+
+    def __init__(self, n, ends, W, g, root, n_cam=None):
+        n_cam = n if n_cam is None else n_cam
+        ends = np.asarray(ends, np.int64).reshape(-1, 2)
+        W, g = np.asarray(W, np.float64), np.asarray(g, np.float64).reshape(-1, 3)
+        on = W != 0.0
+        ends, W, g = ends[on], W[on], g[on]
+        a, c = ends[:, 0], ends[:, 1]
+        assert not ((a >= n_cam) & (c >= n_cam)).any(), "an edge between two point nodes"
+        D = np.bincount(a, weights=W, minlength=n) + np.bincount(c, weights=W, minlength=n)
+        b = np.stack([np.bincount(a, weights=g[:, k], minlength=n) - np.bincount(c, weights=g[:, k], minlength=n) for k in range(3)], 1)
+        free = (D > 0.0) & (np.arange(n) != root)
+        self.n, self.n_cam, self.D, self.bfull, self.free = n, n_cam, D, b, free
+        cams = np.flatnonzero(free[:n_cam])
+        idx = np.full(n, -1, np.int64)
+        idx[cams] = np.arange(len(cams))
+        self.cams, self.idx = cams, idx
+        m = len(cams)
+        # camera-camera edges
+        cc = (a < n_cam) & (c < n_cam)
+        Lf = np.bincount(idx[cams] * m + idx[cams], weights=D[cams], minlength=m * m)
+        for u, v in ((a[cc], c[cc]), (c[cc], a[cc])):
+            k = (idx[u] >= 0) & (idx[v] >= 0)
+            Lf -= np.bincount(idx[u[k]] * m + idx[v[k]], weights=W[cc][k], minlength=m * m)
+        # camera-point edges, grouped by point: every pair (e, f) at a free point
+        pe = ~cc
+        pt = np.where(a[pe] >= n_cam, a[pe], c[pe])
+        cm = np.where(a[pe] >= n_cam, c[pe], a[pe])
+        wp = W[pe]
+        o = np.argsort(pt, kind="stable")
+        pt, cm, wp = pt[o], cm[o], wp[o]
+        self.pt, self.cm, self.wp = pt, cm, wp
+        bc = b[cams].copy()
+        if len(pt):
+            fp = free[pt]
+            k = fp & (idx[cm] >= 0)
+            for q in range(3):
+                bc[:, q] += np.bincount(idx[cm[k]], weights=wp[k] * b[pt[k], q] / D[pt[k]], minlength=m)
+            uniq, first, cnt = np.unique(pt, return_index=True, return_counts=True)
+            for L in np.unique(cnt):
+                sel = first[cnt == L]
+                e = (sel[:, None, None] + np.arange(L)[None, :, None]).repeat(L, 2).reshape(-1)
+                f = (sel[:, None, None] + np.arange(L)[None, None, :]).repeat(L, 1).reshape(-1)
+                k = free[pt[e]] & (idx[cm[e]] >= 0) & (idx[cm[f]] >= 0)
+                e, f = e[k], f[k]
+                Lf -= np.bincount(idx[cm[e]] * m + idx[cm[f]], weights=wp[e] * wp[f] / D[pt[e]], minlength=m * m)
+        self.S, self.b = Lf.reshape(m, m), bc
+
+    def points(self, xc):
+        """every node's x from the free cameras' x (m, 3): the held nodes 0, each free point by its row"""
+        x = np.zeros((self.n, 3))
+        x[self.cams] = xc
+        if len(self.pt):
+            s = np.stack([np.bincount(self.pt, weights=self.wp * x[self.cm, q], minlength=self.n) for q in range(3)], 1)
+            pts = np.flatnonzero(self.free & (np.arange(self.n) >= self.n_cam))
+            x[pts] = (self.bfull[pts] + s[pts]) / self.D[pts][:, None]
+        return x
+
+    def solve(self):
+        return self.points(np.linalg.solve(self.S, self.b) if len(self.cams) else np.zeros((0, 3)))
+
+
+def laplacian_solve_reduced(n, ends, W, g, root, n_cam=None):
+    """laplacian_solve by LaplacianSystem: the same x (n, 3), to rounding"""
+    return LaplacianSystem(n, ends, W, g, root, n_cam).solve()
+
+
+def log_batch(M):
+    """log of each (..., 3, 3): gl_log's branch c > -0.99 vectorised, the rest one by one"""
+    M = np.asarray(M, np.float64).reshape(-1, 3, 3)
+    c = np.clip(0.5 * ((M[:, 0, 0] + M[:, 1, 1] + M[:, 2, 2]) - 1.0), -1.0, 1.0)
+    s = np.stack([0.5 * (M[:, 2, 1] - M[:, 1, 2]), 0.5 * (M[:, 0, 2] - M[:, 2, 0]), 0.5 * (M[:, 1, 0] - M[:, 0, 1])], 1)
+    sn = np.sqrt(s[:, 0] * s[:, 0] + s[:, 1] * s[:, 1] + s[:, 2] * s[:, 2])
+    th = np.arctan2(sn, c)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        f = np.where(sn < 1e-8, 1.0 + sn * sn / 6.0, th / sn)
+    out = f[:, None] * s
+    for k in np.flatnonzero(~(c > -0.99)):
+        out[k] = log(M[k])
+    return out
+
+
+def rotation_averaging(n_sets, pairs, Rp, n_front, loss="cauchy", loss_scale=5.0, max_iters=100, step_tol=1e-4, min_inliers=15,
+                       solve=laplacian_solve):
+    """ps_rotation_averaging, each Laplacian system by solve(n, ends, W, g, root) (default dense; laplacian_solve_reduced
+    for large graphs): (R (S, 3, 3), registered, pair_error (deg), report dict)"""
     pairs = [(int(a), int(b)) for a, b in pairs]
     Rp = np.asarray(Rp, np.float32).reshape(-1, 3, 3)
     Rp = np.stack([orthonormal(m) if np.isfinite(m).all() else m.astype(np.float64) for m in Rp]) if len(Rp) else np.zeros((0, 3, 3))
@@ -171,16 +261,17 @@ def rotation_averaging(n_sets, pairs, Rp, n_front, loss="cauchy", loss_scale=5.0
     rep = dict(iterations=0, n_pairs=int(used.sum()), n_registered=int(reg.sum()), termination=RA_MAX_ITERS, initial_cost=0.0,
                final_cost=0.0)
 
+    ends = np.asarray(pairs, np.int64).reshape(-1, 2)
+
     def lin(R):
-        W, g, err, cost = np.zeros(len(pairs)), np.zeros((len(pairs), 3)), np.full(len(pairs), np.inf), 0.0
-        for p in np.flatnonzero(used):
-            l, r = pairs[p]
-            res = pair_residual(R[l], R[r], Rp[p])
-            r2 = float(res @ res)
-            rho, w = bo.loss(loss, r2 / s2)
-            W[p], g[p], err[p] = float(w), -float(w) * res, math.sqrt(r2) / DEG
-            cost += 0.5 * (s2 * float(rho))
-        return W, g, err, cost
+        W, g, err = np.zeros(len(pairs)), np.zeros((len(pairs), 3)), np.full(len(pairs), np.inf)
+        u = np.flatnonzero(used)
+        l, r = ends[u, 0], ends[u, 1]
+        res = log_batch(np.matmul(np.swapaxes(R[r], 1, 2), np.matmul(Rp[u], R[l])))
+        r2 = (res * res).sum(1)
+        rho, w = bo.loss(loss, r2 / s2)
+        W[u], g[u], err[u] = w, -w[:, None] * res, np.sqrt(r2) / DEG
+        return W, g, err, float(np.sum(0.5 * (s2 * rho)))
 
     if not used.any():
         rep["termination"] = RA_NO_PAIRS
@@ -188,7 +279,7 @@ def rotation_averaging(n_sets, pairs, Rp, n_front, loss="cauchy", loss_scale=5.0
     W, g, err, cost = lin(R)
     rep["initial_cost"] = cost
     for _ in range(max_iters):
-        x = laplacian_solve(n_sets, pairs, W, g, root)
+        x = solve(n_sets, ends, W, g, root)
         for i in np.flatnonzero(reg):
             if i != root:
                 R[i] = R[i] @ exp(x[i])
@@ -216,7 +307,10 @@ def obs(v, X, c):
 class Positioning:
     """the used observations of a scene under rotations R and the registered flags (member order)"""
 
-    def __init__(self, feats, cams, R, registered, start, members, loss="huber", loss_scale=0.1):
+    def __init__(self, feats, cams, R, registered, start, members, loss="huber", loss_scale=0.1, solve=laplacian_solve):
+        """solve(n, ends, W, g, root, n_cam) solves each Laplacian system: laplacian_solve (dense), or for large scenes
+        laplacian_solve_reduced, the point nodes eliminated"""
+        self.solve = solve
         n_feat = [len(f) for f in feats]
         off = np.concatenate([[0], np.cumsum(n_feat)]).astype(np.int64)
         allxy = np.concatenate([np.asarray(f, np.float32).reshape(-1, 2) for f in feats])
@@ -236,7 +330,7 @@ class Positioning:
         self.v = np.where(self.used[:, None], self.v, 0.0)
         self.positioned = np.bincount(self.set[self.used], minlength=self.S) > 0
         self.root = int(np.flatnonzero(self.positioned)[0]) if self.positioned.any() else -1
-        self.ends = list(zip((self.S + self.track).tolist(), self.set.tolist()))
+        self.ends = np.stack([self.S + self.track, self.set], 1)
         self.loss, self.s2 = loss, float(loss_scale) ** 2
 
     def lin(self, pos, init=False):
@@ -259,13 +353,13 @@ class Positioning:
 
     def step(self, pos, init=False):
         W, g, _ = self.lin(pos, init)
-        return pos + laplacian_solve(self.S + self.T, self.ends, W, g, self.root)
+        return pos + self.solve(self.S + self.T, self.ends, W, g, self.root, n_cam=self.S)
 
     def extended_step(self, pos, max_doublings=20):
         """the header's iteration: the majorise-minimise step x, then pos + 2^k x for k = 1 .. 20 while the cost keeps
         decreasing (the device adds x, x, 2x, 4x, ... in place, so the two agree to rounding): (positions, cost)"""
         W, g, _ = self.lin(pos)
-        x = laplacian_solve(self.S + self.T, self.ends, W, g, self.root)
+        x = self.solve(self.S + self.T, self.ends, W, g, self.root, n_cam=self.S)
         best = pos + x
         bc, a = self.cost(best), 1.0
         for _ in range(max_doublings):
@@ -334,10 +428,11 @@ def random_rotation(rng):
                      [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
 
 
-def view_graph(rng, n_cams, n_pairs, noise_deg=0.5, outliers=0.2):
+def view_graph(rng, n_cams, n_pairs, noise_deg=0.5, outliers=0.2, hub=None):
     """random true rotations, n_pairs distinct pairs over a connected graph (a random tree first), R_p = R_r R_l^T turned
     by noise_deg about a random axis, or a random rotation for the outlier fraction; n_front from 30 to 500, outliers
-    below 100.  Returns (R_true, pairs, Rp, n_front, is_outlier)."""
+    below 100.  hub = (node, degree): that node gets pairs with `degree` distinct others (added after the tree).
+    Returns (R_true, pairs, Rp, n_front, is_outlier)."""
     Rt = np.stack([random_rotation(rng) for _ in range(n_cams)])
     perm = rng.permutation(n_cams)
     edges = set()
@@ -345,6 +440,15 @@ def view_graph(rng, n_cams, n_pairs, noise_deg=0.5, outliers=0.2):
         j = int(rng.integers(0, i))
         a, b = int(perm[i]), int(perm[j])
         edges.add((min(a, b), max(a, b)))
+    if hub is not None:
+        h, deg = hub
+        others = [int(o) for o in rng.permutation(n_cams) if o != h]
+        have = {a if b == h else b for a, b in edges if h in (a, b)}
+        for o in others:
+            if len(have) >= deg:
+                break
+            have.add(o)
+            edges.add((min(h, o), max(h, o)))
     while len(edges) < n_pairs:
         a, b = rng.choice(n_cams, 2, replace=False)
         edges.add((int(min(a, b)), int(max(a, b))))

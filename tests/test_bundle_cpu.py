@@ -171,3 +171,111 @@ def test_header_exports_and_layouts():
     for k, name in enumerate(api.BA_LOSS):
         assert "PS_LOSS_%s = %d" % (name.upper(), k) in body
     assert bo.LOSSES == api.BA_LOSS
+
+
+# ---- the vectorised Schur-complement step against the dense one ----
+
+def _edge_scene(seed):
+    """fixed sets 0 and 3, an empty set in the middle (4) and at the end (7), masked members, non-OK tracks"""
+    import scale_shapes as ss
+    import triangulate_oracle as tro
+    rng = np.random.default_rng(seed)
+    sc = ss.bundle_scene(seed, 8, lengths=list(rng.integers(2, 7, size=50)), empty=(4, 7), fixed=(0, 3))
+    sc["mask"][::6] = 0
+    sc["status"][::9] = tro.TOO_FEW_INLIERS
+    return sc
+
+
+@pytest.mark.parametrize("loss", bo.LOSSES)
+def test_schur_step_equals_dense(loss):
+    for seed, held in ((21, (1, 2)), (22, (5, 0)), (23, (-1, 0))):
+        sc = _edge_scene(seed)
+        p = bo.problem(sc, sc["fixed"], loss_kind=loss, loss_scale=2.0, scale_set=held[0], scale_axis=held[1])
+        assert len(p.free) == 4 and (held[0] < 0 or p.held)
+        for lam in (1e-4, 1e-3, 10.0):
+            d1, pr1 = p.step(sc["poses"], sc["X0"], lam)
+            d2, pr2, sy = p.schur_step(sc["poses"], sc["X0"], lam)
+            assert np.abs(d1 - d2).max() <= 1e-10 * np.abs(d1).max(), (seed, lam)
+            assert abs(pr1 - pr2) <= 1e-10 * abs(pr1) and pr1 > 0
+            # the reduced system is the dense one's Schur complement
+            J, e = p.system(sc["poses"], sc["X0"])
+            H = J.T @ J
+            H[np.diag_indices(p.n)] = bo.damp(np.diag(H), lam)
+            A, B, C = H[:p.n_cam, :p.n_cam], H[:p.n_cam, p.n_cam:], H[p.n_cam:, p.n_cam:]
+            g = J.T @ e
+            Ci = np.linalg.inv(C)
+            S = A - B @ Ci @ B.T
+            assert np.abs(sy.S - S).max() <= 1e-10 * np.abs(S).max()
+            assert np.abs(sy.b - (-g[:p.n_cam] + B @ Ci @ g[p.n_cam:])).max() <= 1e-10 * np.abs(sy.b).max()
+
+
+def test_lm_with_schur_steps_equals_dense():
+    sc = _edge_scene(24)
+    p = bo.problem(sc, sc["fixed"], loss_kind="cauchy", loss_scale=2.0, scale_set=1, scale_axis=0)
+    a = bo.lm(p, sc["poses"], sc["X0"], max_iters=4, initial_lambda=1e-3)
+    b = bo.lm(p, sc["poses"], sc["X0"], max_iters=4, initial_lambda=1e-3, solve=bo.schur_step)
+    assert a[2]["accepted"] == b[2]["accepted"] and a[2]["iterations"] == b[2]["iterations"] == 4
+    assert abs(a[2]["final_cost"] - b[2]["final_cost"]) <= 1e-10 * a[2]["final_cost"]
+    assert np.abs(a[1] - b[1]).max() <= 1e-9
+
+
+# ---- the boundary table against the kernel sources ----
+
+def kernel_constants():
+    """kCamT, kT, kCgT (k_bundle.cu), kNodeT, kRedT (k_global.cu), kScanChunk and kRadixTile (k_scan.h)"""
+    import re
+    src = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "popsift_b200", "csrc")
+
+    def ints(name):
+        return {m.group(1): m.group(2) for m in re.finditer(r"constexpr\s+(?:long long|int)\s+(\w+)\s*=\s*([^;]+);",
+                                                             open(os.path.join(src, name)).read())}
+    b, g, s = ints("k_bundle.cu"), ints("k_global.cu"), ints("k_scan.h")
+    assert b["kT"] == g["kT"]
+    k = {n: int(b[n]) for n in ("kCamT", "kT", "kCgT")}
+    k.update({n: int(g[n]) for n in ("kNodeT", "kRedT")})
+    env = {n: int(s[n]) for n in ("kScanT", "kScanPer", "kRadixT", "kRadixRounds")}
+    k["kScanChunk"] = eval(s["kScanChunk"].replace("(long long)", ""), {}, env)
+    k["kRadixTile"] = eval(s["kRadixTile"].replace("(long long)", ""), {}, env)
+    assert int(s["kRadixT"]) == 256          # one digit per thread: the histogram has 256 entries per tile
+    return k
+
+
+def test_boundary_rows_sit_on_their_boundaries():
+    """every row of tests/scale_shapes.py still straddles the boundary it names, so that a changed constant cannot leave
+    a scale test running on the easy side"""
+    import scale_shapes as ss
+    k = kernel_constants()
+    assert k == dict(kCamT=128, kT=256, kCgT=256, kNodeT=128, kRedT=256, kScanChunk=4096, kRadixTile=4096), k
+    cache = {}
+    for row, (kind, scene, doc, claims) in ss.ROWS.items():
+        key = (kind == "rotation", scene)
+        if key not in cache:
+            cache[key] = (ss.GRAPHS if kind == "rotation" else ss.SCENES)[scene]()
+        q = ss.quantities(kind, ss.stats(row, cache[key]), k)
+        for name, want in claims.items():
+            got = q[name][:len(want)] if isinstance(want, list) else q[name]
+            assert got == want, (row, doc, name, got, want)
+    # the rows come in pairs on each side of a boundary
+    st = {r: ss.stats(r, cache[(ss.ROWS[r][0] == "rotation", ss.ROWS[r][1])]) for r in ss.ROWS}
+    assert (st["ba_sets_256"]["S"], st["ba_sets_257"]["S"]) == (256, 257) and (st["gp_sets_255"]["S"], st["gp_sets_256"]["S"]) == (255, 256)
+    assert list(st["ba_counts"]["counts"][:6]) == list(ss.COUNTS) + [ss.FIXED_COUNT] and st["ba_counts"]["counts"][[8, 21]].sum() == 0
+    assert (st["ba_tracks_256"]["T"], st["ba_tracks_257"]["T"]) == (256, 257)
+    assert [st["ba_members_%d" % m]["M"] for m in (4095, 4096, 4097)] == [4095, 4096, 4097]
+    assert st["ba_large"]["T"] > 65536 and st["ba_large"]["S"] + st["ba_large"]["T"] > 256 * 256
+    assert (st["ra_pairs_256"]["P"], st["ra_pairs_257"]["P"]) == (256, 257) and st["ra_large"]["P"] > 65536
+    assert st["ra_sets_257_hub"]["S"] == 257 and st["ra_sets_257_hub"]["degree"].max() >= 129
+
+
+def test_large_oracle_runtime():
+    """the largest bundle scene's scene, Schur step and costs stay well inside the GPU tests' budget"""
+    import time
+    import scale_shapes as ss
+    t0 = time.perf_counter()
+    sc = ss.SCENES["large"]()
+    p = bo.problem(sc, sc["fixed"])
+    d, pred, _ = p.schur_step(sc["poses"], sc["X0"], 1e-3)
+    c0 = p.cost(sc["poses"], sc["X0"])
+    c1 = p.cost(*p.apply(sc["poses"], sc["X0"], d))
+    dt = time.perf_counter() - t0
+    print("large: %d observations, %d camera columns, %.1f s" % (len(p.set), p.n_cam, dt))
+    assert c1 < c0 and pred > 0 and dt < 30.0

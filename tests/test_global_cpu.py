@@ -204,3 +204,62 @@ def test_header_exports_and_layouts():
         assert "PS_RA_%s = %d" % (name.upper(), k) in body
     for k, name in enumerate(api.GP_TERMINATION):
         assert "PS_GP_%s = %d" % (name.upper(), k) in body
+
+
+# ---- the Laplacian with the point nodes eliminated against the dense one ----
+
+@pytest.mark.parametrize("loss", ["squared", "huber", "cauchy"])
+def test_reduced_laplacian_equals_dense(loss):
+    """positioning with an unregistered set, a track left with one member and a set without features; rotations with a
+    set outside the registered component and a pair below min_inliers"""
+    sc = _scene(9, n_cams=7, n_tracks=60, noise=0.3)
+    sc["feats"] = list(sc["feats"][:4]) + [np.zeros((0, 2), np.float32)] + list(sc["feats"][4:])
+    sc["cams"] = np.concatenate([sc["cams"][:4], sc["cams"][:1], sc["cams"][4:]])
+    sc["poses_true"] = list(sc["poses_true"][:4]) + [sc["poses_true"][0]] + list(sc["poses_true"][4:])
+    R = np.stack([np.asarray(r) for r, _ in sc["poses_true"]])
+    reg = np.ones(8, bool)
+    reg[2] = False
+    kw = dict(loss=loss, loss_scale=0.1)
+    a = go.Positioning(sc["feats"], sc["cams"], R, reg, sc["start"], sc["members"], **kw)
+    b = go.Positioning(sc["feats"], sc["cams"], R, reg, sc["start"], sc["members"], solve=go.laplacian_solve_reduced, **kw)
+    assert not a.positioned[[2, 4]].any() and (~a.tpart).any()
+    pa, ra = a.run(max_iters=4, function_tol=0.0)
+    pb, rb = b.run(max_iters=4, function_tol=0.0)
+    assert np.abs(pa - pb).max() <= 1e-10 * np.abs(pa).max() and abs(ra["final_cost"] - rb["final_cost"]) <= 1e-10 * ra["final_cost"]
+    W, g, _ = a.lin(pa)
+    assert np.abs(go.laplacian_solve(a.S + a.T, a.ends, W, g, a.root) -
+                  go.laplacian_solve_reduced(a.S + a.T, a.ends, W, g, a.root, n_cam=a.S)).max() <= 1e-10 * np.abs(pa).max()
+    Rt, pairs, Rp, nf, _ = go.view_graph(np.random.default_rng(10), 30, 120, hub=(3, 20))
+    pairs = pairs + [(30, 31)]
+    Rp = np.concatenate([Rp, Rp[:1]])
+    nf = np.r_[nf, 400]
+    nf[5] = 3
+    ra = go.rotation_averaging(32, pairs, Rp, nf, loss=loss, loss_scale=2.0, max_iters=3)
+    rb = go.rotation_averaging(32, pairs, Rp, nf, loss=loss, loss_scale=2.0, max_iters=3, solve=go.laplacian_solve_reduced)
+    assert not ra[1][30:].any() and ra[3]["n_pairs"] < len(pairs)
+    assert np.abs(ra[0] - rb[0]).max() <= 1e-10 and abs(ra[3]["final_cost"] - rb[3]["final_cost"]) <= 1e-10 * ra[3]["final_cost"]
+    fin = np.isfinite(ra[2])
+    assert np.array_equal(fin, np.isfinite(rb[2])) and np.abs(ra[2][fin] - rb[2][fin]).max() <= 1e-9
+
+
+def test_view_graph_hub():
+    _, pairs, _, _, _ = go.view_graph(np.random.default_rng(11), 300, 600, hub=(7, 150))
+    deg = np.bincount(np.asarray(pairs).reshape(-1), minlength=300)
+    assert deg[7] >= 150 and len(set(map(tuple, pairs))) == 600
+
+
+def test_large_oracles_runtime():
+    """the largest positioning scene's first solve and the largest view graph's IRLS stay inside the GPU tests' budget"""
+    import time
+    import scale_shapes as ss
+    t0 = time.perf_counter()
+    sc = ss.SCENES["large"]()
+    P = go.Positioning(sc["feats"], sc["cams"], sc["R"], np.ones(len(sc["R"]), bool), sc["start"], sc["members"],
+                       solve=go.laplacian_solve_reduced)
+    pos, rep = P.run(max_iters=1, function_tol=0.0)
+    t1 = time.perf_counter()
+    g = ss.GRAPHS["large"]()
+    go.rotation_averaging(600, g[1], g[2], g[3], max_iters=1, min_inliers=0, solve=go.laplacian_solve_reduced)
+    t2 = time.perf_counter()
+    print("positioning %.1f s, rotations %.1f s" % (t1 - t0, t2 - t1), rep)
+    assert rep["final_cost"] < rep["initial_cost"] and t2 - t0 < 40.0

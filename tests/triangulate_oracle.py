@@ -261,21 +261,18 @@ def project(cam, R, t, X):
     return np.stack([cam[0] * Xc[:, 0] / Xc[:, 2] + cam[2], cam[1] * Xc[:, 1] / Xc[:, 2] + cam[3]], 1)
 
 
-def planted_scene(rng, n_cams, lengths, noise=0.5, outliers=0.2, radius=10.0, spread=2.0, shift=(0.0, 0.0, 0.0)):
+def planted_scene(rng, n_cams, lengths, noise=0.5, outliers=0.2, radius=10.0, spread=2.0, shift=(0.0, 0.0, 0.0), sets=None):
     """Cameras on a sphere of `radius` around a cloud of `spread`, one track per entry of `lengths` (that many distinct
     cameras), pixel noise, and a fraction of outlier observations (uniform over the image).  The world frame is translated
-    by `shift`.  Returns dict(feats, cams, poses, start, members, Xtrue, outlier (members,) bool)."""
+    by `shift`.  `sets`, when given, is one array of distinct cameras per track (lengths must be their sizes): the cameras
+    that see it, so that a test can set every camera's observation count exactly; the observations are then drawn in bulk.
+    Returns dict(feats, cams, poses, start, members, Xtrue, outlier (members,) bool)."""
     shift = np.asarray(shift, np.float64)
-    cams = np.zeros((n_cams, 4), np.float32)
-    poses = []
-    for i in range(n_cams):
-        c = rng.normal(size=3); c *= radius / np.linalg.norm(c)
-        R, t = look_at(c + shift, shift + rng.normal(scale=0.2, size=3), rng)
-        f = rng.uniform(600, 1400)
-        cams[i] = (f, f * rng.uniform(0.98, 1.02), rng.uniform(300, 340), rng.uniform(230, 250))
-        poses.append((R, t))
+    cams, poses = _cameras(rng, n_cams, radius, shift)
     T = len(lengths)
     X = rng.normal(scale=spread / 2, size=(T, 3)) + shift
+    if sets is not None:
+        return _planted_sets(rng, cams, poses, X, lengths, noise, outliers, sets)
     obs_set, obs_xy, obs_track, outl = [], [], [], []
     for k, L in enumerate(lengths):
         cs = np.sort(rng.choice(n_cams, size=int(L), replace=False))
@@ -285,6 +282,39 @@ def planted_scene(rng, n_cams, lengths, noise=0.5, outliers=0.2, radius=10.0, sp
             if o:
                 uv = rng.uniform([0, 0], [640, 480])
             obs_set.append(c); obs_xy.append(uv); obs_track.append(k); outl.append(o)
+    return _pack(cams, poses, X, lengths, obs_set, obs_xy, outl)
+
+
+def _cameras(rng, n_cams, radius, shift):
+    cams = np.zeros((n_cams, 4), np.float32)
+    poses = []
+    for i in range(n_cams):
+        c = rng.normal(size=3); c *= radius / np.linalg.norm(c)
+        R, t = look_at(c + shift, shift + rng.normal(scale=0.2, size=3), rng)
+        f = rng.uniform(600, 1400)
+        cams[i] = (f, f * rng.uniform(0.98, 1.02), rng.uniform(300, 340), rng.uniform(230, 250))
+        poses.append((R, t))
+    return cams, poses
+
+
+def _planted_sets(rng, cams, poses, X, lengths, noise, outliers, sets):
+    """planted_scene's observations for the given cameras of every track, drawn in bulk"""
+    sets = [np.sort(np.asarray(s, np.int64)) for s in sets]
+    assert [len(s) for s in sets] == [int(L) for L in lengths] and all(len(np.unique(s)) == len(s) for s in sets)
+    obs_set = np.concatenate(sets) if sets else np.zeros(0, np.int64)
+    obs_track = np.repeat(np.arange(len(sets)), [len(s) for s in sets])
+    uv = np.zeros((len(obs_set), 2))
+    for c in np.unique(obs_set):
+        m = obs_set == c
+        uv[m] = project(cams[c].astype(np.float64), poses[c][0], poses[c][1], X[obs_track[m]])
+    uv += rng.normal(scale=noise, size=uv.shape)
+    outl = rng.random(len(uv)) < outliers
+    uv[outl] = rng.uniform([0, 0], [640, 480], size=(int(outl.sum()), 2))
+    return _pack(cams, poses, X, lengths, obs_set, uv, outl)
+
+
+def _pack(cams, poses, X, lengths, obs_set, obs_xy, outl):
+    n_cams = len(cams)
     obs_set = np.asarray(obs_set, np.int64)
     obs_xy = np.asarray(obs_xy, np.float32).reshape(-1, 2)
     order = np.lexsort((np.arange(len(obs_set)), obs_set))     # features of each set in observation order

@@ -219,3 +219,31 @@ if only in ("all", "bundle"):
     bad[4] = (np.diag([-1.0, 1.0, -1.0]) @ R, np.diag([-1.0, 1.0, -1.0]) @ t)
     _, _, rep = api.bundle_adjust(feats, tr, tp, sc["cams"], bad, fixed)
     print("bundle non-finite start", rep, flush=True)
+if only in ("all", "scale"):
+    # bundle adjustment, positioning and rotation averaging at the exact work-split boundaries (tests/scale_shapes.py):
+    # S = 257 sets, set observation counts of 128 and 129 with empty sets between, T = 257 tracks, M = 4097 members
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import scale_shapes as ss
+    for name in ("sets_257", "counts", "tracks_257", "members_4097"):
+        sc = ss.SCENES[name]()
+        off = np.cumsum([0] + [len(f) for f in sc["feats"]])
+        sets_of = np.searchsorted(off, sc["members"], side="right") - 1
+        tr = api.Tracks(sc["start"], sets_of, sc["members"] - off[sets_of], None, 0, 0, 0)
+        feats = []
+        for f in sc["feats"]:
+            r = np.zeros(len(f), api.FEATURE_DTYPE)
+            r["x"], r["y"] = f[:, 0], f[:, 1]
+            feats.append(r)
+        T = len(sc["start"]) - 1
+        tp = api.TrackPoints(sc["X0"], np.zeros(T, np.float32), np.zeros(T, np.float32), np.diff(sc["start"]).astype(np.int32), sc["status"],
+                             sc["mask"], None, None)
+        _, _, rep = api.bundle_adjust(feats, tr, tp, sc["cams"], sc["poses"], sc["fixed"].astype(bool), loss="huber", loss_scale=2.0,
+                                      max_iters=2, cg_max_iters=50, scale_set=int(np.flatnonzero(sc["fixed"] == 0)[0]), scale_axis=2)
+        print("scale bundle", name, rep, flush=True)
+        out = api.global_positioning(feats, tr, sc["cams"], sc["R"], np.ones(len(feats), bool), max_iters=2, cg_max_iters=50)
+        print("scale positioning", name, out[-1], flush=True)
+    Rt, pairs, Rp, nf, _ = ss.GRAPHS["sets_257_hub"]()
+    tv = np.zeros(len(pairs), api.TWO_VIEW_DTYPE)
+    tv["R"], tv["n_front"], tv["n_inliers"] = np.asarray(Rp, np.float32), nf, nf
+    out = api.rotation_averaging(257, pairs, tv, max_iters=2, cg_max_iters=50, min_inliers=0)
+    print("scale rotations", out[-1], flush=True)
