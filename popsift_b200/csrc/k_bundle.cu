@@ -1,7 +1,7 @@
 // Bundle adjustment, hand-written for sm_90a: ps_bundle_adjust (contract in include/popsift_b200_bundle.h).  The
 // per-observation math is in k_bundle.h (built on k_triangulate.h), the scan and the radix sort in k_scan.h.
 //
-// One workspace from the matcher's pool, all launches on one stream.  Setup (once per call):
+// One workspace (workspace.h), all launches on one stream.  Setup (once per call):
 //   ba_check_kernel     one thread per member: the checks of ps_triangulate_tracks' ray pass (a flag read back before any
 //                       output is written), each member's set and pixel
 //   ba_flag_kernel      one thread per track: the used flag of each member; an exclusive scan numbers the used observations
@@ -24,10 +24,10 @@
 // CTA sums are xor butterflies within warps and the warps in index order; a thread's share is summed in index order;
 // no floating-point atomics, so two identical calls give identical bytes.
 #include "k_bundle.h"
-#include "k_match_common.h"
 #include "k_scan.h"
 #include "ps_internal.h"
 #include "popsift_b200_bundle.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <cmath>
@@ -42,8 +42,6 @@ constexpr int kT = 256;                 // threads of the per-member / per-track
 constexpr int kCamT = 128;              // threads of a per-set CTA
 constexpr int kCgT = 256;               // threads of the single-CTA CG kernels
 constexpr unsigned kFull = 0xffffffffu;
-
-unsigned blocks_for(long long n, long long per) { return (unsigned)((n + per - 1) / per); }
 
 // one set's pose and intrinsics, and its role: active = free with a used observation; held = the index (3 + axis) of a
 // held translation component, or -1
@@ -647,53 +645,40 @@ int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const
     // observation (sized by M, the bound), per track and per set
     const long long n_part = std::max<long long>(blocks_for(std::max(T, 1), kT), 1);
     const int nbr = (int)blocks_for(std::max(M, 1), kRadixTile);
-    size_t o = 0;
-    auto take = [&](size_t bytes) { const size_t r = o; o = align_up(o + bytes, 256); return r; };
-    const size_t o_feat = take((size_t)S * sizeof(void*)), o_off = take(off.size() * sizeof(int32_t));
-    const size_t plan_bytes = o;
-    const size_t o_stat = take(sizeof(BaStat)), o_cg = take(sizeof(BaCg)), o_step = take(sizeof(BaStep));
-    const size_t o_mset = take((size_t)M * 4), o_mxy = take((size_t)M * 8), o_upos = take(((size_t)M + 1) * 4);
-    const size_t o_part = take(8ull * scan_partials(std::max<long long>({(long long)M + 1, 256ll * nbr, (long long)S + 1})));
-    const size_t o_umem = take((size_t)M * 4), o_utrack = take((size_t)M * 4), o_uset = take((size_t)M * 4);
-    const size_t o_la = take((size_t)M * 4), o_lb = take((size_t)M * 4), o_hist = take(4ull * 256 * nbr);
-    const size_t o_obs = take((size_t)M * sizeof(BaObs));
-    const size_t o_pts = take((size_t)T * sizeof(BaPoint)), o_X = take((size_t)T * 24), o_Xn = take((size_t)T * 24);
-    const size_t o_cpart = take((size_t)n_part * 8), o_ppart = take((size_t)n_part * 8);
-    const size_t o_cstart = take(((size_t)S + 1) * 4), o_sys = take((size_t)S * sizeof(BaCamSys));
-    const size_t o_cams = take((size_t)S * sizeof(BaCam)), o_camn = take((size_t)S * sizeof(BaCam));
-    std::vector<uint8_t> plan(plan_bytes, 0);
-    if (S > 0) std::memcpy(plan.data() + o_feat, feat, (size_t)S * sizeof(void*));
-    std::memcpy(plan.data() + o_off, off.data(), off.size() * sizeof(int32_t));
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, o, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (bundle)"; cudaGetLastError(); return -1; }
-    auto fail = [&](const char* msg) { cudaGetLastError(); cudaFreeAsync(ws, st); *err = msg; return -1; };
-    auto sync_read = [&](void* dst, const void* src, size_t bytes) {
-        return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st) == cudaSuccess && cudaStreamSynchronize(st) == cudaSuccess;
-    };
-    if (!upload_plan(ws, plan, st)) return fail("bundle: plan upload failed");
-    BaStat* stat = reinterpret_cast<BaStat*>(ws + o_stat);
-    BaCg* d_cg = reinterpret_cast<BaCg*>(ws + o_cg);
-    BaStep* d_step = reinterpret_cast<BaStep*>(ws + o_step);
-    int32_t* mset = reinterpret_cast<int32_t*>(ws + o_mset);
-    float2* mxy = reinterpret_cast<float2*>(ws + o_mxy);
-    int32_t* upos = reinterpret_cast<int32_t*>(ws + o_upos);
-    int32_t* cstart = reinterpret_cast<int32_t*>(ws + o_cstart);
-    double* X = reinterpret_cast<double*>(ws + o_X);
-    double* Xn = reinterpret_cast<double*>(ws + o_Xn);
-    BaCam* d_cur = reinterpret_cast<BaCam*>(ws + o_cams);
-    BaCam* d_nxt = reinterpret_cast<BaCam*>(ws + o_camn);
-    double* cpart = reinterpret_cast<double*>(ws + o_cpart);
-    double* ppart = reinterpret_cast<double*>(ws + o_ppart);
-    if (cudaMemsetAsync(stat, 0, sizeof(BaStat), st) != cudaSuccess) return fail("bundle: memset failed");
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (bundle)", "bundle: plan upload failed");
+    const size_t o_feat = ws.put(feat, (size_t)S * sizeof(void*)), o_off = ws.put(off.data(), off.size() * sizeof(int32_t));
+    const size_t o_stat = ws.take(sizeof(BaStat)), o_cg = ws.take(sizeof(BaCg)), o_step = ws.take(sizeof(BaStep));
+    const size_t o_mset = ws.take((size_t)M * 4), o_mxy = ws.take((size_t)M * 8), o_upos = ws.take(((size_t)M + 1) * 4);
+    const size_t o_part = ws.take(8ull * scan_partials(std::max<long long>({(long long)M + 1, 256ll * nbr, (long long)S + 1})));
+    const size_t o_umem = ws.take((size_t)M * 4), o_utrack = ws.take((size_t)M * 4), o_uset = ws.take((size_t)M * 4);
+    const size_t o_la = ws.take((size_t)M * 4), o_lb = ws.take((size_t)M * 4), o_hist = ws.take(4ull * 256 * nbr);
+    const size_t o_obs = ws.take((size_t)M * sizeof(BaObs));
+    const size_t o_pts = ws.take((size_t)T * sizeof(BaPoint)), o_X = ws.take((size_t)T * 24), o_Xn = ws.take((size_t)T * 24);
+    const size_t o_cpart = ws.take((size_t)n_part * 8), o_ppart = ws.take((size_t)n_part * 8);
+    const size_t o_cstart = ws.take(((size_t)S + 1) * 4), o_sys = ws.take((size_t)S * sizeof(BaCamSys));
+    const size_t o_cams = ws.take((size_t)S * sizeof(BaCam)), o_camn = ws.take((size_t)S * sizeof(BaCam));
+    if (!ws.alloc(err)) return -1;
+    BaStat* stat = ws.at<BaStat>(o_stat);
+    BaCg* d_cg = ws.at<BaCg>(o_cg);
+    BaStep* d_step = ws.at<BaStep>(o_step);
+    int32_t* mset = ws.at<int32_t>(o_mset);
+    float2* mxy = ws.at<float2>(o_mxy);
+    int32_t* upos = ws.at<int32_t>(o_upos);
+    int32_t* part = ws.at<int32_t>(o_part);
+    int32_t* cstart = ws.at<int32_t>(o_cstart);
+    double* X = ws.at<double>(o_X);
+    double* Xn = ws.at<double>(o_Xn);
+    BaCam* d_cur = ws.at<BaCam>(o_cams);
+    BaCam* d_nxt = ws.at<BaCam>(o_camn);
+    double* cpart = ws.at<double>(o_cpart);
+    double* ppart = ws.at<double>(o_ppart);
+    if (cudaMemsetAsync(stat, 0, sizeof(BaStat), st) != cudaSuccess) return ws.fail("bundle: memset failed", err);
     const long long n_items = std::max<long long>(M, (long long)T + 1);
-    ba_check_kernel<<<blocks_for(n_items, kT), kT, 0, st>>>(track_start, T, members, M, reinterpret_cast<const int32_t*>(ws + o_off), S,
-                                                            reinterpret_cast<const ps_feature* const*>(ws + o_feat), mset, mxy, &stat->bad);
+    ba_check_kernel<<<blocks_for(n_items, kT), kT, 0, st>>>(track_start, T, members, M, ws.at<const int32_t>(o_off), S,
+                                                            ws.at<const ps_feature* const>(o_feat), mset, mxy, &stat->bad);
     BaStat h{};
-    if (!sync_read(&h, stat, sizeof(h))) return fail("bundle: read-back failed");
+    if (!read_back(&h, stat, sizeof(h), st)) return ws.fail("bundle: read-back failed", err);
     if (h.bad) {
-        cudaFreeAsync(ws, st);
         *bad = true;
         return 1;
     }
@@ -701,14 +686,14 @@ int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const
     BaArgs A{};
     A.start = track_start;
     A.upos = upos;
-    A.umem = reinterpret_cast<const int32_t*>(ws + o_umem);
-    A.utrack = reinterpret_cast<const int32_t*>(ws + o_utrack);
-    A.uset = reinterpret_cast<const int32_t*>(ws + o_uset);
+    A.umem = ws.at<const int32_t>(o_umem);
+    A.utrack = ws.at<const int32_t>(o_utrack);
+    A.uset = ws.at<const int32_t>(o_uset);
     A.cstart = cstart;
     A.mxy = mxy;
-    A.obs = reinterpret_cast<BaObs*>(ws + o_obs);
-    A.pts = reinterpret_cast<BaPoint*>(ws + o_pts);
-    A.sys = reinterpret_cast<BaCamSys*>(ws + o_sys);
+    A.obs = ws.at<BaObs>(o_obs);
+    A.pts = ws.at<BaPoint>(o_pts);
+    A.sys = ws.at<BaCamSys>(o_sys);
     A.cg = d_cg;
     A.n_tracks = T;
     A.n_sets = S;
@@ -716,27 +701,26 @@ int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const
     A.s2 = prm.loss_scale * prm.loss_scale;
     int launches = 1;
     ba_flag_kernel<<<blocks_for(std::max(T, 1), kT), kT, 0, st>>>(track_start, T, M, points, obs_mask, upos);
-    launches += 1 + scan_exclusive(upos, (long long)M + 1, reinterpret_cast<int32_t*>(ws + o_part), &stat->n_obs, st);
-    if (cudaMemsetAsync(cstart, 0, ((size_t)S + 1) * 4, st) != cudaSuccess) return fail("bundle: memset failed");
-    ba_compact_kernel<<<blocks_for(std::max(T, 1), kT), kT, 0, st>>>(A, mset, points, reinterpret_cast<int32_t*>(ws + o_umem),
-                                                                     reinterpret_cast<int32_t*>(ws + o_utrack),
-                                                                     reinterpret_cast<int32_t*>(ws + o_uset), cstart, X, stat);
-    launches += 1 + scan_exclusive(cstart, (long long)S + 1, reinterpret_cast<int32_t*>(ws + o_part), &stat->pad_, st);
-    if (!sync_read(&h, stat, sizeof(h))) return fail("bundle: read-back failed");
+    launches += 1 + scan_exclusive(upos, (long long)M + 1, part, &stat->n_obs, st);
+    if (cudaMemsetAsync(cstart, 0, ((size_t)S + 1) * 4, st) != cudaSuccess) return ws.fail("bundle: memset failed", err);
+    ba_compact_kernel<<<blocks_for(std::max(T, 1), kT), kT, 0, st>>>(A, mset, points, ws.at<int32_t>(o_umem), ws.at<int32_t>(o_utrack),
+                                                                     ws.at<int32_t>(o_uset), cstart, X, stat);
+    launches += 1 + scan_exclusive(cstart, (long long)S + 1, part, &stat->pad_, st);
+    if (!read_back(&h, stat, sizeof(h), st)) return ws.fail("bundle: read-back failed", err);
     const int U = h.n_obs;
     std::vector<int32_t> cs(S + 1);
-    if (!sync_read(cs.data(), cstart, cs.size() * 4)) return fail("bundle: read-back failed");
-    int32_t* la = reinterpret_cast<int32_t*>(ws + o_la);
-    int32_t* lb = reinterpret_cast<int32_t*>(ws + o_lb);
+    if (!read_back(cs.data(), cstart, cs.size() * 4, st)) return ws.fail("bundle: read-back failed", err);
+    int32_t* la = ws.at<int32_t>(o_la);
+    int32_t* lb = ws.at<int32_t>(o_lb);
     if (U > 0) {
         ba_iota_kernel<<<blocks_for(U, kT), kT, 0, st>>>(la, U);
         int bits = 0;
         while (bits < 31 && ((S - 1) >> bits) != 0) ++bits;
         const int nb = (int)blocks_for(U, kRadixTile);
-        int32_t* hist = reinterpret_cast<int32_t*>(ws + o_hist);
+        int32_t* hist = ws.at<int32_t>(o_hist);
         for (int p = 0; p < (bits + 7) / 8; ++p) {
             radix_hist_kernel<<<nb, kRadixT, 0, st>>>(la, U, SetKey{A.uset}, 8 * p, hist, nb);
-            launches += 1 + scan_exclusive(hist, 256ll * nb, reinterpret_cast<int32_t*>(ws + o_part), &stat->pad_, st);
+            launches += 1 + scan_exclusive(hist, 256ll * nb, part, &stat->pad_, st);
             radix_scatter_kernel<<<nb, kRadixT, 0, st>>>(la, lb, U, SetKey{A.uset}, 8 * p, hist, nb);
             ++launches;
             std::swap(la, lb);
@@ -749,9 +733,8 @@ int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const
         n_free += bc[i].active;
         if (i == prm.scale_set && !fixed[i]) bc[i].held = 3 + prm.scale_axis;
     }
-    std::vector<uint8_t> cam_bytes(S * sizeof(BaCam));
-    if (S > 0) std::memcpy(cam_bytes.data(), bc.data(), cam_bytes.size());
-    if (!upload_plan(d_cur, cam_bytes, st)) return fail("bundle: camera upload failed");
+    ws.stage(o_cams, bc.data(), (size_t)S * sizeof(BaCam));
+    if (!ws.upload()) return ws.fail("bundle: camera upload failed", err);
 
     ps_bundle_report rep{};
     rep.n_obs = U;
@@ -772,7 +755,7 @@ int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const
         ba_cost_kernel<<<nt, kT, 0, st>>>(A, d_cur, X, cpart);
         ba_reduce_kernel<<<1, kCgT, 0, st>>>(A, cpart, nullptr, (int)n_part, d_step);
         launches += 2;
-        if (!sync_read(&step, d_step, sizeof(step))) return fail("bundle: read-back failed");
+        if (!read_back(&step, d_step, sizeof(step), st)) return ws.fail("bundle: read-back failed", err);
         rep.initial_cost = rep.final_cost = step.cost;
         if (!std::isfinite(step.cost)) {
             rep.termination = PS_BA_NONFINITE_START;
@@ -804,7 +787,7 @@ int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const
                 ba_cost_kernel<<<nt, kT, 0, st>>>(A, d_nxt, Xn, cpart);
                 ba_reduce_kernel<<<1, kCgT, 0, st>>>(A, cpart, ppart, (int)n_part, d_step);
                 launches += 4;
-                if (!sync_read(&step, d_step, sizeof(step))) return fail("bundle: read-back failed");
+                if (!read_back(&step, d_step, sizeof(step), st)) return ws.fail("bundle: read-back failed", err);
                 rep.iterations += 1;
                 rep.cg_iterations += step.cg_iters;
                 const double nc = step.cost;
@@ -831,9 +814,8 @@ int run_bundle_adjust(int n_sets, const int32_t* n_feat, const ps_feature* const
     }
     finish_outputs(write_points);
     std::vector<BaCam> fin(S);
-    if (S > 0 && !sync_read(fin.data(), d_cur, S * sizeof(BaCam))) return fail("bundle: read-back failed");
+    if (S > 0 && !read_back(fin.data(), d_cur, S * sizeof(BaCam), st)) return ws.fail("bundle: read-back failed", err);
     const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     for (int i = 0; i < S; ++i) {
         ps_rigid r;

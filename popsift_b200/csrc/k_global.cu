@@ -25,10 +25,10 @@
 // Sums are xor butterflies within warps and the warps in index order, partials summed by one CTA in index order; no
 // floating-point atomics, so two identical calls give identical bytes.
 #include "k_global.h"
-#include "k_match_common.h"
 #include "k_scan.h"
 #include "ps_internal.h"
 #include "popsift_b200_global.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <cmath>
@@ -45,8 +45,6 @@ constexpr int kNodeT = 128;             // threads of a per-camera-node CTA
 constexpr int kRedT = 256;              // threads of the single-CTA kernels
 constexpr double kDeg = 3.141592653589793 / 180.0;
 constexpr int kMaxDoublings = 20;       // positioning: the longest step tried is 2^20 times the solve's
-
-unsigned blocks_for(long long n, long long per) { return (unsigned)((n + per - 1) / per); }
 
 struct GlCg {
     double rz, rr0, tol2, alpha, beta;
@@ -497,11 +495,6 @@ __global__ void __launch_bounds__(kT) gp_out_kernel(const double* __restrict__ p
     for (int c = 0; c < 3; ++c) X[3 * t + c] = tpart[t] ? scale * pos[3 * t + c] : 0.0;
 }
 
-// workspace layout helper
-struct Carve {
-    size_t o = 0;
-    size_t take(size_t bytes) { const size_t r = o; o = align_up(o + bytes, 256); return r; }
-};
 
 } // namespace
 
@@ -524,8 +517,7 @@ int run_rotation_averaging(int n_sets, int n_pairs, const int32_t* pairs, const 
     *err = nullptr;
     const int S = n_sets, P = n_pairs;
     std::vector<ps_two_view> tv(P);
-    if (P > 0 && (cudaMemcpyAsync(tv.data(), d_two_view, (size_t)P * sizeof(ps_two_view), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-                  cudaStreamSynchronize(st) != cudaSuccess)) {
+    if (P > 0 && !read_back(tv.data(), d_two_view, (size_t)P * sizeof(ps_two_view), st)) {
         cudaGetLastError();
         *err = "rotation averaging: read-back failed";
         return -1;
@@ -613,42 +605,28 @@ int run_rotation_averaging(int n_sets, int n_pairs, const int32_t* pairs, const 
             if (used[p]) { list[fill[pairs[2 * p]]++] = p; list[fill[pairs[2 * p + 1]]++] = p; }
         const int nbp = (int)blocks_for(P, kT);
         const size_t npart = gl_part_count(S, 0, S);
-        Carve cv;
-        const size_t o_cg = cv.take(sizeof(GlCg)), o_step = cv.take(sizeof(GlStep));
-        const size_t o_Rp = cv.take((size_t)P * 72), o_ends = cv.take((size_t)P * 8), o_used = cv.take(P), o_W = cv.take((size_t)P * 8);
-        const size_t o_g = cv.take((size_t)P * 24), o_err = cv.take((size_t)P * 4), o_cpart = cv.take((size_t)nbp * 8);
-        const size_t o_off = cv.take(off.size() * 4), o_list = cv.take(std::max<size_t>(list.size(), 1) * 4);
-        const size_t o_R = cv.take((size_t)S * 72), o_reg = cv.take(S), o_vec = cv.take((size_t)S * 5 * 24), o_D = cv.take((size_t)S * 8);
-        const size_t o_part = cv.take(npart * 8);
-        std::vector<uint8_t> plan(o_part, 0);
         std::vector<int2> ends(P);
         for (int p = 0; p < P; ++p) ends[p] = make_int2(pairs[2 * p], pairs[2 * p + 1]);
-        std::memcpy(plan.data() + o_Rp, Rp.data(), Rp.size() * 8);
-        if (P) std::memcpy(plan.data() + o_ends, ends.data(), (size_t)P * 8);
-        if (P) std::memcpy(plan.data() + o_used, used.data(), P);
-        std::memcpy(plan.data() + o_off, off.data(), off.size() * 4);
-        if (!list.empty()) std::memcpy(plan.data() + o_list, list.data(), list.size() * 4);
-        std::memcpy(plan.data() + o_R, R.data(), R.size() * 8);
-        std::memcpy(plan.data() + o_reg, reg.data(), S);
-        cudaMemPool_t pool = match_pool(err);
-        if (!pool) return -1;
-        uint8_t* ws = nullptr;
-        if (cudaMallocFromPoolAsync(&ws, cv.o, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (rotation averaging)"; cudaGetLastError(); return -1; }
-        auto fail = [&](const char* msg) { cudaGetLastError(); cudaFreeAsync(ws, st); *err = msg; return -1; };
-        auto sync_read = [&](void* dst, const void* src, size_t bytes) {
-            return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st) == cudaSuccess && cudaStreamSynchronize(st) == cudaSuccess;
-        };
-        if (!upload_plan(ws, plan, st)) return fail("rotation averaging: upload failed");
-        GlStep* d_step = reinterpret_cast<GlStep*>(ws + o_step);
+        // everything before the partials is uploaded, the solver's state and the per-pair outputs as zeros
+        Workspace ws(st, "cudaMallocFromPoolAsync failed (rotation averaging)", "rotation averaging: upload failed");
+        const size_t o_cg = ws.put(nullptr, sizeof(GlCg)), o_step = ws.put(nullptr, sizeof(GlStep));
+        const size_t o_Rp = ws.put(Rp.data(), (size_t)P * 72), o_ends = ws.put(ends.data(), (size_t)P * 8), o_used = ws.put(used.data(), P);
+        const size_t o_W = ws.put(nullptr, (size_t)P * 8), o_g = ws.put(nullptr, (size_t)P * 24), o_err = ws.put(nullptr, (size_t)P * 4);
+        const size_t o_cpart = ws.put(nullptr, (size_t)nbp * 8), o_off = ws.put(off.data(), off.size() * 4);
+        const size_t o_list = ws.put(list.data(), list.size() * 4), o_R = ws.put(R.data(), (size_t)S * 72), o_reg = ws.put(reg.data(), S);
+        const size_t o_vec = ws.put(nullptr, (size_t)S * 5 * 24), o_D = ws.put(nullptr, (size_t)S * 8);
+        const size_t o_part = ws.take(npart * 8);
+        if (!ws.alloc(err)) return -1;
+        GlStep* d_step = ws.at<GlStep>(o_step);
         RaArgs A{};
-        A.Rp = reinterpret_cast<const double*>(ws + o_Rp);
-        A.ends = reinterpret_cast<const int2*>(ws + o_ends);
-        A.used = ws + o_used;
-        A.R = reinterpret_cast<double*>(ws + o_R);
-        A.W = reinterpret_cast<double*>(ws + o_W);
-        A.g = reinterpret_cast<double*>(ws + o_g);
-        A.err = reinterpret_cast<float*>(ws + o_err);
-        A.cpart = reinterpret_cast<double*>(ws + o_cpart);
+        A.Rp = ws.at<const double>(o_Rp);
+        A.ends = ws.at<const int2>(o_ends);
+        A.used = ws.at<uint8_t>(o_used);
+        A.R = ws.at<double>(o_R);
+        A.W = ws.at<double>(o_W);
+        A.g = ws.at<double>(o_g);
+        A.err = ws.at<float>(o_err);
+        A.cpart = ws.at<double>(o_cpart);
         A.n_pairs = P;
         A.loss = prm.loss;
         const double s = prm.loss_scale * kDeg;
@@ -658,21 +636,21 @@ int run_rotation_averaging(int n_sets, int n_pairs, const int32_t* pairs, const 
         G.nP = 0;
         G.N = S;
         G.root = root;
-        G.off_c = reinterpret_cast<const int32_t*>(ws + o_off);
-        G.list_c = reinterpret_cast<const int32_t*>(ws + o_list);
+        G.off_c = ws.at<const int32_t>(o_off);
+        G.list_c = ws.at<const int32_t>(o_list);
         G.ends = A.ends;
         G.W = A.W;
         G.g = A.g;
-        double* vec = reinterpret_cast<double*>(ws + o_vec);
+        double* vec = ws.at<double>(o_vec);
         G.x = vec;
         G.r = vec + 3 * (size_t)S;
         G.z = vec + 6 * (size_t)S;
         G.p = vec + 9 * (size_t)S;
         G.q = vec + 12 * (size_t)S;
-        G.D = reinterpret_cast<double*>(ws + o_D);
-        G.part = reinterpret_cast<double*>(ws + o_part);
-        G.cg = reinterpret_cast<GlCg*>(ws + o_cg);
-        const uint8_t* d_reg = ws + o_reg;
+        G.D = ws.at<double>(o_D);
+        G.part = ws.at<double>(o_part);
+        G.cg = ws.at<GlCg>(o_cg);
+        const uint8_t* d_reg = ws.at<const uint8_t>(o_reg);
         GlStep step{};
         auto lin = [&]() {
             gl_rot_lin_kernel<<<nbp, kT, 0, st>>>(A);
@@ -686,20 +664,19 @@ int run_rotation_averaging(int n_sets, int n_pairs, const int32_t* pairs, const 
             launches += gl_solve(G, prm.cg_max_iters, prm.cg_tol, st);
             gl_rot_update_kernel<<<1, kRedT, 0, st>>>(A, G, d_reg, S, d_step);
             ++launches;
-            if (!sync_read(&step, d_step, sizeof(step))) return fail("rotation averaging: read-back failed");
+            if (!read_back(&step, d_step, sizeof(step), st)) return ws.fail("rotation averaging: read-back failed", err);
             if (it == 0) rep.initial_cost = step.cost;
             rep.iterations += 1;
             rep.cg_iterations += step.cg_iters;
             lin();
             if (step.max_step < step_tol) { rep.termination = PS_RA_STEP_TOL; break; }
         }
-        if (!sync_read(&step, d_step, sizeof(step))) return fail("rotation averaging: read-back failed");
+        if (!read_back(&step, d_step, sizeof(step), st)) return ws.fail("rotation averaging: read-back failed", err);
         if (prm.max_iters == 0) rep.initial_cost = step.cost;
         rep.final_cost = step.cost;
-        if (!sync_read(R.data(), A.R, R.size() * 8) || (P > 0 && !sync_read(perr.data(), A.err, (size_t)P * 4)))
-            return fail("rotation averaging: read-back failed");
+        if (!read_back(R.data(), A.R, R.size() * 8, st) || (P > 0 && !read_back(perr.data(), A.err, (size_t)P * 4, st)))
+            return ws.fail("rotation averaging: read-back failed", err);
         const cudaError_t e = cudaGetLastError();
-        cudaFreeAsync(ws, st);
         if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     }
     for (int i = 0; i < S; ++i) {
@@ -731,86 +708,71 @@ int run_global_positioning(int n_sets, const int32_t* n_feat, const ps_feature* 
     const int nbm = (int)blocks_for(std::max(M, 1), kT);
     const int nbr = (int)blocks_for(std::max(M, 1), kRadixTile);
     const size_t npart = gl_part_count(S, T, N);
-    Carve cv;
-    const size_t o_feat = cv.take((size_t)S * sizeof(void*)), o_off = cv.take(off.size() * 4), o_cams = cv.take((size_t)S * sizeof(TriCam));
-    const size_t o_reg = cv.take(std::max(S, 1));
-    const size_t plan_bytes = cv.o;
-    const size_t o_stat = cv.take(sizeof(GpStat)), o_cg = cv.take(sizeof(GlCg)), o_step = cv.take(sizeof(GlStep));
-    const size_t o_mset = cv.take((size_t)M * 4), o_ray = cv.take((size_t)M * 24), o_obs = cv.take(M), o_ends = cv.take((size_t)M * 8);
-    const size_t o_key = cv.take((size_t)M * 4), o_la = cv.take((size_t)M * 4), o_lb = cv.take((size_t)M * 4);
-    const size_t o_W = cv.take((size_t)M * 8), o_g = cv.take((size_t)M * 24), o_cpart = cv.take((size_t)nbm * 8);
-    const size_t o_hist = cv.take(4ull * 256 * nbr);
-    const size_t o_spart = cv.take(4ull * scan_partials(std::max<long long>(256ll * nbr, (long long)S + 1)));
-    const size_t o_cstart = cv.take(((size_t)S + 1) * 4), o_tpart = cv.take(std::max(T, 1));
-    const size_t o_pos = cv.take((size_t)N * 24), o_vec = cv.take((size_t)N * 5 * 24), o_D = cv.take((size_t)N * 8);
-    const size_t o_part = cv.take(npart * 8);
-    std::vector<uint8_t> plan(plan_bytes, 0);
-    if (S > 0) {
-        std::memcpy(plan.data() + o_feat, feat, (size_t)S * sizeof(void*));
-        std::memcpy(plan.data() + o_cams, tc.data(), (size_t)S * sizeof(TriCam));
-        std::memcpy(plan.data() + o_reg, registered, S);
-    }
-    std::memcpy(plan.data() + o_off, off.data(), off.size() * 4);
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, cv.o, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (positioning)"; cudaGetLastError(); return -1; }
-    auto fail = [&](const char* msg) { cudaGetLastError(); cudaFreeAsync(ws, st); *err = msg; return -1; };
-    auto sync_read = [&](void* dst, const void* src, size_t bytes) {
-        return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st) == cudaSuccess && cudaStreamSynchronize(st) == cudaSuccess;
-    };
-    if (!upload_plan(ws, plan, st)) return fail("positioning: plan upload failed");
-    GpStat* stat = reinterpret_cast<GpStat*>(ws + o_stat);
-    GlStep* d_step = reinterpret_cast<GlStep*>(ws + o_step);
-    int32_t* mset = reinterpret_cast<int32_t*>(ws + o_mset);
-    double* ray = reinterpret_cast<double*>(ws + o_ray);
-    uint8_t* obs = ws + o_obs;
-    int2* ends = reinterpret_cast<int2*>(ws + o_ends);
-    int32_t* key = reinterpret_cast<int32_t*>(ws + o_key);
-    int32_t* cstart = reinterpret_cast<int32_t*>(ws + o_cstart);
-    uint8_t* tpart = ws + o_tpart;
-    double* pos = reinterpret_cast<double*>(ws + o_pos);
-    double* W = reinterpret_cast<double*>(ws + o_W);
-    double* g = reinterpret_cast<double*>(ws + o_g);
-    double* cpart = reinterpret_cast<double*>(ws + o_cpart);
-    if (cudaMemsetAsync(stat, 0, sizeof(GpStat), st) != cudaSuccess) return fail("positioning: memset failed");
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (positioning)", "positioning: plan upload failed");
+    const size_t o_feat = ws.put(feat, (size_t)S * sizeof(void*)), o_off = ws.put(off.data(), off.size() * 4);
+    const size_t o_cams = ws.put(tc.data(), (size_t)S * sizeof(TriCam)), o_reg = ws.put(S > 0 ? registered : nullptr, std::max(S, 1));
+    const size_t o_stat = ws.take(sizeof(GpStat)), o_cg = ws.take(sizeof(GlCg)), o_step = ws.take(sizeof(GlStep));
+    const size_t o_mset = ws.take((size_t)M * 4), o_ray = ws.take((size_t)M * 24), o_obs = ws.take(M), o_ends = ws.take((size_t)M * 8);
+    const size_t o_key = ws.take((size_t)M * 4), o_la = ws.take((size_t)M * 4), o_lb = ws.take((size_t)M * 4);
+    const size_t o_W = ws.take((size_t)M * 8), o_g = ws.take((size_t)M * 24), o_cpart = ws.take((size_t)nbm * 8);
+    const size_t o_hist = ws.take(4ull * 256 * nbr);
+    const size_t o_spart = ws.take(4ull * scan_partials(std::max<long long>(256ll * nbr, (long long)S + 1)));
+    const size_t o_cstart = ws.take(((size_t)S + 1) * 4), o_tpart = ws.take(std::max(T, 1));
+    const size_t o_pos = ws.take((size_t)N * 24), o_vec = ws.take((size_t)N * 5 * 24), o_D = ws.take((size_t)N * 8);
+    const size_t o_part = ws.take(npart * 8);
+    if (!ws.alloc(err)) return -1;
+    GpStat* stat = ws.at<GpStat>(o_stat);
+    GlStep* d_step = ws.at<GlStep>(o_step);
+    int32_t* mset = ws.at<int32_t>(o_mset);
+    double* ray = ws.at<double>(o_ray);
+    uint8_t* obs = ws.at<uint8_t>(o_obs);
+    int2* ends = ws.at<int2>(o_ends);
+    int32_t* key = ws.at<int32_t>(o_key);
+    int32_t* spart = ws.at<int32_t>(o_spart);
+    int32_t* cstart = ws.at<int32_t>(o_cstart);
+    uint8_t* tpart = ws.at<uint8_t>(o_tpart);
+    double* pos = ws.at<double>(o_pos);
+    double* W = ws.at<double>(o_W);
+    double* g = ws.at<double>(o_g);
+    double* cpart = ws.at<double>(o_cpart);
+    if (cudaMemsetAsync(stat, 0, sizeof(GpStat), st) != cudaSuccess) return ws.fail("positioning: memset failed", err);
     const long long n_items = std::max<long long>(M, (long long)T + 1);
-    gp_check_kernel<<<blocks_for(n_items, kT), kT, 0, st>>>(track_start, T, members, M, reinterpret_cast<const int32_t*>(ws + o_off), S,
-                                                            reinterpret_cast<const ps_feature* const*>(ws + o_feat),
-                                                            reinterpret_cast<const TriCam*>(ws + o_cams), ws + o_reg, mset, ray, obs, &stat->bad);
+    gp_check_kernel<<<blocks_for(n_items, kT), kT, 0, st>>>(track_start, T, members, M, ws.at<const int32_t>(o_off), S,
+                                                            ws.at<const ps_feature* const>(o_feat), ws.at<const TriCam>(o_cams),
+                                                            ws.at<const uint8_t>(o_reg), mset, ray, obs, &stat->bad);
     GpStat h{};
-    if (!sync_read(&h, stat, sizeof(h))) return fail("positioning: read-back failed");
+    if (!read_back(&h, stat, sizeof(h), st)) return ws.fail("positioning: read-back failed", err);
     if (h.bad) {
-        cudaFreeAsync(ws, st);
         *bad = true;
         return 1;
     }
     int launches = 1;
     if (cudaMemsetAsync(cstart, 0, ((size_t)S + 1) * 4, st) != cudaSuccess || cudaMemsetAsync(pos, 0, (size_t)N * 24, st) != cudaSuccess)
-        return fail("positioning: memset failed");
+        return ws.fail("positioning: memset failed", err);
     if (T > 0) {
         gp_track_kernel<<<blocks_for(T, kT), kT, 0, st>>>(track_start, T, S, mset, obs, ends, key, cstart, tpart, stat);
         ++launches;
     }
-    launches += scan_exclusive(cstart, (long long)S + 1, reinterpret_cast<int32_t*>(ws + o_spart), &stat->pad_, st);
-    int32_t* la = reinterpret_cast<int32_t*>(ws + o_la);
-    int32_t* lb = reinterpret_cast<int32_t*>(ws + o_lb);
+    launches += scan_exclusive(cstart, (long long)S + 1, spart, &stat->pad_, st);
+    int32_t* la = ws.at<int32_t>(o_la);
+    int32_t* lb = ws.at<int32_t>(o_lb);
     if (M > 0) {
         gp_iota_kernel<<<nbm, kT, 0, st>>>(la, M);
         ++launches;
         int bits = 0;
         while (bits < 31 && (S >> bits) != 0) ++bits;      // keys 0 .. S
-        int32_t* hist = reinterpret_cast<int32_t*>(ws + o_hist);
+        int32_t* hist = ws.at<int32_t>(o_hist);
         for (int p = 0; p < (bits + 7) / 8; ++p) {
             radix_hist_kernel<<<nbr, kRadixT, 0, st>>>(la, M, KeyOf{key}, 8 * p, hist, nbr);
-            launches += 1 + scan_exclusive(hist, 256ll * nbr, reinterpret_cast<int32_t*>(ws + o_spart), &stat->pad_, st);
+            launches += 1 + scan_exclusive(hist, 256ll * nbr, spart, &stat->pad_, st);
             radix_scatter_kernel<<<nbr, kRadixT, 0, st>>>(la, lb, M, KeyOf{key}, 8 * p, hist, nbr);
             ++launches;
             std::swap(la, lb);
         }
     }
     std::vector<int32_t> cs(S + 1);
-    if (!sync_read(&h, stat, sizeof(h)) || !sync_read(cs.data(), cstart, cs.size() * 4)) return fail("positioning: read-back failed");
+    if (!read_back(&h, stat, sizeof(h), st) || !read_back(cs.data(), cstart, cs.size() * 4, st))
+        return ws.fail("positioning: read-back failed", err);
     int root = -1, n_cams = 0;
     for (int i = 0; i < S; ++i) {
         positioned[i] = cs[i + 1] > cs[i];
@@ -837,15 +799,15 @@ int run_global_positioning(int n_sets, const int32_t* n_feat, const ps_feature* 
         G.ends = ends;
         G.W = W;
         G.g = g;
-        double* vec = reinterpret_cast<double*>(ws + o_vec);
+        double* vec = ws.at<double>(o_vec);
         G.x = vec;
         G.r = vec + 3 * (size_t)N;
         G.z = vec + 6 * (size_t)N;
         G.p = vec + 9 * (size_t)N;
         G.q = vec + 12 * (size_t)N;
-        G.D = reinterpret_cast<double*>(ws + o_D);
-        G.part = reinterpret_cast<double*>(ws + o_part);
-        G.cg = reinterpret_cast<GlCg*>(ws + o_cg);
+        G.D = ws.at<double>(o_D);
+        G.part = ws.at<double>(o_part);
+        G.cg = ws.at<GlCg>(o_cg);
         const double s2 = prm.loss_scale * prm.loss_scale;
         const unsigned nbn3 = blocks_for(3ll * N, kT);
         GlStep step{};
@@ -855,27 +817,27 @@ int run_global_positioning(int n_sets, const int32_t* n_feat, const ps_feature* 
             gp_lin_kernel<false><<<nbm, kT, 0, st>>>(M, S, key, ends, ray, pos, prm.loss, s2, W, g, cpart);
             gl_cost_kernel<<<1, kRedT, 0, st>>>(cpart, nbm, G.cg, d_step);
             launches += 3;
-            return sync_read(&step, d_step, sizeof(step));
+            return read_back(&step, d_step, sizeof(step), st);
         };
         gp_lin_kernel<true><<<nbm, kT, 0, st>>>(M, S, key, ends, ray, pos, prm.loss, s2, W, g, cpart);
         ++launches;
         launches += gl_solve(G, prm.cg_max_iters, prm.cg_tol, st);
-        if (!move_lin(1.0)) return fail("positioning: read-back failed");
+        if (!move_lin(1.0)) return ws.fail("positioning: read-back failed", err);
         rep.initial_cost = rep.final_cost = step.cost;
         rep.cg_iterations = step.cg_iters;
         rep.termination = PS_GP_MAX_ITERS;
         double cost = step.cost;
         for (int it = 0; it < prm.max_iters; ++it) {
             launches += gl_solve(G, prm.cg_max_iters, prm.cg_tol, st);
-            if (!move_lin(1.0)) return fail("positioning: read-back failed");
+            if (!move_lin(1.0)) return ws.fail("positioning: read-back failed", err);
             rep.iterations += 1;
             rep.cg_iterations += step.cg_iters;
             // the step lengthened: 2^k x for k = 1 .. kMaxDoublings while the cost keeps decreasing
             double best = step.cost, a = 1.0;
             for (int k = 0; k < kMaxDoublings; ++k) {
-                if (!move_lin(a)) return fail("positioning: read-back failed");
+                if (!move_lin(a)) return ws.fail("positioning: read-back failed", err);
                 if (!(step.cost < best)) {
-                    if (!move_lin(-a)) return fail("positioning: read-back failed");
+                    if (!move_lin(-a)) return ws.fail("positioning: read-back failed", err);
                     break;
                 }
                 best = step.cost;
@@ -887,7 +849,7 @@ int run_global_positioning(int n_sets, const int32_t* n_feat, const ps_feature* 
             if (small) { rep.termination = PS_GP_FUNCTION_TOL; break; }
         }
         rep.final_cost = cost;
-        if (S > 0 && !sync_read(cpos.data(), pos, cpos.size() * 8)) return fail("positioning: read-back failed");
+        if (S > 0 && !read_back(cpos.data(), pos, cpos.size() * 8, st)) return ws.fail("positioning: read-back failed", err);
         double ss = 0.0;
         for (int i = 0; i < S; ++i)
             if (positioned[i])
@@ -898,9 +860,8 @@ int run_global_positioning(int n_sets, const int32_t* n_feat, const ps_feature* 
         gp_out_kernel<<<blocks_for(T, kT), kT, 0, st>>>(pos + 3 * (size_t)S, tpart, T, scale, X_out);
         ++launches;
     }
-    if (cudaStreamSynchronize(st) != cudaSuccess) return fail("positioning: synchronise failed");
+    if (cudaStreamSynchronize(st) != cudaSuccess) return ws.fail("positioning: synchronise failed", err);
     const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     for (int i = 0; i < S; ++i) {
         ps_rigid r;

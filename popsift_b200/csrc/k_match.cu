@@ -36,12 +36,12 @@
 #include "k_match_plan.h"
 #include "k_guided.h"
 #include "tma_util.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
-#include <mutex>
 #include <vector>
 
 namespace psb {
@@ -637,56 +637,6 @@ int match_choice(int flags)
     return flags ? flags : env;
 }
 
-// the library's own memory pool of the current device: a pool gives freed memory back to the OS at the next
-// synchronisation unless told to keep it, and mapping the workspace again on every call costs more than the matching
-// itself (the application's default pool is left alone)
-cudaMemPool_t match_pool(const char** err)
-{
-    static std::mutex mu;
-    static cudaMemPool_t pools[64] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); *err = "cudaGetDevice failed (matcher)"; return nullptr; }
-    std::lock_guard<std::mutex> g(mu);
-    if (!pools[dev]) {
-        cudaMemPoolProps props = {};
-        props.allocType = cudaMemAllocationTypePinned;
-        props.handleTypes = cudaMemHandleTypeNone;
-        props.location.type = cudaMemLocationTypeDevice;
-        props.location.id = dev;
-        if (cudaMemPoolCreate(&pools[dev], &props) != cudaSuccess) { cudaGetLastError(); pools[dev] = nullptr; *err = "cudaMemPoolCreate failed (matcher)"; return nullptr; }
-        unsigned long long keep = kMatchPoolKeep;                              // freed workspace that stays mapped
-        cudaMemPoolSetAttribute(pools[dev], cudaMemPoolAttrReleaseThreshold, &keep);
-    }
-    return pools[dev];
-}
-
-// Copies the plan's metadata to `dst` on `st` from a page-locked staging buffer of the current device, so that the copy
-// is queued without waiting (a pageable source would hold the host until the transfer is done).  The buffer is reused
-// by the next call once the event recorded after this copy has completed.
-bool upload_plan(void* dst, const std::vector<uint8_t>& host, cudaStream_t st)
-{
-    struct Stage { uint8_t* buf = nullptr; size_t cap = 0; cudaEvent_t done = nullptr; };
-    static std::mutex mu;
-    static Stage stages[64];
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); return false; }
-    std::lock_guard<std::mutex> g(mu);
-    Stage& s = stages[dev];
-    if (!s.done && cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); s.done = nullptr; return false; }
-    if (cudaEventSynchronize(s.done) != cudaSuccess) { cudaGetLastError(); return false; }     // the previous copy has left the buffer
-    if (s.cap < host.size()) {
-        if (s.buf) cudaFreeHost(s.buf);
-        s.buf = nullptr; s.cap = 0;
-        const size_t cap = std::max<size_t>(align_up(host.size(), 1 << 16), 1 << 16);
-        if (cudaHostAlloc(reinterpret_cast<void**>(&s.buf), cap, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); s.buf = nullptr; return false; }
-        s.cap = cap;
-    }
-    std::memcpy(s.buf, host.data(), host.size());
-    if (cudaMemcpyAsync(dst, s.buf, host.size(), cudaMemcpyHostToDevice, st) != cudaSuccess) { cudaGetLastError(); return false; }
-    if (cudaEventRecord(s.done, st) != cudaSuccess) { cudaGetLastError(); return false; }
-    return true;
-}
-
 size_t match_workspace_cap()
 {
     static const size_t cap = [] {
@@ -741,45 +691,36 @@ int run_batch(const ps_descriptor* const* sets, const ps_feature* const* feat, c
     // once; one workspace for the largest group's planes, reused in turn
     struct Meta { size_t sets, csets, pairs, gpair, items; };
     std::vector<Meta> meta;
-    size_t meta_bytes = 0, planes = 0;
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (matcher workspace)", "matcher: plan upload failed");
+    size_t planes = 0;
     for (const MatchGroup& g : plan.groups) {
         if (g.rows > 0x7fffff80) { *err = "matcher: a group of pairs has more than 2^31 rows"; return -1; }
-        Meta m;
-        m.sets = meta_bytes;  meta_bytes = align_up(meta_bytes + g.sets.size() * sizeof(SplitSet), 16);
-        m.csets = meta_bytes; meta_bytes = align_up(meta_bytes + (guided ? g.sets.size() * sizeof(MatchCoordSet) : 0), 16);
-        m.pairs = meta_bytes; meta_bytes = align_up(meta_bytes + g.pairs.size() * sizeof(RerankPair), 16);
-        m.gpair = meta_bytes; meta_bytes = align_up(meta_bytes + (guided ? g.pairs.size() * sizeof(int32_t) : 0), 16);
-        m.items = meta_bytes; meta_bytes = align_up(meta_bytes + g.items.size() * sizeof(MatchItem), 16);
-        meta.push_back(m);
-        planes = std::max(planes, g.bytes());
-    }
-    meta_bytes = align_up(meta_bytes, 1024);
-    std::vector<uint8_t> host(meta_bytes);
-    for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
-        const MatchGroup& g = plan.groups[gi];
-        SplitSet* hs = reinterpret_cast<SplitSet*>(host.data() + meta[gi].sets);
-        MatchCoordSet* hc = reinterpret_cast<MatchCoordSet*>(host.data() + meta[gi].csets);
+        std::vector<SplitSet> hs(g.sets.size());
+        std::vector<MatchCoordSet> hc(guided ? g.sets.size() : 0);
         for (size_t k = 0; k < g.sets.size(); ++k) {
             const int si = g.sets[k].set;
             hs[k] = {sets[si], n_desc[si], (int32_t)g.sets[k].row};
             if (guided) hc[k] = {feat[si], rev[si], n_desc[si], (int32_t)g.sets[k].row};
         }
-        RerankPair* hp = reinterpret_cast<RerankPair*>(host.data() + meta[gi].pairs);
-        int32_t* hg = reinterpret_cast<int32_t*>(host.data() + meta[gi].gpair);
+        std::vector<RerankPair> hp(g.pairs.size());
+        std::vector<int32_t> hg(guided ? g.pairs.size() : 0);
         for (size_t k = 0; k < g.pairs.size(); ++k) {
             const MatchGroupPair& gp = g.pairs[k];
             const int l = pairs[2 * gp.pair], r = pairs[2 * gp.pair + 1];
             hp[k] = {sets[l], sets[r], plan.out_row[gp.pair], gp.row, gp.cand, n_desc[r], gp.chunks};
             if (guided) hg[k] = gp.pair;
         }
-        if (!g.items.empty()) std::memcpy(host.data() + meta[gi].items, g.items.data(), g.items.size() * sizeof(MatchItem));
+        Meta m;
+        m.sets = ws.put(hs.data(), hs.size() * sizeof(SplitSet), 16);
+        m.csets = ws.put(hc.data(), hc.size() * sizeof(MatchCoordSet), 16);
+        m.pairs = ws.put(hp.data(), hp.size() * sizeof(RerankPair), 16);
+        m.gpair = ws.put(hg.data(), hg.size() * sizeof(int32_t), 16);
+        m.items = ws.put(g.items.data(), g.items.size() * sizeof(MatchItem), 16);
+        meta.push_back(m);
+        planes = std::max(planes, g.bytes());
     }
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    // stream-ordered, so nothing blocks
-    if (cudaMallocFromPoolAsync(&ws, meta_bytes + planes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (matcher workspace)"; cudaGetLastError(); return -1; }
-    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "matcher: plan upload failed"; return -1; }
+    const size_t o_planes = ws.take(planes, 1024);
+    if (!ws.alloc(err)) return -1;
     static_assert(TC_SMEM + 1024 <= 227 * 1024, "matcher shared memory");
     static_assert(TC_SMEM + 1024 + BN * sizeof(float2) <= 227 * 1024, "guided matcher shared memory");
     static_assert(BM == kMatchTile && BN == kMatchTile && kCand == kMatchCand, "planner and kernel tile sizes");
@@ -789,28 +730,27 @@ int run_batch(const ps_descriptor* const* sets, const ps_feature* const* feat, c
     const int sms = sm_count();
     for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
         const MatchGroup& g = plan.groups[gi];
-        const RerankPair* d_pairs = reinterpret_cast<const RerankPair*>(ws + meta[gi].pairs);
+        const RerankPair* d_pairs = ws.at<const RerankPair>(meta[gi].pairs);
         int32_t* cand = nullptr;
         if (!g.items.empty()) {
             const int rows = (int)g.rows;
-            float* hi = reinterpret_cast<float*>(ws + meta_bytes);
-            float* lo = reinterpret_cast<float*>(ws + meta_bytes + (size_t)rows * 512);
-            float* norm = reinterpret_cast<float*>(ws + meta_bytes + (size_t)rows * 1024);
-            cand = reinterpret_cast<int32_t*>(ws + meta_bytes + (size_t)rows * row_bytes);
+            uint8_t* plane = ws.at<uint8_t>(o_planes);
+            float* hi = reinterpret_cast<float*>(plane);
+            float* lo = reinterpret_cast<float*>(plane + (size_t)rows * 512);
+            float* norm = reinterpret_cast<float*>(plane + (size_t)rows * 1024);
+            cand = reinterpret_cast<int32_t*>(plane + (size_t)rows * row_bytes);
             // one tensor map per plane: a left tile and a right tile are both row offsets into it
             CUtensorMap m_hi, m_lo;
-            if (!make_tmap_2d(&m_hi, hi, 128, rows, 512, KB, BM, true) || !make_tmap_2d(&m_lo, lo, 128, rows, 512, KB, BM, true)) {
-                cudaFreeAsync(ws, st); *err = "cuTensorMapEncodeTiled failed (matcher)"; return -1;
-            }
-            match_split_kernel<<<(rows + 3) / 4, 128, 0, st>>>(reinterpret_cast<const SplitSet*>(ws + meta[gi].sets), (int)g.sets.size(),
-                                                               rows, hi, lo, norm);
+            if (!make_tmap_2d(&m_hi, hi, 128, rows, 512, KB, BM, true) || !make_tmap_2d(&m_lo, lo, 128, rows, 512, KB, BM, true))
+                return ws.fail("cuTensorMapEncodeTiled failed (matcher)", err);
+            match_split_kernel<<<(rows + 3) / 4, 128, 0, st>>>(ws.at<const SplitSet>(meta[gi].sets), (int)g.sets.size(), rows, hi, lo, norm);
             const int n_items = (int)g.items.size();
-            const MatchItem* d_items = reinterpret_cast<const MatchItem*>(ws + meta[gi].items);
+            const MatchItem* d_items = ws.at<const MatchItem>(meta[gi].items);
             if constexpr (guided) {
-                float2* pos = reinterpret_cast<float2*>(ws + meta_bytes + (size_t)rows * kMatchRowBytes);
-                launch_match_coords(reinterpret_cast<const MatchCoordSet*>(ws + meta[gi].csets), (int)g.sets.size(), rows, pos, st);
+                float2* pos = reinterpret_cast<float2*>(plane + (size_t)rows * kMatchRowBytes);
+                launch_match_coords(ws.at<const MatchCoordSet>(meta[gi].csets), (int)g.sets.size(), rows, pos, st);
                 match_tc_guided_kernel<MODE><<<std::min(sms, n_items), TC_THREADS, TC_SMEM, st>>>(
-                    m_hi, m_lo, norm, pos, models, reinterpret_cast<const int32_t*>(ws + meta[gi].gpair), t2, d_items, n_items, cand);
+                    m_hi, m_lo, norm, pos, models, ws.at<const int32_t>(meta[gi].gpair), t2, d_items, n_items, cand);
                 ++launches;
             } else {
                 match_tc_kernel<<<std::min(sms, n_items), TC_THREADS, TC_SMEM, st>>>(m_hi, m_lo, norm, d_items, n_items, cand);
@@ -820,7 +760,6 @@ int run_batch(const ps_descriptor* const* sets, const ps_feature* const* feat, c
         match_rerank_kernel<<<(unsigned)((g.left_rows + 3) / 4), 128, 0, st>>>(d_pairs, (int)g.pairs.size(), g.left_rows, cand, out);
         ++launches;
     }
-    cudaFreeAsync(ws, st);
     return launches;
 }
 

@@ -1,12 +1,11 @@
 // What both brute-force matchers (k_match.cu: float32 descriptors, k_match_u8.cu: 8-bit descriptors) share: the
-// mbarrier / TMA / wgmma-descriptor helpers of their persistent tensor-core kernels, the matcher's memory pool and the
-// upload of a plan's metadata.
+// mbarrier / TMA / wgmma-descriptor helpers of their persistent tensor-core kernels and the guided matchers' position
+// helpers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstddef>
 #include <cstdint>
-#include <vector>
 
 #include "popsift_b200.h"
 
@@ -50,8 +49,6 @@ __device__ __forceinline__ void bulk_copy(void* dst, const void* src, unsigned b
                  :: "r"(s32(dst)), "l"(src), "r"(bytes), "r"(s32(bar)) : "memory");
 }
 
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 // Guided matching: the pixel position of every pooled row of a group, (feat[rev[i]].xpos, .ypos) for the set's row i and
 // NaN for padding rows (k_match.cu), so that the kernels' epilogues read a right tile's 128 points as one 1 KB block.
 struct MatchCoordSet { const ps_feature* f; const int32_t* rev; int32_t n; int32_t row; };
@@ -70,12 +67,5 @@ __device__ __forceinline__ void load_model(float (&m)[9], const float* __restric
 #pragma unroll
     for (int k = 0; k < 9; ++k) m[k] = __ldg(p + k);
 }
-
-// the library's own memory pool of the current device (k_match.cu): a pool gives freed memory back to the OS at the next
-// synchronisation unless told to keep it, and mapping the workspace again on every call costs more than the matching
-// itself (the application's default pool is left alone)
-cudaMemPool_t match_pool(const char** err);
-// Copies a plan's metadata to `dst` on `st` from a page-locked staging buffer of the current device (k_match.cu)
-bool upload_plan(void* dst, const std::vector<uint8_t>& host, cudaStream_t st);
 
 } // namespace psb

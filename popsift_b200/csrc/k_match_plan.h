@@ -27,7 +27,7 @@ constexpr size_t kMatchU8RowBytes = 128 + 4;    // pooled 8-bit row and its norm
 // guided matching adds the row's pixel position (float2) to either
 constexpr size_t kMatchGuidedRowBytes = kMatchRowBytes + 8;
 constexpr size_t kMatchU8GuidedRowBytes = kMatchU8RowBytes + 8;
-// freed workspace the matcher's memory pool keeps mapped, and the default cap of one group's workspace
+// freed workspace the library's memory pool (workspace.cu) keeps mapped, and the default cap of one group's workspace
 // (POPSIFT_B200_MATCH_WS=bytes overrides the cap)
 constexpr size_t kMatchPoolKeep = (size_t)1 << 30;
 

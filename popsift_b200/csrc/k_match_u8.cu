@@ -34,6 +34,7 @@
 #include "k_match_plan.h"
 #include "k_guided.h"
 #include "tma_util.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <climits>
@@ -554,31 +555,19 @@ int run_u8_batch(const uint8_t* const* sets, const ps_feature* const* feat, cons
     // once; one workspace for the largest group's plane, reused in turn
     struct Meta { size_t sets, csets, pairs, gpair, items; };
     std::vector<Meta> meta;
-    size_t meta_bytes = 0, planes = 0;
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (u8 matcher workspace)", "u8 matcher: plan upload failed");
+    size_t planes = 0;
     for (const MatchGroup& g : plan.groups) {
         if (g.rows > 0x7fffff80) { *err = "matcher: a group of pairs has more than 2^31 rows"; return -1; }
-        Meta m;
-        m.sets = meta_bytes;  meta_bytes = align_up(meta_bytes + g.sets.size() * sizeof(PackSet), 16);
-        m.csets = meta_bytes; meta_bytes = align_up(meta_bytes + (guided ? g.sets.size() * sizeof(MatchCoordSet) : 0), 16);
-        m.pairs = meta_bytes; meta_bytes = align_up(meta_bytes + g.pairs.size() * sizeof(FinalPair), 16);
-        m.gpair = meta_bytes; meta_bytes = align_up(meta_bytes + (guided ? g.pairs.size() * sizeof(int32_t) : 0), 16);
-        m.items = meta_bytes; meta_bytes = align_up(meta_bytes + g.items.size() * sizeof(MatchItem), 16);
-        meta.push_back(m);
-        planes = std::max(planes, g.bytes());
-    }
-    meta_bytes = align_up(meta_bytes, 1024);
-    std::vector<uint8_t> host(meta_bytes);
-    for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
-        const MatchGroup& g = plan.groups[gi];
-        PackSet* hs = reinterpret_cast<PackSet*>(host.data() + meta[gi].sets);
-        MatchCoordSet* hc = reinterpret_cast<MatchCoordSet*>(host.data() + meta[gi].csets);
+        std::vector<PackSet> hs(g.sets.size());
+        std::vector<MatchCoordSet> hc(guided ? g.sets.size() : 0);
         for (size_t k = 0; k < g.sets.size(); ++k) {
             const int si = g.sets[k].set;
             hs[k] = {sets[si], n_desc[si], (int32_t)g.sets[k].row};
             if (guided) hc[k] = {feat[si], rev[si], n_desc[si], (int32_t)g.sets[k].row};
         }
-        FinalPair* hp = reinterpret_cast<FinalPair*>(host.data() + meta[gi].pairs);
-        int32_t* hg = reinterpret_cast<int32_t*>(host.data() + meta[gi].gpair);
+        std::vector<FinalPair> hp(g.pairs.size());
+        std::vector<int32_t> hg(guided ? g.pairs.size() : 0);
         for (size_t k = 0; k < g.pairs.size(); ++k) {
             const MatchGroupPair& gp = g.pairs[k];
             const int l = pairs[2 * gp.pair], r = pairs[2 * gp.pair + 1];
@@ -587,14 +576,17 @@ int run_u8_batch(const uint8_t* const* sets, const ps_feature* const* feat, cons
             hp[k] = {plan.out_row[gp.pair], gp.row, gp.cand, (int32_t)a_row, n_desc[r], gp.chunks, 0};
             if (guided) hg[k] = gp.pair;
         }
-        if (!g.items.empty()) std::memcpy(host.data() + meta[gi].items, g.items.data(), g.items.size() * sizeof(MatchItem));
+        Meta m;
+        m.sets = ws.put(hs.data(), hs.size() * sizeof(PackSet), 16);
+        m.csets = ws.put(hc.data(), hc.size() * sizeof(MatchCoordSet), 16);
+        m.pairs = ws.put(hp.data(), hp.size() * sizeof(FinalPair), 16);
+        m.gpair = ws.put(hg.data(), hg.size() * sizeof(int32_t), 16);
+        m.items = ws.put(g.items.data(), g.items.size() * sizeof(MatchItem), 16);
+        meta.push_back(m);
+        planes = std::max(planes, g.bytes());
     }
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    // stream-ordered, so nothing blocks
-    if (cudaMallocFromPoolAsync(&ws, meta_bytes + planes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (u8 matcher workspace)"; cudaGetLastError(); return -1; }
-    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "u8 matcher: plan upload failed"; return -1; }
+    const size_t o_plane = ws.take(planes, 1024);
+    if (!ws.alloc(err)) return -1;
     // the guided kernel's ring stages carry a right tile's 128 positions next to the tile
     constexpr size_t smem_bytes = U8_SMEM + (guided ? (size_t)STAGES * BN * sizeof(float2) : 0);
     static_assert(smem_bytes + 1024 <= 227 * 1024, "u8 matcher shared memory");
@@ -607,28 +599,25 @@ int run_u8_batch(const uint8_t* const* sets, const ps_feature* const* feat, cons
     const int sms = sm_count();
     for (size_t gi = 0; gi < plan.groups.size(); ++gi) {
         const MatchGroup& g = plan.groups[gi];
-        const FinalPair* d_pairs = reinterpret_cast<const FinalPair*>(ws + meta[gi].pairs);
+        const FinalPair* d_pairs = ws.at<const FinalPair>(meta[gi].pairs);
         const int32_t* nkey = nullptr;
         const int4* cand = nullptr;
         if (!g.items.empty()) {
             const int rows = (int)g.rows;
-            uint8_t* plane = ws + meta_bytes;
-            int32_t* nk = reinterpret_cast<int32_t*>(ws + meta_bytes + (size_t)rows * 128);
-            int4* cd = reinterpret_cast<int4*>(ws + meta_bytes + (size_t)rows * row_bytes);
+            uint8_t* plane = ws.at<uint8_t>(o_plane);
+            int32_t* nk = reinterpret_cast<int32_t*>(plane + (size_t)rows * 128);
+            int4* cd = reinterpret_cast<int4*>(plane + (size_t)rows * row_bytes);
             // one tensor map: a left tile and a right tile are both row offsets into it
             CUtensorMap tm;
-            if (!make_tmap_2d(&tm, plane, 128, rows, 128, 128, BM, true)) {
-                cudaFreeAsync(ws, st); *err = "cuTensorMapEncodeTiled failed (u8 matcher)"; return -1;
-            }
-            match_u8_pack_kernel<<<(rows + 3) / 4, 128, 0, st>>>(reinterpret_cast<const PackSet*>(ws + meta[gi].sets), (int)g.sets.size(),
-                                                                 rows, plane, nk);
+            if (!make_tmap_2d(&tm, plane, 128, rows, 128, 128, BM, true)) return ws.fail("cuTensorMapEncodeTiled failed (u8 matcher)", err);
+            match_u8_pack_kernel<<<(rows + 3) / 4, 128, 0, st>>>(ws.at<const PackSet>(meta[gi].sets), (int)g.sets.size(), rows, plane, nk);
             const int n_items = (int)g.items.size();
-            const MatchItem* d_items = reinterpret_cast<const MatchItem*>(ws + meta[gi].items);
+            const MatchItem* d_items = ws.at<const MatchItem>(meta[gi].items);
             if constexpr (guided) {
-                float2* pos = reinterpret_cast<float2*>(ws + meta_bytes + (size_t)rows * kMatchU8RowBytes);
-                launch_match_coords(reinterpret_cast<const MatchCoordSet*>(ws + meta[gi].csets), (int)g.sets.size(), rows, pos, st);
+                float2* pos = reinterpret_cast<float2*>(plane + (size_t)rows * kMatchU8RowBytes);
+                launch_match_coords(ws.at<const MatchCoordSet>(meta[gi].csets), (int)g.sets.size(), rows, pos, st);
                 match_u8_guided_kernel<MODE><<<std::min(sms, n_items), TC_THREADS, smem_bytes, st>>>(
-                    tm, nk, pos, models, reinterpret_cast<const int32_t*>(ws + meta[gi].gpair), t2, d_items, n_items, cd);
+                    tm, nk, pos, models, ws.at<const int32_t>(meta[gi].gpair), t2, d_items, n_items, cd);
                 ++launches;
             } else {
                 match_u8_kernel<<<std::min(sms, n_items), TC_THREADS, smem_bytes, st>>>(tm, nk, d_items, n_items, cd);
@@ -641,7 +630,6 @@ int run_u8_batch(const uint8_t* const* sets, const ps_feature* const* feat, cons
         else match_u8_finalize_kernel<<<blocks, 128, 0, st>>>(d_pairs, (int)g.pairs.size(), g.left_rows, nkey, cand, out);
         ++launches;
     }
-    cudaFreeAsync(ws, st);
     return launches;
 }
 

@@ -3,7 +3,7 @@
 // scoring loop, the selection rule and the refit's normal matrix are ps_verify_batch's (k_verify_common.h); the
 // calibrated math is in k_pose_solve.h.
 //
-// One workspace from the matcher's pool, all launches on one stream:
+// One workspace (workspace.h), all launches on one stream:
 //   1. pose_calibrate_kernel  one CTA per pair: the calibrated float4 rows.
 //   2. pose_solve_kernel      one lane per minimal sample, in double: the five-point solver; ten slots per sample, count
 //                             0 (valid) or -1 (invalid).  The 5 x 9 and 10 x 20 eliminations are in local memory.
@@ -18,6 +18,7 @@
 #include "k_verify_common.h"
 #include "k_verify_sample.h"
 #include "ps_internal.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <cmath>
@@ -305,42 +306,29 @@ int run_relative_pose_batch(int n_pairs, const float* corr, const int32_t* corr_
     }
     if (solve.size() > 0x7fffffffu) { *err = "ps_relative_pose_batch: too many work items"; return -1; }
     const size_t n_hyp = (size_t)n_pairs * nh;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off = align_up(off + bytes, 256); return o; };
-    const size_t o_pairs = take(vp.size() * sizeof(VPair)), o_cams = take(pc.size() * sizeof(PCam));
-    const size_t o_solve = take(solve.size() * sizeof(PSolveItem));
-    const size_t meta_bytes = off;
-    const size_t o_pts = take((size_t)total_rows * sizeof(float4)), o_models = take(n_hyp * 9 * sizeof(float));
-    const size_t o_counts = take(n_hyp * sizeof(int32_t)), o_dense = take(n_hyp * sizeof(int32_t));
-    const size_t o_nvalid = take((size_t)n_pairs * sizeof(int32_t));
-    std::vector<uint8_t> host(meta_bytes);
-    std::memcpy(host.data() + o_pairs, vp.data(), vp.size() * sizeof(VPair));
-    std::memcpy(host.data() + o_cams, pc.data(), pc.size() * sizeof(PCam));
-    std::memcpy(host.data() + o_solve, solve.data(), solve.size() * sizeof(PSolveItem));
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, off, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (pose workspace)"; cudaGetLastError(); return -1; }
-    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "pose: plan upload failed"; return -1; }
-    const VPair* d_pairs = reinterpret_cast<const VPair*>(ws + o_pairs);
-    const PCam* d_cams = reinterpret_cast<const PCam*>(ws + o_cams);
-    float4* d_pts = reinterpret_cast<float4*>(ws + o_pts);
-    float* hyp_models = reinterpret_cast<float*>(ws + o_models);
-    int32_t* hyp_counts = reinterpret_cast<int32_t*>(ws + o_counts);
-    int32_t* d_dense = reinterpret_cast<int32_t*>(ws + o_dense);
-    int32_t* d_nvalid = reinterpret_cast<int32_t*>(ws + o_nvalid);
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (pose workspace)", "pose: plan upload failed");
+    const size_t o_pairs = ws.put(vp.data(), vp.size() * sizeof(VPair)), o_cams = ws.put(pc.data(), pc.size() * sizeof(PCam));
+    const size_t o_solve = ws.put(solve.data(), solve.size() * sizeof(PSolveItem));
+    const size_t o_pts = ws.take((size_t)total_rows * sizeof(float4)), o_models = ws.take(n_hyp * 9 * sizeof(float));
+    const size_t o_counts = ws.take(n_hyp * sizeof(int32_t)), o_dense = ws.take(n_hyp * sizeof(int32_t));
+    const size_t o_nvalid = ws.take((size_t)n_pairs * sizeof(int32_t));
+    if (!ws.alloc(err)) return -1;
+    const VPair* d_pairs = ws.at<const VPair>(o_pairs);
+    const PCam* d_cams = ws.at<const PCam>(o_cams);
+    float4* d_pts = ws.at<float4>(o_pts);
+    float* hyp_models = ws.at<float>(o_models);
+    int32_t* hyp_counts = ws.at<int32_t>(o_counts);
+    int32_t* d_dense = ws.at<int32_t>(o_dense);
+    int32_t* d_nvalid = ws.at<int32_t>(o_nvalid);
     pose_calibrate_kernel<<<n_pairs, kCalThreads, 0, st>>>(d_pairs, d_cams, reinterpret_cast<const float4*>(corr), d_pts);
-    pose_solve_kernel<<<(unsigned)solve.size(), kPoseSolveThreads, 0, st>>>(reinterpret_cast<const PSolveItem*>(ws + o_solve), d_pairs, d_pts,
+    pose_solve_kernel<<<(unsigned)solve.size(), kPoseSolveThreads, 0, st>>>(ws.at<const PSolveItem>(o_solve), d_pairs, d_pts,
                                                                             ns, prm.seed, hyp_models, hyp_counts);
     pose_compact_kernel<<<n_pairs, kCompactThreads, 0, st>>>(nh, hyp_counts, d_dense, d_nvalid);
     int launches = 3;
     // the scoring plan needs each pair's number of valid hypotheses
     std::vector<int32_t> nv(n_pairs);
-    if (cudaMemcpyAsync(nv.data(), d_nvalid, (size_t)n_pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess) {
-        const cudaError_t e = cudaGetLastError();
-        cudaFreeAsync(ws, st);
-        *err = cudaGetErrorString(e);
+    if (!read_back(nv.data(), d_nvalid, (size_t)n_pairs * sizeof(int32_t), st)) {
+        *err = cudaGetErrorString(cudaGetLastError());
         return -1;
     }
     double work = 0.0;
@@ -356,16 +344,12 @@ int run_relative_pose_batch(int n_pairs, const float* corr, const int32_t* corr_
             for (int k0 = 0; k0 < nv[p]; k0 += kScoreThreads)
                 score.push_back({p, k0, c0, (int)std::min<long long>((long long)c0 + chunk, n_corr[p])});
     }
-    if (score.size() > 0x7fffffffu) { cudaFreeAsync(ws, st); *err = "ps_relative_pose_batch: too many work items"; return -1; }
-    uint8_t* sws = nullptr;
+    if (score.size() > 0x7fffffffu) { *err = "ps_relative_pose_batch: too many work items"; return -1; }
+    Workspace sws(st, "cudaMallocFromPoolAsync failed (pose score plan)", "pose: plan upload failed");
     if (!score.empty()) {
-        std::vector<uint8_t> sh(score.size() * sizeof(PScoreItem));
-        std::memcpy(sh.data(), score.data(), sh.size());
-        if (cudaMallocFromPoolAsync(&sws, sh.size(), pool, st) != cudaSuccess) {
-            cudaFreeAsync(ws, st); *err = "cudaMallocFromPoolAsync failed (pose score plan)"; cudaGetLastError(); return -1;
-        }
-        if (!upload_plan(sws, sh, st)) { cudaFreeAsync(sws, st); cudaFreeAsync(ws, st); *err = "pose: plan upload failed"; return -1; }
-        pose_score_kernel<<<(unsigned)score.size(), kScoreThreads, 0, st>>>(reinterpret_cast<const PScoreItem*>(sws), d_pairs, d_cams, d_pts, nh,
+        const size_t o_score = sws.put(score.data(), score.size() * sizeof(PScoreItem));
+        if (!sws.alloc(err)) return -1;
+        pose_score_kernel<<<(unsigned)score.size(), kScoreThreads, 0, st>>>(sws.at<const PScoreItem>(o_score), d_pairs, d_cams, d_pts, nh,
                                                                             d_dense, d_nvalid, hyp_models, hyp_counts);
         ++launches;
     }
@@ -377,8 +361,6 @@ int run_relative_pose_batch(int n_pairs, const float* corr, const int32_t* corr_
         ++launches;
     }
     const cudaError_t e = cudaGetLastError();
-    if (sws) cudaFreeAsync(sws, st);
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return launches;
 }

@@ -6,6 +6,7 @@
 #include "k_retrieval.h"
 #include "k_verify_sample.h"
 #include "tma_util.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <cstring>
@@ -350,22 +351,23 @@ int assign_group(const ps_descriptor* const* sets, const int32_t* n_desc, int a,
     return run_match_batch(gs.data(), gn.data(), (int)gs.size(), pairs.data(), b - a, match, flags, st, err);
 }
 
-// Workspace layout of one group: match rows, partial sums and counts, segment sums, metadata
-struct AggWs {
-    int32_t* match; double* part; int32_t* cnt; double* sum; AggItem* items; int32_t* seg_first;
-};
+// The workspace regions of the group of sets [a, b), laid out from the start of the workspace (the groups reuse them in
+// turn): match rows, partial sums and counts, segment sums, metadata
+struct AggWs { size_t rows, match, part, cnt, sum, items, seg_first; };
 
-size_t agg_bytes(size_t rows, size_t items, size_t segs, int k, size_t* off)
+AggWs agg_layout(Workspace& ws, const int32_t* n_desc, int a, int b, size_t segs, int k)
 {
-    size_t o = 0;
-    auto take = [&](size_t bytes) { const size_t r = o; o = align_up(o + bytes, 256); return r; };
-    off[0] = take(rows * 12);
-    off[1] = take(items * k * 128 * sizeof(double));
-    off[2] = take(items * k * sizeof(int32_t));
-    off[3] = take(segs * k * 128 * sizeof(double));
-    off[4] = take(items * sizeof(AggItem));
-    off[5] = take((segs + 1) * sizeof(int32_t));
-    return o;
+    AggWs L{};
+    size_t items = 0;
+    for (int s = a; s < b; ++s) { L.rows += n_desc[s]; items += chunks_of(n_desc[s]); }
+    ws.rewind(0);
+    L.match = ws.take(L.rows * 12);
+    L.part = ws.take(items * k * 128 * sizeof(double));
+    L.cnt = ws.take(items * k * sizeof(int32_t));
+    L.sum = ws.take(segs * k * 128 * sizeof(double));
+    L.items = ws.take(items * sizeof(AggItem));
+    L.seg_first = ws.take((segs + 1) * sizeof(int32_t));
+    return L;
 }
 
 } // namespace
@@ -385,40 +387,36 @@ static void vlad_draw(uint64_t seed, uint32_t N, int k, uint32_t* idx)
     }
 }
 
-// the aggregation of one group on `st`: assignment, items, merge; the group's workspace is ws (agg_bytes)
+// the aggregation of one group on `st`: assignment, items, merge, in the group's regions L of ws
 static int aggregate_group(const ps_descriptor* const* sets, const int32_t* n_desc, int a, int b, const float* centroids, int k,
-                           bool encode, uint8_t* ws, const size_t* off, double* train_sum, long long* train_cnt, int flags,
-                           cudaStream_t st, const char** err, AggPlan* plan_out)
+                           bool encode, Workspace& ws, const AggWs& L, double* train_sum, long long* train_cnt, int flags,
+                           cudaStream_t st, const char** err)
 {
-    int32_t* match = reinterpret_cast<int32_t*>(ws + off[0]);
-    int64_t rows = 0;
-    for (int s = a; s < b; ++s) rows += n_desc[s];
-    int launches = rows > 0 ? assign_group(sets, n_desc, a, b, centroids, k, match, flags, st, err) : 0;
+    int32_t* match = ws.at<int32_t>(L.match);
+    int launches = L.rows > 0 ? assign_group(sets, n_desc, a, b, centroids, k, match, flags, st, err) : 0;
     if (launches < 0) return -1;
     AggPlan plan = agg_plan(sets, n_desc, a, b, match, encode);
     const size_t segs = plan.seg_first.size() - 1;
-    std::vector<uint8_t> host(off[5] - off[4] + (segs + 1) * sizeof(int32_t));
-    std::memcpy(host.data(), plan.items.data(), plan.items.size() * sizeof(AggItem));
-    std::memcpy(host.data() + (off[5] - off[4]), plan.seg_first.data(), (segs + 1) * sizeof(int32_t));
-    if (!upload_plan(ws + off[4], host, st)) { *err = "vlad: plan upload failed"; return -1; }
-    double* part = reinterpret_cast<double*>(ws + off[1]);
-    int32_t* cnt = reinterpret_cast<int32_t*>(ws + off[2]);
+    ws.stage(L.items, plan.items.data(), plan.items.size() * sizeof(AggItem));
+    ws.stage(L.seg_first, plan.seg_first.data(), (segs + 1) * sizeof(int32_t));
+    if (!ws.upload()) { *err = "vlad: plan upload failed"; return -1; }
+    double* part = ws.at<double>(L.part);
+    int32_t* cnt = ws.at<int32_t>(L.cnt);
     if (!plan.items.empty()) {
-        vlad_aggregate_kernel<<<dim3((unsigned)plan.items.size(), k), 128, 0, st>>>(reinterpret_cast<const AggItem*>(ws + off[4]), centroids,
-                                                                                   encode ? 1 : 0, k, part, cnt);
+        vlad_aggregate_kernel<<<dim3((unsigned)plan.items.size(), k), 128, 0, st>>>(ws.at<const AggItem>(L.items), centroids, encode ? 1 : 0,
+                                                                                   k, part, cnt);
         ++launches;
     }
     if (encode) {
         if (segs > 0) {
-            vlad_merge_kernel<<<dim3((unsigned)segs, k), 128, 0, st>>>(reinterpret_cast<const int32_t*>(ws + off[5]), part, cnt, k, 0,
-                                                                      reinterpret_cast<double*>(ws + off[3]), nullptr);
+            vlad_merge_kernel<<<dim3((unsigned)segs, k), 128, 0, st>>>(ws.at<const int32_t>(L.seg_first), part, cnt, k, 0, ws.at<double>(L.sum),
+                                                                      nullptr);
             ++launches;
         }
     } else {
-        vlad_merge_kernel<<<dim3(1, k), 128, 0, st>>>(reinterpret_cast<const int32_t*>(ws + off[5]), part, cnt, k, 1, train_sum, train_cnt);
+        vlad_merge_kernel<<<dim3(1, k), 128, 0, st>>>(ws.at<const int32_t>(L.seg_first), part, cnt, k, 1, train_sum, train_cnt);
         ++launches;
     }
-    if (plan_out) *plan_out = std::move(plan);
     return launches;
 }
 
@@ -434,46 +432,35 @@ int run_vlad_train(const ps_descriptor* const* sets, const int32_t* n_desc, int 
     vlad_draw(seed, (uint32_t)N, k, idx.data());
     std::vector<int64_t> start(n_sets + 1, 0);
     for (int i = 0; i < n_sets; ++i) start[i + 1] = start[i] + n_desc[i];
-    std::vector<uint8_t> src(align_up((size_t)k * sizeof(const float*), 256));
+    std::vector<const float*> src(k);
     for (int c = 0; c < k; ++c) {
         const int s = (int)(std::upper_bound(start.begin(), start.end(), (int64_t)idx[c]) - start.begin()) - 1;
-        const float* p = reinterpret_cast<const float*>(sets[s]) + (size_t)(idx[c] - start[s]) * 128;
-        std::memcpy(src.data() + c * sizeof(const float*), &p, sizeof(p));
+        src[c] = reinterpret_cast<const float*>(sets[s]) + (size_t)(idx[c] - start[s]) * 128;
     }
     const auto groups = set_groups(n_sets, n_desc, [k](int n) { return (size_t)n * 12 + chunks_of(n) * k * (128 * 8 + 4) + 256; });
     // one workspace for the largest group, plus the running sums and counts
-    size_t off[6], ws_bytes = 0;
-    for (const auto& g : groups) {
-        size_t rows = 0, items = 0;
-        for (int s = g.first; s < g.second; ++s) { rows += n_desc[s]; items += chunks_of(n_desc[s]); }
-        ws_bytes = std::max(ws_bytes, agg_bytes(rows, items, 1, k, off));
-    }
-    const size_t o_sum = align_up(ws_bytes, 256), o_cnt = align_up(o_sum + (size_t)k * 128 * 8, 256);
-    const size_t o_src = align_up(o_cnt + (size_t)k * 8, 256);
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, o_src + src.size(), pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (vlad)"; cudaGetLastError(); return -1; }
-    if (!upload_plan(ws + o_src, src, st)) { cudaFreeAsync(ws, st); *err = "vlad: upload failed"; return -1; }
-    vlad_gather_kernel<<<k, 128, 0, st>>>(reinterpret_cast<const float* const*>(ws + o_src), centroids);
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (vlad)", "vlad: upload failed");
+    for (const auto& g : groups) agg_layout(ws, n_desc, g.first, g.second, 1, k);
+    ws.rewind(ws.size());
+    const size_t o_sum = ws.take((size_t)k * 128 * 8), o_cnt = ws.take((size_t)k * 8);
+    const size_t o_src = ws.put(src.data(), src.size() * sizeof(const float*));
+    if (!ws.alloc(err)) return -1;
+    vlad_gather_kernel<<<k, 128, 0, st>>>(ws.at<const float* const>(o_src), centroids);
     int launches = 1;
-    double* sum = reinterpret_cast<double*>(ws + o_sum);
-    long long* cnt = reinterpret_cast<long long*>(ws + o_cnt);
+    double* sum = ws.at<double>(o_sum);
+    long long* cnt = ws.at<long long>(o_cnt);
     for (int it = 0; it < iters; ++it) {
-        if (cudaMemsetAsync(sum, 0, o_src - o_sum, st) != cudaSuccess) { cudaGetLastError(); cudaFreeAsync(ws, st); *err = "vlad: memset failed"; return -1; }
+        if (cudaMemsetAsync(sum, 0, o_src - o_sum, st) != cudaSuccess) return ws.fail("vlad: memset failed", err);
         for (const auto& g : groups) {
-            size_t rows = 0, items = 0;
-            for (int s = g.first; s < g.second; ++s) { rows += n_desc[s]; items += chunks_of(n_desc[s]); }
-            agg_bytes(rows, items, 1, k, off);
-            const int n = aggregate_group(sets, n_desc, g.first, g.second, centroids, k, false, ws, off, sum, cnt, flags, st, err, nullptr);
-            if (n < 0) { cudaFreeAsync(ws, st); return -1; }
+            const AggWs L = agg_layout(ws, n_desc, g.first, g.second, 1, k);
+            const int n = aggregate_group(sets, n_desc, g.first, g.second, centroids, k, false, ws, L, sum, cnt, flags, st, err);
+            if (n < 0) return -1;
             launches += n;
         }
         vlad_update_kernel<<<k, 128, 0, st>>>(sum, cnt, centroids);
         ++launches;
     }
     const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return launches;
 }
@@ -486,36 +473,26 @@ int run_vlad_encode(const ps_descriptor* const* sets, const int32_t* n_desc, int
     const size_t dim = (size_t)k * 128;
     const auto groups = set_groups(n_sets, n_desc, [k](int n) {
         return (size_t)n * 12 + chunks_of(n) * k * (128 * 8 + 4) + (size_t)k * 128 * 8 + 256; });
-    size_t off[6], ws_bytes = 0;
-    for (const auto& g : groups) {
-        size_t rows = 0, items = 0;
-        for (int s = g.first; s < g.second; ++s) { rows += n_desc[s]; items += chunks_of(n_desc[s]); }
-        ws_bytes = std::max(ws_bytes, agg_bytes(rows, items, g.second - g.first, k, off));
-    }
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, ws_bytes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (vlad)"; cudaGetLastError(); return -1; }
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (vlad)", "vlad: plan upload failed");
+    for (const auto& g : groups) agg_layout(ws, n_desc, g.first, g.second, g.second - g.first, k);
+    if (!ws.alloc(err)) return -1;
     int launches = 0;
     size_t row0 = 0;
     for (const auto& g : groups) {
-        size_t rows = 0, items = 0;
-        for (int s = g.first; s < g.second; ++s) { rows += n_desc[s]; items += chunks_of(n_desc[s]); }
         const int segs = g.second - g.first;
-        agg_bytes(rows, items, segs, k, off);
-        const int n = aggregate_group(sets, n_desc, g.first, g.second, centroids, k, true, ws, off, nullptr, nullptr, flags, st, err, nullptr);
-        if (n < 0) { cudaFreeAsync(ws, st); return -1; }
+        const AggWs L = agg_layout(ws, n_desc, g.first, g.second, segs, k);
+        const int n = aggregate_group(sets, n_desc, g.first, g.second, centroids, k, true, ws, L, nullptr, nullptr, flags, st, err);
+        if (n < 0) return -1;
         launches += n;
-        vlad_normalize_kernel<<<segs, 128, 0, st>>>(reinterpret_cast<double*>(ws + off[3]), k, vlad + (size_t)g.first * dim);
+        vlad_normalize_kernel<<<segs, 128, 0, st>>>(ws.at<double>(L.sum), k, vlad + (size_t)g.first * dim);
         ++launches;
-        if (assign && rows > 0) {
-            vlad_assign_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>(reinterpret_cast<const int32_t*>(ws + off[0]), (int)rows, assign + row0);
+        if (assign && L.rows > 0) {
+            vlad_assign_kernel<<<(unsigned)((L.rows + 255) / 256), 256, 0, st>>>(ws.at<const int32_t>(L.match), (int)L.rows, assign + row0);
             ++launches;
         }
-        row0 += rows;
+        row0 += L.rows;
     }
     const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return launches;
 }
@@ -536,35 +513,27 @@ int run_retrieve_pairs(int n, const float* vec, int dim, int m, int32_t* nbr, fl
         for (int bi = b0; bi < std::min(T, b0 + grp_tiles); ++bi)
             for (int bj = mirror ? bi : 0; bj < T; ++bj) gtiles.back().push_back({bi, bj});
     }
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (retrieval)", "retrieval: plan upload failed");
     std::vector<size_t> toff;
-    size_t meta = 0;
-    for (const auto& g : gtiles) { toff.push_back(meta); meta = align_up(meta + g.size() * sizeof(RTile), 256); }
-    std::vector<uint8_t> host(meta);
-    for (size_t q = 0; q < gtiles.size(); ++q) std::memcpy(host.data() + toff[q], gtiles[q].data(), gtiles[q].size() * sizeof(RTile));
+    for (const auto& g : gtiles) toff.push_back(ws.put(g.data(), g.size() * sizeof(RTile)));
     const size_t s_rows = std::min<size_t>((size_t)grp_tiles * kRT, (size_t)n);
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, meta + s_rows * row_bytes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (retrieval)"; cudaGetLastError(); return -1; }
-    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "retrieval: plan upload failed"; return -1; }
+    const size_t o_S = ws.take(s_rows * row_bytes);
+    if (!ws.alloc(err)) return -1;
     CUtensorMap map;
-    if (!make_tmap_2d(&map, vec, dim, n, (size_t)dim * sizeof(float), kRK, kRT, true)) {
-        cudaFreeAsync(ws, st); *err = "cuTensorMapEncodeTiled failed (retrieval)"; return -1;
-    }
+    if (!make_tmap_2d(&map, vec, dim, n, (size_t)dim * sizeof(float), kRK, kRT, true)) return ws.fail("cuTensorMapEncodeTiled failed (retrieval)", err);
     static_assert(kRSmem + kRStages * 8 <= 227 * 1024, "retrieval shared memory");
     cudaFuncSetAttribute(retrieve_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRSmem);
-    float* S = reinterpret_cast<float*>(ws + meta);
+    float* S = ws.at<float>(o_S);
     int launches = 0;
     for (size_t q = 0; q < gtiles.size(); ++q) {
         const int r0 = gtiles[q].front().bi * kRT;
         const int rows = std::min(n, r0 + grp_tiles * kRT) - r0;
-        retrieve_score_kernel<<<(unsigned)gtiles[q].size(), kRThreads, kRSmem, st>>>(map, reinterpret_cast<const RTile*>(ws + toff[q]), n, dim,
-                                                                                    r0, mirror ? 1 : 0, S);
+        retrieve_score_kernel<<<(unsigned)gtiles[q].size(), kRThreads, kRSmem, st>>>(map, ws.at<const RTile>(toff[q]), n, dim, r0,
+                                                                                    mirror ? 1 : 0, S);
         retrieve_topm_kernel<<<rows, kTopThreads, 0, st>>>(S, n, r0, m, nbr, score);
         launches += 2;
     }
     const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return launches;
 }

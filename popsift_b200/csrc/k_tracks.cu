@@ -16,9 +16,9 @@
 //             d_track_of
 // No library sort or scan: both are in k_scan.h.
 #include "ps_internal.h"
-#include "k_match_common.h"
 #include "k_scan.h"
 #include "popsift_b200_tracks.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <cstring>
@@ -32,8 +32,6 @@ constexpr int kT = 256;                 // threads of the element-wise kernels
 constexpr uint32_t kConflict = 0x80000000u;
 
 __device__ __forceinline__ long long gtid() { return (long long)blockIdx.x * blockDim.x + threadIdx.x; }
-
-unsigned blocks_for(long long n, long long per) { return (unsigned)((n + per - 1) / per); }
 
 // ---- union-find
 
@@ -286,38 +284,30 @@ int run_tracks(int n_sets, const int32_t* n_feat, long long n_items, const std::
     // partial sums; then the set offsets, the pair plan and the statistics
     const int nbt = (int)blocks_for(std::max(N, 1), kRadixTile);
     const long long n_hist = 256ll * nbt;
-    const size_t o_parent = 0, o_cnt = align_up(o_parent + 4ull * N, 256), o_va = align_up(o_cnt + 4ull * N, 256);
-    const size_t o_vb = align_up(o_va + 4ull * N, 256), o_key = align_up(o_vb + 4ull * N, 256);
-    const size_t o_hist = align_up(o_key + 8ull * N, 256), o_part = align_up(o_hist + 4ull * n_hist, 256);
-    const size_t o_off = align_up(o_part + 8ull * scan_partials(std::max<long long>({(long long)N, n_hist, 1})), 256);
-    const size_t o_plan = align_up(o_off + 4ull * off.size(), 256), o_stat = align_up(o_plan + plan.size(), 256);
-    const size_t ws_bytes = o_stat + sizeof(Stat);
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, ws_bytes, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (tracks)"; cudaGetLastError(); return -1; }
-    int* parent = reinterpret_cast<int*>(ws + o_parent);
-    int* cnt = reinterpret_cast<int*>(ws + o_cnt);
-    int* va = reinterpret_cast<int*>(ws + o_va);
-    int* vb = reinterpret_cast<int*>(ws + o_vb);
-    unsigned long long* key = reinterpret_cast<unsigned long long*>(ws + o_key);
-    int* hist = reinterpret_cast<int*>(ws + o_hist);
-    void* part = ws + o_part;
-    int32_t* d_off = reinterpret_cast<int32_t*>(ws + o_off);
-    Stat* stat = reinterpret_cast<Stat*>(ws + o_stat);
-    auto fail = [&](const char* msg) { cudaGetLastError(); cudaFreeAsync(ws, st); *err = msg; return -1; };
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (tracks)", "tracks: upload failed");
+    const size_t o_parent = ws.take(4ull * N), o_cnt = ws.take(4ull * N), o_va = ws.take(4ull * N), o_vb = ws.take(4ull * N);
+    const size_t o_key = ws.take(8ull * N), o_hist = ws.take(4ull * n_hist);
+    const size_t o_part = ws.take(8ull * scan_partials(std::max<long long>({(long long)N, n_hist, 1})));
+    const size_t o_off = ws.put(off.data(), 4ull * off.size()), o_plan = ws.put(plan.data(), plan.size());
+    const size_t o_stat = ws.take(sizeof(Stat));
+    if (!ws.alloc(err)) return -1;
+    int* parent = ws.at<int>(o_parent);
+    int* cnt = ws.at<int>(o_cnt);
+    int* va = ws.at<int>(o_va);
+    int* vb = ws.at<int>(o_vb);
+    unsigned long long* key = ws.at<unsigned long long>(o_key);
+    int* hist = ws.at<int>(o_hist);
+    void* part = ws.at<void>(o_part);
+    int32_t* d_off = ws.at<int32_t>(o_off);
+    Stat* stat = ws.at<Stat>(o_stat);
 
-    std::vector<uint8_t> head(o_stat - o_off, 0);
-    std::memcpy(head.data(), off.data(), off.size() * 4);
-    if (!plan.empty()) std::memcpy(head.data() + (o_plan - o_off), plan.data(), plan.size());
-    if (!upload_plan(ws + o_off, head, st)) return fail("tracks: upload failed");
-    if (cudaMemsetAsync(stat, 0, sizeof(Stat), st) != cudaSuccess) return fail("tracks: memset failed");
+    if (cudaMemsetAsync(stat, 0, sizeof(Stat), st) != cudaSuccess) return ws.fail("tracks: memset failed", err);
     int launches = 0;
     if (N > 0) {
         tracks_init_kernel<<<blocks_for(N, kT), kT, 0, st>>>(parent, cnt, N);
         ++launches;
         if (n_items > 0) {
-            tracks_hook_kernel<<<blocks_for(n_items, kT), kT, 0, st>>>(make_src(ws + o_plan, N), n_items, parent, &stat->bad);
+            tracks_hook_kernel<<<blocks_for(n_items, kT), kT, 0, st>>>(make_src(ws.at<uint8_t>(o_plan), N), n_items, parent, &stat->bad);
             ++launches;
         }
         tracks_compress_kernel<<<blocks_for(N, kT), kT, 0, st>>>(parent, N);
@@ -328,21 +318,19 @@ int run_tracks(int n_sets, const int32_t* n_feat, long long n_items, const std::
         tracks_gather_kernel<<<blocks_for(N, kT), kT, 0, st>>>(parent, cnt, vb, va, N);
         ++launches;
     } else if (n_items > 0) {
-        tracks_hook_kernel<<<blocks_for(n_items, kT), kT, 0, st>>>(make_src(ws + o_plan, N), n_items, parent, &stat->bad);
+        tracks_hook_kernel<<<blocks_for(n_items, kT), kT, 0, st>>>(make_src(ws.at<uint8_t>(o_plan), N), n_items, parent, &stat->bad);
         ++launches;
     }
     Stat h{};
-    if (cudaMemcpyAsync(&h, stat, sizeof(Stat), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
-        return fail("tracks: read-back failed");
+    if (!read_back(&h, stat, sizeof(Stat), st)) return ws.fail("tracks: read-back failed", err);
     if (h.bad) {
-        cudaFreeAsync(ws, st);
         *bad_edge = true;
         return launches;
     }
     const int A = h.active;
-    if (N > 0 && cudaMemsetAsync(track_of, 0xff, 4ull * N, st) != cudaSuccess) return fail("tracks: memset failed");
+    if (N > 0 && cudaMemsetAsync(track_of, 0xff, 4ull * N, st) != cudaSuccess) return ws.fail("tracks: memset failed", err);
     if (A == 0) {
-        if (cudaMemsetAsync(track_start, 0, 4, st) != cudaSuccess) return fail("tracks: memset failed");
+        if (cudaMemsetAsync(track_start, 0, 4, st) != cudaSuccess) return ws.fail("tracks: memset failed", err);
     } else {
         int bits = 0;
         while (bits < 31 && ((N - 1) >> bits) != 0) ++bits;
@@ -364,11 +352,9 @@ int run_tracks(int n_sets, const int32_t* n_feat, long long n_items, const std::
         tracks_start_kernel<<<blocks_for(A, kT), kT, 0, st>>>(src, A, parent, cnt, key, &stat->total, min_length, spare, track_start);
         tracks_members_kernel<<<blocks_for(A, kT), kT, 0, st>>>(src, A, parent, cnt, spare, members, track_of);
         launches += 2;
-        if (cudaMemcpyAsync(&h, stat, sizeof(Stat), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
-            return fail("tracks: read-back failed");
+        if (!read_back(&h, stat, sizeof(Stat), st)) return ws.fail("tracks: read-back failed", err);
     }
     const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     counts->n_tracks = (int32_t)(h.total >> 32);
     counts->n_members = (int32_t)(uint32_t)h.total;

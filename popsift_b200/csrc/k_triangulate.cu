@@ -2,7 +2,7 @@
 // The per-observation math is in k_triangulate.h, the two-ray rule in k_pose_solve.h and the sample hash in
 // k_verify_sample.h.
 //
-// One workspace from the matcher's pool, all launches on one stream:
+// One workspace (workspace.h), all launches on one stream:
 //   1. tri_ray_kernel    one thread per member: the member id's bounds and the monotonicity of d_track_start (a flag), the
 //                        member's set, pixel and unit ray direction.  The flag is read back before anything is written.
 //   2. tri_track_kernel  one warp per track.  Hypotheses go across the lanes; each lane scores its hypotheses on all of
@@ -13,11 +13,11 @@
 //                        exchanged by shuffles.  Each lane reads from memory only what it wrote itself.
 //   3. tri_count_kernel  tracks per status and inlier observations: a shared histogram per block, one atomic per block
 //                        and counter.
-#include "k_match_common.h"
 #include "k_triangulate.h"
 #include "k_verify_sample.h"
 #include "ps_internal.h"
 #include "popsift_b200_triangulate.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <cmath>
@@ -57,8 +57,6 @@ struct TriArgs {
     uint8_t* mask;
     float* err;
 };
-
-unsigned blocks_for(long long n, long long per) { return (unsigned)((n + per - 1) / per); }
 
 __device__ __forceinline__ int tri_set_of(const int32_t* __restrict__ off, int n_sets, int g)
 {
@@ -325,36 +323,23 @@ int run_triangulate_tracks(int n_sets, const int32_t* n_feat, const ps_feature* 
         K.fx = cams[i].fx; K.fy = cams[i].fy; K.cx = cams[i].cx; K.cy = cams[i].cy;
     }
     // workspace: the plan (cameras, feature pointers, set offsets), the statistics, then 40 bytes per member
-    size_t o = 0;
-    auto take = [&](size_t bytes) { const size_t r = o; o = align_up(o + bytes, 256); return r; };
-    const size_t o_cams = take(tc.size() * sizeof(TriCam)), o_feat = take((size_t)n_sets * sizeof(void*));
-    const size_t o_off = take(off.size() * sizeof(int32_t));
-    const size_t plan_bytes = o;
-    const size_t o_stat = take(sizeof(TriStat));
-    const size_t o_rays = take((size_t)n_members * sizeof(TriRay));
-    std::vector<uint8_t> plan(plan_bytes, 0);
-    if (!tc.empty()) std::memcpy(plan.data() + o_cams, tc.data(), tc.size() * sizeof(TriCam));
-    if (n_sets > 0) std::memcpy(plan.data() + o_feat, feat, (size_t)n_sets * sizeof(void*));
-    std::memcpy(plan.data() + o_off, off.data(), off.size() * sizeof(int32_t));
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, o, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (triangulate)"; cudaGetLastError(); return -1; }
-    auto fail = [&](const char* msg) { cudaGetLastError(); cudaFreeAsync(ws, st); *err = msg; return -1; };
-    if (!upload_plan(ws, plan, st)) return fail("triangulate: plan upload failed");
-    TriStat* stat = reinterpret_cast<TriStat*>(ws + o_stat);
-    if (cudaMemsetAsync(stat, 0, sizeof(TriStat), st) != cudaSuccess) return fail("triangulate: memset failed");
-    const TriCam* d_cams = reinterpret_cast<const TriCam*>(ws + o_cams);
-    TriRay* rays = reinterpret_cast<TriRay*>(ws + o_rays);
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (triangulate)", "triangulate: plan upload failed");
+    const size_t o_cams = ws.put(tc.data(), tc.size() * sizeof(TriCam)), o_feat = ws.put(feat, (size_t)n_sets * sizeof(void*));
+    const size_t o_off = ws.put(off.data(), off.size() * sizeof(int32_t));
+    const size_t o_stat = ws.take(sizeof(TriStat));
+    const size_t o_rays = ws.take((size_t)n_members * sizeof(TriRay));
+    if (!ws.alloc(err)) return -1;
+    TriStat* stat = ws.at<TriStat>(o_stat);
+    if (cudaMemsetAsync(stat, 0, sizeof(TriStat), st) != cudaSuccess) return ws.fail("triangulate: memset failed", err);
+    const TriCam* d_cams = ws.at<const TriCam>(o_cams);
+    TriRay* rays = ws.at<TriRay>(o_rays);
     const long long n_items = std::max<long long>(n_members, (long long)n_tracks + 1);
     tri_ray_kernel<<<blocks_for(n_items, kRayThreads), kRayThreads, 0, st>>>(
-        track_start, n_tracks, members, n_members, reinterpret_cast<const int32_t*>(ws + o_off), n_sets,
-        reinterpret_cast<const ps_feature* const*>(ws + o_feat), d_cams, rays, &stat->bad);
+        track_start, n_tracks, members, n_members, ws.at<const int32_t>(o_off), n_sets, ws.at<const ps_feature* const>(o_feat), d_cams,
+        rays, &stat->bad);
     TriStat h{};
-    if (cudaMemcpyAsync(&h, stat, sizeof(TriStat), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
-        return fail("triangulate: read-back failed");
+    if (!read_back(&h, stat, sizeof(TriStat), st)) return ws.fail("triangulate: read-back failed", err);
     if (h.bad) {
-        cudaFreeAsync(ws, st);
         *bad = true;
         return 1;
     }
@@ -375,10 +360,8 @@ int run_triangulate_tracks(int n_sets, const int32_t* n_feat, const ps_feature* 
     tri_track_kernel<<<blocks_for(n_tracks, kTrackWarps), kTrackWarps * 32, 0, st>>>(A);
     const unsigned nc = std::min<unsigned>(blocks_for(n_tracks, kCountThreads), 4u * (unsigned)sm_count());
     tri_count_kernel<<<nc, kCountThreads, 0, st>>>(points, n_tracks, stat);
-    if (cudaMemcpyAsync(&h, stat, sizeof(TriStat), cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
-        return fail("triangulate: read-back failed");
+    if (!read_back(&h, stat, sizeof(TriStat), st)) return ws.fail("triangulate: read-back failed", err);
     const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     std::memcpy(counts->n_status, h.n_status, sizeof(counts->n_status));
     counts->n_inlier_obs = h.n_inlier_obs;

@@ -5,7 +5,7 @@
 // against the three rows before it); an order-preserving block scan (warp ballots + a prefix over the warps) compacts
 // the kept rows, so no atomic decides the output order.
 //
-// ps_verify_batch, one workspace from the matcher's pool, all launches on one stream:
+// ps_verify_batch, one workspace (workspace.h), all launches on one stream:
 //   1. verify_normalize_kernel  one CTA per pair: centroids and the common scale in double (fixed-order reductions), then
 //                               the pair's points as normalised float4 rows and the normalised squared threshold.
 //   2. verify_solve_kernel      one lane per minimal sample, in double: the sample hash (k_verify_sample.h), the 4-point
@@ -21,10 +21,10 @@
 //                               double, fixed order; smallest eigenvector by warp-parallel Jacobi; for F the rank-2 step),
 //                               the output model in pixels, the mask and its sum.
 //   5. verify_taps_kernel       (taps only) every hypothesis's count and pixel model.
-#include "k_match_common.h"
 #include "k_verify_common.h"
 #include "k_verify_sample.h"
 #include "ps_internal.h"
+#include "workspace.h"
 
 #include <algorithm>
 #include <cmath>
@@ -618,24 +618,21 @@ int run_match_correspondences(const ps_feature* const* feat, const int32_t* cons
                               const char** err)
 {
     *err = nullptr;
-    std::vector<uint8_t> host(align_up((size_t)n_pairs * sizeof(CorrPair), 16) + align_up((size_t)n_pairs * sizeof(int32_t), 16));
-    CorrPair* hp = reinterpret_cast<CorrPair*>(host.data());
+    std::vector<CorrPair> hp(n_pairs);
     long long row = 0;
     for (int p = 0; p < n_pairs; ++p) {
         const int l = pairs[2 * p], r = pairs[2 * p + 1];
         hp[p] = {feat[l], rev[l], feat[r], rev[r], row, n_desc[l], n_desc[r]};
         row += n_desc[l];
     }
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, host.size(), pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (correspondences)"; cudaGetLastError(); return -1; }
-    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "correspondences: upload failed"; return -1; }
-    int32_t* d_counts = reinterpret_cast<int32_t*>(ws + align_up((size_t)n_pairs * sizeof(CorrPair), 16));
-    corr_gather_kernel<<<n_pairs, kGatherThreads, 0, st>>>(reinterpret_cast<const CorrPair*>(ws), match, reinterpret_cast<float4*>(corr), src, d_counts);
-    const bool ok = cudaMemcpyAsync(n_corr, d_counts, (size_t)n_pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, st) == cudaSuccess;
-    cudaFreeAsync(ws, st);
-    if (!ok) { *err = "correspondences: count download failed"; cudaGetLastError(); return -1; }
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (correspondences)", "correspondences: upload failed");
+    const size_t o_pairs = ws.put(hp.data(), hp.size() * sizeof(CorrPair), 16);
+    const size_t o_counts = ws.put(nullptr, (size_t)n_pairs * sizeof(int32_t), 16);
+    if (!ws.alloc(err)) return -1;
+    int32_t* d_counts = ws.at<int32_t>(o_counts);
+    corr_gather_kernel<<<n_pairs, kGatherThreads, 0, st>>>(ws.at<const CorrPair>(o_pairs), match, reinterpret_cast<float4*>(corr), src, d_counts);
+    if (cudaMemcpyAsync(n_corr, d_counts, (size_t)n_pairs * sizeof(int32_t), cudaMemcpyDeviceToHost, st) != cudaSuccess)
+        return ws.fail("correspondences: count download failed", err);
     return 1;
 }
 
@@ -666,31 +663,21 @@ int run_verify_batch(int n_pairs, const float* corr, const int32_t* corr_start, 
     }
     if (solve.size() > 0x7fffffffu || score.size() > 0x7fffffffu) { *err = "ps_verify_batch: too many work items"; return -1; }
     const size_t n_hyp = (size_t)n_pairs * K * ns;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off = align_up(off + bytes, 256); return o; };
-    const size_t o_pairs = take(vp.size() * sizeof(VPair)), o_solve = take(solve.size() * sizeof(VSolveItem));
-    const size_t o_score = take(score.size() * sizeof(VScoreItem));
-    const size_t meta_bytes = off;
-    const size_t o_xf = take((size_t)n_pairs * sizeof(VXform)), o_pts = take((size_t)total_rows * sizeof(float4));
-    const size_t o_models = take(n_hyp * 9 * sizeof(float)), o_counts = take(n_hyp * sizeof(int32_t));
-    std::vector<uint8_t> host(meta_bytes);
-    std::memcpy(host.data() + o_pairs, vp.data(), vp.size() * sizeof(VPair));
-    std::memcpy(host.data() + o_solve, solve.data(), solve.size() * sizeof(VSolveItem));
-    if (!score.empty()) std::memcpy(host.data() + o_score, score.data(), score.size() * sizeof(VScoreItem));
-    cudaMemPool_t pool = match_pool(err);
-    if (!pool) return -1;
-    uint8_t* ws = nullptr;
-    if (cudaMallocFromPoolAsync(&ws, off, pool, st) != cudaSuccess) { *err = "cudaMallocFromPoolAsync failed (verify workspace)"; cudaGetLastError(); return -1; }
-    if (!upload_plan(ws, host, st)) { cudaFreeAsync(ws, st); *err = "verify: plan upload failed"; return -1; }
-    const VPair* d_pairs = reinterpret_cast<const VPair*>(ws + o_pairs);
-    VXform* d_xf = reinterpret_cast<VXform*>(ws + o_xf);
-    float4* d_pts = reinterpret_cast<float4*>(ws + o_pts);
+    Workspace ws(st, "cudaMallocFromPoolAsync failed (verify workspace)", "verify: plan upload failed");
+    const size_t o_pairs = ws.put(vp.data(), vp.size() * sizeof(VPair)), o_solve = ws.put(solve.data(), solve.size() * sizeof(VSolveItem));
+    const size_t o_score = ws.put(score.data(), score.size() * sizeof(VScoreItem));
+    const size_t o_xf = ws.take((size_t)n_pairs * sizeof(VXform)), o_pts = ws.take((size_t)total_rows * sizeof(float4));
+    const size_t o_models = ws.take(n_hyp * 9 * sizeof(float)), o_counts = ws.take(n_hyp * sizeof(int32_t));
+    if (!ws.alloc(err)) return -1;
+    const VPair* d_pairs = ws.at<const VPair>(o_pairs);
+    VXform* d_xf = ws.at<VXform>(o_xf);
+    float4* d_pts = ws.at<float4>(o_pts);
     verify_normalize_kernel<<<n_pairs, kNormThreads, 0, st>>>(d_pairs, reinterpret_cast<const float4*>(corr), d_pts, d_xf, (double)prm.threshold);
     int launches = 1;
-    const VSolveItem* d_solve = reinterpret_cast<const VSolveItem*>(ws + o_solve);
-    const VScoreItem* d_score = reinterpret_cast<const VScoreItem*>(ws + o_score);
-    float* hyp_models = reinterpret_cast<float*>(ws + o_models);
-    int32_t* hyp_counts = reinterpret_cast<int32_t*>(ws + o_counts);
+    const VSolveItem* d_solve = ws.at<const VSolveItem>(o_solve);
+    const VScoreItem* d_score = ws.at<const VScoreItem>(o_score);
+    float* hyp_models = ws.at<float>(o_models);
+    int32_t* hyp_counts = ws.at<int32_t>(o_counts);
     if (prm.model == PS_GEOM_HOMOGRAPHY)
         launches += launch_verify<PS_GEOM_HOMOGRAPHY>(d_pairs, d_xf, d_pts, d_solve, (int)solve.size(), d_score, (int)score.size(), n_pairs, prm,
                                                       hyp_models, hyp_counts, d_models, d_n, d_mask, taps, st);
@@ -698,7 +685,6 @@ int run_verify_batch(int n_pairs, const float* corr, const int32_t* corr_start, 
         launches += launch_verify<PS_GEOM_FUNDAMENTAL>(d_pairs, d_xf, d_pts, d_solve, (int)solve.size(), d_score, (int)score.size(), n_pairs, prm,
                                                        hyp_models, hyp_counts, d_models, d_n, d_mask, taps, st);
     const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(ws, st);
     if (e != cudaSuccess) { *err = cudaGetErrorString(e); return -1; }
     return launches;
 }
