@@ -351,6 +351,45 @@ struct Rotations
 Rotations rotationAveraging(int n_sets, const std::vector<std::pair<int, int>>& pairs, const std::vector<TwoViewPose>& poses,
                             const RotationParams& params = RotationParams());
 
+/// Settings of filterViewGraph (same fields and rules as ps_view_graph_params in popsift_b200_viewgraph.h).
+struct ViewGraphParams
+{
+    double max_cycle_error = 3.0;    // degrees: a triangle whose cycle error is at most this is consistent
+    int    min_consistent = 1;       // a pair in some triangle is kept with at least this many consistent ones ...
+    double min_fraction = 0.0;       // ... and at least this fraction of its triangles consistent, [0, 1]
+    bool   keep_untested = false;    // the fate of a used pair that lies in no triangle
+    int    min_inliers = 15;         // a pair is used when its n_front reaches this (as in RotationParams)
+};
+
+/// One pair's triangles (ps_cycle_stats): how many, how many consistent, the smallest cycle error in degrees (+inf: none).
+struct CycleStats
+{
+    int   n_triangles = 0, n_consistent = 0;
+    float min_error = 0;
+};
+
+/// What filterViewGraph did (ps_view_graph_report).
+struct ViewGraphReport
+{
+    long long n_triangles = 0, n_consistent_triangles = 0;
+    int       n_used = 0, n_kept = 0, n_untested = 0;
+};
+
+/// The pairs kept, one CycleStats per pair and the totals.
+struct ViewGraph
+{
+    std::vector<bool>       keep;
+    std::vector<CycleStats> stats;
+    ViewGraphReport         report;
+};
+
+/// View-graph cleaning on device 0 (an addition to the reference's interface; C ABI ps_view_graph_filter): drops the pairs
+/// whose relative rotations fail loop consistency over the triangles of the view graph.  `poses` is what relativePoses
+/// gave for `pairs` (its R and n_front are uploaded); the kept pairs and their poses go to rotationAveraging.  Throws when
+/// poses.size() != pairs.size(), and for the arguments ps_view_graph_filter refuses (a duplicate pair among them).
+ViewGraph filterViewGraph(int n_sets, const std::vector<std::pair<int, int>>& pairs, const std::vector<TwoViewPose>& poses,
+                          const ViewGraphParams& params = ViewGraphParams());
+
 /// Settings of globalPositioning (same fields and rules as ps_position_params).
 struct PositionParams
 {

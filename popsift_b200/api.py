@@ -160,6 +160,28 @@ class PsPositionReport(C.Structure):
                 ("n_obs", C.c_int32), ("n_points", C.c_int32), ("n_cams", C.c_int32), ("termination", C.c_int32)]
 
 
+class PsViewGraphParams(C.Structure):
+    """ps_view_graph_params (32 bytes)"""
+    _fields_ = [("min_inliers", C.c_int32), ("min_consistent", C.c_int32), ("keep_untested", C.c_int32), ("pad_", C.c_int32),
+                ("max_cycle_error", C.c_double), ("min_fraction", C.c_double)]
+
+
+class PsCycleStats(C.Structure):
+    """ps_cycle_stats (12 bytes)"""
+    _fields_ = [("n_triangles", C.c_int32), ("n_consistent", C.c_int32), ("min_error", C.c_float)]
+
+
+class PsViewGraphReport(C.Structure):
+    """ps_view_graph_report (32 bytes)"""
+    _fields_ = [("n_triangles", C.c_int64), ("n_consistent_triangles", C.c_int64), ("n_used", C.c_int32), ("n_kept", C.c_int32),
+                ("n_untested", C.c_int32), ("pad_", C.c_int32)]
+
+
+# ps_cycle_stats as a numpy record
+CYCLE_STATS_DTYPE = np.dtype([("n_triangles", "<i4"), ("n_consistent", "<i4"), ("min_error", "<f4")])
+assert C.sizeof(PsViewGraphParams) == 32 and C.sizeof(PsCycleStats) == 12 and C.sizeof(PsViewGraphReport) == 32
+assert CYCLE_STATS_DTYPE.itemsize == 12
+
 RA_TERMINATION = ("max_iters", "step_tol", "no_pairs")
 GP_TERMINATION = ("max_iters", "function_tol", "no_observations")
 assert C.sizeof(PsRotationParams) == 40 and C.sizeof(PsRotationReport) == 40
@@ -186,6 +208,8 @@ TRIANGULATE_EXPORTS = ["ps_triangulate_tracks"]
 BUNDLE_EXPORTS = ["ps_bundle_adjust"]
 # global poses, declared in popsift_b200_global.h (same library)
 GLOBAL_EXPORTS = ["ps_rotation_averaging", "ps_global_positioning"]
+# view-graph cleaning, declared in popsift_b200_viewgraph.h (same library)
+VIEWGRAPH_EXPORTS = ["ps_view_graph_filter"]
 
 _lib = None
 
@@ -260,6 +284,9 @@ def load_library():
         L.ps_global_positioning.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                             C.c_void_p, C.c_void_p, C.c_int, C.POINTER(PsPositionParams), C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.POINTER(PsPositionReport)]
+    if hasattr(L, "ps_view_graph_filter"):
+        L.ps_view_graph_filter.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(PsViewGraphParams), C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.POINTER(PsViewGraphReport)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -1302,6 +1329,22 @@ def _rotation_dev(lib, device, n_sets, pairs, d_two_view, prm: PsRotationParams)
     return R[:n_sets].reshape(-1, 3, 3), reg[:n_sets].astype(bool), err[:P].copy(), out
 
 
+def _two_view_records(two_view, n_pairs) -> np.ndarray:
+    """ps_two_view records (TWO_VIEW_DTYPE) from TwoView tuples, such records or (R, n_front) tuples, one per pair"""
+    if isinstance(two_view, np.ndarray) and two_view.dtype == TWO_VIEW_DTYPE:
+        rec = np.ascontiguousarray(two_view)
+    else:
+        rec = np.zeros(len(two_view), TWO_VIEW_DTYPE)
+        for p, tv in enumerate(two_view):
+            if isinstance(tv, TwoView):
+                rec[p]["R"], rec[p]["t"], rec[p]["n_inliers"], rec[p]["n_front"] = tv.R, tv.t, tv.n_inliers, tv.n_front
+            else:
+                rec[p]["R"], rec[p]["n_front"] = np.asarray(tv[0], np.float32).reshape(3, 3), int(tv[1])
+    if len(rec) != n_pairs:
+        raise PopSiftError("one two-view record per pair expected")
+    return rec
+
+
 def rotation_averaging(n_sets, pairs, two_view, device=0, **params):
     """Robust rotation averaging over a view graph (C ABI ps_rotation_averaging in popsift_b200_global.h; an addition to the
     reference's interface): a maximum-spanning-tree start, then IRLS on the device.  `pairs` is the (l, r) list and
@@ -1312,20 +1355,52 @@ def rotation_averaging(n_sets, pairs, two_view, device=0, **params):
     lib = load_library()
     prm = _rotation_params(**params)
     pairs = [(int(a), int(b)) for a, b in pairs]
-    if isinstance(two_view, np.ndarray) and two_view.dtype == TWO_VIEW_DTYPE:
-        rec = np.ascontiguousarray(two_view)
-    else:
-        rec = np.zeros(len(two_view), TWO_VIEW_DTYPE)
-        for p, tv in enumerate(two_view):
-            if isinstance(tv, TwoView):
-                rec[p]["R"], rec[p]["t"], rec[p]["n_inliers"], rec[p]["n_front"] = tv.R, tv.t, tv.n_inliers, tv.n_front
-            else:
-                rec[p]["R"], rec[p]["n_front"] = np.asarray(tv[0], np.float32).reshape(3, 3), int(tv[1])
-    if len(rec) != len(pairs):
-        raise PopSiftError("one two-view record per pair expected")
+    rec = _two_view_records(two_view, len(pairs))
     bufs = _DevBuffers(lib)
     try:
         return _rotation_dev(lib, device, n_sets, pairs, bufs.upload(rec) if len(rec) else None, prm)
+    finally:
+        bufs.free()
+
+
+ViewGraphReport = namedtuple("ViewGraphReport", "n_triangles n_consistent_triangles n_used n_kept n_untested")
+ViewGraphReport.__doc__ = """ps_view_graph_report of ps_view_graph_filter (popsift_b200_viewgraph.h)."""
+ViewGraph = namedtuple("ViewGraph", "keep n_triangles n_consistent min_error report")
+ViewGraph.__doc__ = """filter_view_graph's result: keep bool (P,), per pair the triangles it lies in, the consistent ones and
+the smallest cycle error in degrees (+inf: none), and the ViewGraphReport."""
+
+
+def _view_graph_params(max_cycle_error=3.0, min_consistent=1, min_fraction=0.0, keep_untested=False, min_inliers=15) -> PsViewGraphParams:
+    return PsViewGraphParams(int(min_inliers), int(min_consistent), 1 if keep_untested else 0, 0, float(max_cycle_error), float(min_fraction))
+
+
+def _view_graph_dev(lib, device, n_sets, pairs, d_two_view, prm: PsViewGraphParams, d_kept=None) -> ViewGraph:
+    """ps_view_graph_filter on device two-view records; the kept records go to d_kept when it is given"""
+    P = len(pairs)
+    keep = np.zeros(max(P, 1), np.uint8)
+    st = np.zeros(max(P, 1), CYCLE_STATS_DTYPE)
+    rep = PsViewGraphReport()
+    rc = lib.ps_view_graph_filter(device, int(n_sets), P, _c_pairs(pairs), d_two_view if P else None, C.byref(prm), keep.ctypes.data,
+                                  st.ctypes.data, d_kept, C.byref(rep))
+    _check(lib, rc, "ps_view_graph_filter")
+    r = ViewGraphReport(int(rep.n_triangles), int(rep.n_consistent_triangles), int(rep.n_used), int(rep.n_kept), int(rep.n_untested))
+    return ViewGraph(keep[:P].astype(bool), st["n_triangles"][:P].copy(), st["n_consistent"][:P].copy(), st["min_error"][:P].copy(), r)
+
+
+def filter_view_graph(n_sets, pairs, two_view, device=0, **params) -> ViewGraph:
+    """View-graph cleaning by rotation loop consistency (C ABI ps_view_graph_filter in popsift_b200_viewgraph.h; an addition
+    to the reference's interface): every triangle of the used pairs is tested, R(c->a) R(b->c) R(a->b) against the identity,
+    and a pair is kept when enough of its triangles close.  `pairs` and `two_view` as for rotation_averaging (pairs must be
+    distinct, in either order).  params: max_cycle_error (degrees, 3.0), min_consistent (1), min_fraction (0.0),
+    keep_untested (False: a used pair in no triangle is dropped), min_inliers (n_front threshold, 15; use rotation
+    averaging's).  Returns a ViewGraph."""
+    lib = load_library()
+    prm = _view_graph_params(**params)
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    rec = _two_view_records(two_view, len(pairs))
+    bufs = _DevBuffers(lib)
+    try:
+        return _view_graph_dev(lib, device, n_sets, pairs, bufs.upload(rec) if len(rec) else None, prm)
     finally:
         bufs.free()
 
@@ -1386,19 +1461,25 @@ def global_positioning(sets, tracks, cameras, rotations, registered, device=None
 
 
 def global_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=None, min_length=2, max_pair_error=5.0, pose=None,
-                 rotation=None, position=None) -> GlobalPoses:
+                 rotation=None, position=None, view_graph=None) -> GlobalPoses:
     """Poses for every image from images and intrinsics alone, without leaving the device: relative_poses' chain
     (matching unless `matches` is given, correspondences, ps_relative_pose_batch with the parameters in the dict `pose`),
     ps_rotation_averaging on its records (dict `rotation`: rotation_averaging's params), ps_tracks_from_matches on the
     pose masks of the pairs that were used, are registered and have a final rotation error <= max_pair_error degrees
     (the other pairs contribute no correspondence), then ps_global_positioning on those tracks (dict `position`:
-    global_positioning's params).  `sets` are FeaturesDev objects and `cameras` one (fx, fy, cx, cy) per set.  The
-    result feeds triangulate() and then bundle_adjust()."""
+    global_positioning's params).  A dict `view_graph` (filter_view_graph's params but min_inliers, which is the
+    rotation's) cleans the view graph first: ps_view_graph_filter on the relative poses, rotation averaging on the kept
+    pairs only, and the dropped pairs get pair_error +inf (so they contribute no correspondence).  `sets` are FeaturesDev
+    objects and `cameras` one (fx, fy, cx, cy) per set.  The result feeds triangulate() and then bundle_adjust()."""
     lib = load_library()
     pairs = [(int(a), int(b)) for a, b in pairs]
     pprm = _pose_params(**(pose or {}))
     rprm = _rotation_params(**(rotation or {}))
     gprm = _position_params(**(position or {}))
+    if view_graph is not None:
+        if "min_inliers" in view_graph:
+            raise PopSiftError("view_graph takes min_inliers from the rotation parameters")
+        vgprm = _view_graph_params(min_inliers=rprm.min_inliers, **view_graph)
     cam = np.asarray(cameras, np.float32).reshape(-1, 4)
     if len(cam) != len(sets):
         raise PopSiftError("one camera per set expected")
@@ -1407,7 +1488,16 @@ def global_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=N
         _, device, rows, d_match, d_corr, d_src, start, n_corr = _matched_rows(lib, bufs, sets, pairs, matches, flags, u8, device,
                                                                               u8 and matches is None)
         d_out, d_mask = _pose_dev(lib, bufs, device, d_corr, start, n_corr, _c_cameras([cam[i] for lr in pairs for i in lr]), pprm)[:2]
-        R, reg, perr, rrep = _rotation_dev(lib, device, len(sets), pairs, d_out, rprm)
+        if view_graph is None:
+            R, reg, perr, rrep = _rotation_dev(lib, device, len(sets), pairs, d_out, rprm)
+        else:
+            # rotation averaging on the kept pairs' records, its errors scattered back to the full pair list
+            d_kept = bufs.alloc(max(len(pairs), 1) * TWO_VIEW_DTYPE.itemsize)
+            vg = _view_graph_dev(lib, device, len(sets), pairs, d_out, vgprm, d_kept)
+            kept = np.flatnonzero(vg.keep)
+            R, reg, perr_k, rrep = _rotation_dev(lib, device, len(sets), [pairs[p] for p in kept], d_kept, rprm)
+            perr = np.full(len(pairs), np.inf, np.float32)
+            perr[kept] = perr_k
         keep = np.ascontiguousarray(np.where(perr <= float(max_pair_error), n_corr, 0), np.int32)
         n = max(len(sets), 1)
         n_feat = [s.getFeatureCount() for s in sets]

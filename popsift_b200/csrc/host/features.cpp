@@ -11,6 +11,7 @@
 #include "popsift_b200_triangulate.h"
 #include "popsift_b200_bundle.h"
 #include "popsift_b200_global.h"
+#include "popsift_b200_viewgraph.h"
 
 #include <algorithm>
 #include <cmath>
@@ -762,6 +763,56 @@ Rotations rotationAveraging(int n_sets, const std::vector<std::pair<int, int>>& 
     o.n_pairs = r.n_pairs;
     o.n_registered = r.n_registered;
     o.termination = r.termination;
+    return out;
+}
+
+ViewGraph filterViewGraph(int n_sets, const std::vector<std::pair<int, int>>& pairs, const std::vector<TwoViewPose>& poses,
+                          const ViewGraphParams& params)
+{
+    const std::string who = "popsift::filterViewGraph";
+    if (n_sets < 0) throw std::runtime_error(who + ": n_sets < 0");
+    if (poses.size() != pairs.size()) throw std::runtime_error(who + ": one relative pose per pair expected");
+    const size_t np = pairs.size();
+    std::vector<ps_two_view> rec(np);
+    std::vector<int32_t> flat(2 * np);
+    for (size_t p = 0; p < np; ++p) {
+        rec[p] = ps_two_view{};
+        std::copy(poses[p].R, poses[p].R + 9, rec[p].R);
+        std::copy(poses[p].t, poses[p].t + 3, rec[p].t);
+        rec[p].n_inliers = poses[p].n_inliers;
+        rec[p].n_front = poses[p].n_front;
+        flat[2 * p] = pairs[p].first;
+        flat[2 * p + 1] = pairs[p].second;
+    }
+    DevBuf d(std::max<size_t>(np, 1) * sizeof(ps_two_view), who);
+    if (np) check(ps_host_to_dev(d.p, rec.data(), np * sizeof(ps_two_view)), who);
+    ps_view_graph_params prm{};
+    prm.min_inliers = params.min_inliers;
+    prm.min_consistent = params.min_consistent;
+    prm.keep_untested = params.keep_untested ? 1 : 0;
+    prm.max_cycle_error = params.max_cycle_error;
+    prm.min_fraction = params.min_fraction;
+    std::vector<uint8_t> keep(std::max<size_t>(np, 1));
+    std::vector<ps_cycle_stats> cs(std::max<size_t>(np, 1));
+    ps_view_graph_report r;
+    check(ps_view_graph_filter(0, n_sets, (int)np, flat.data(), static_cast<const ps_two_view*>(d.p), &prm, keep.data(), cs.data(), nullptr,
+                               &r),
+          who, "ps_view_graph_filter");
+    ViewGraph out;
+    out.keep.resize(np);
+    out.stats.resize(np);
+    for (size_t p = 0; p < np; ++p) {
+        out.keep[p] = keep[p] != 0;
+        out.stats[p].n_triangles = cs[p].n_triangles;
+        out.stats[p].n_consistent = cs[p].n_consistent;
+        out.stats[p].min_error = cs[p].min_error;
+    }
+    ViewGraphReport& o = out.report;
+    o.n_triangles = r.n_triangles;
+    o.n_consistent_triangles = r.n_consistent_triangles;
+    o.n_used = r.n_used;
+    o.n_kept = r.n_kept;
+    o.n_untested = r.n_untested;
     return out;
 }
 

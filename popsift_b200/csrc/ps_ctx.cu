@@ -1599,6 +1599,56 @@ extern "C" int ps_global_positioning(int device, int n_sets, const int32_t* n_fe
     return rc;
 }
 
+extern "C" int ps_view_graph_filter(int device, int n_sets, int n_pairs, const int32_t* pairs, const ps_two_view* d_two_view,
+                                    const ps_view_graph_params* prm, uint8_t* keep, ps_cycle_stats* stats, ps_two_view* d_kept,
+                                    ps_view_graph_report* report)
+{
+    if (n_sets < 0 || n_pairs < 0 || !prm || !keep || !report || (n_pairs > 0 && !pairs)) return PS_ERR_ARG;
+    for (int p = 0; p < 2 * n_pairs; ++p)
+        if (pairs[p] < 0 || pairs[p] >= n_sets) return PS_ERR_ARG;
+    if (prm->min_inliers < 0 || prm->min_consistent < 0 || prm->keep_untested < 0 || prm->keep_untested > 1) return PS_ERR_ARG;
+    if (!std::isfinite(prm->max_cycle_error) || !(prm->max_cycle_error >= 0.0)) return PS_ERR_ARG;
+    if (!(prm->min_fraction >= 0.0 && prm->min_fraction <= 1.0)) return PS_ERR_ARG;
+    // duplicates, in either order, in O(pairs + sets): the larger ends bucketed by the smaller end, then each bucket's
+    // larger ends stamped with the bucket's set
+    std::vector<int32_t> start(n_sets + 1, 0), larger(n_pairs), seen(n_sets, -1);
+    for (int p = 0; p < n_pairs; ++p) ++start[std::min(pairs[2 * p], pairs[2 * p + 1]) + 1];
+    for (int i = 0; i < n_sets; ++i) start[i + 1] += start[i];
+    {
+        std::vector<int32_t> fill(start.begin(), start.end() - 1);
+        for (int p = 0; p < n_pairs; ++p)
+            larger[fill[std::min(pairs[2 * p], pairs[2 * p + 1])]++] = std::max(pairs[2 * p], pairs[2 * p + 1]);
+    }
+    for (int a = 0; a < n_sets; ++a)
+        for (int k = start[a]; k < start[a + 1]; ++k) {
+            if (seen[larger[k]] == a) {
+                g_create_error = "ps_view_graph_filter: two pairs join the same two sets";
+                return PS_ERR_ARG;
+            }
+            seen[larger[k]] = a;
+        }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (n_pairs > 0 && ps_pointer_device(d_two_view) != device) return PS_ERR_ARG;
+    if (d_kept && ps_pointer_device(d_kept) != device) return PS_ERR_ARG;
+    if (n_pairs == 0) {
+        std::memset(report, 0, sizeof(*report));
+        return PS_OK;
+    }
+    const char* err = nullptr;
+    std::vector<uint8_t> kp(n_pairs);
+    std::vector<ps_cycle_stats> cs(stats ? n_pairs : 0);
+    ps_view_graph_report rep{};
+    const int n = run_view_graph_filter(n_sets, n_pairs, pairs, d_two_view, *prm, kp.data(), stats ? cs.data() : nullptr, d_kept, &rep,
+                                        nullptr, &err);
+    const int rc = finish("ps_view_graph_filter", n, err);
+    if (rc == PS_OK) {
+        std::memcpy(keep, kp.data(), kp.size());
+        if (stats) std::memcpy(stats, cs.data(), cs.size() * sizeof(ps_cycle_stats));
+        *report = rep;
+    }
+    return rc;
+}
+
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)
 {
     if (bytes == 0) return PS_OK;

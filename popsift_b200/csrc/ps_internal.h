@@ -6,6 +6,7 @@
 #include "popsift_b200_triangulate.h"
 #include "popsift_b200_bundle.h"
 #include "popsift_b200_global.h"
+#include "popsift_b200_viewgraph.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
@@ -312,5 +313,12 @@ int run_global_positioning(int n_sets, const int32_t* n_feat, const ps_feature* 
                            const uint8_t* registered, int n_tracks, const int32_t* track_start, const int32_t* members, int n_members,
                            const ps_position_params& prm, ps_rigid* poses_out, uint8_t* positioned, double* X_out,
                            ps_position_report* report, bool* bad, cudaStream_t st, const char** err);
+
+// view-graph filter (include/popsift_b200_viewgraph.h, k_viewgraph.cu), arguments already validated (duplicates included)
+// and n_pairs > 0.  Synchronous on `st`; keep, stats (optional), d_kept (optional) and *report are written when it returns
+// >= 0.  Returns the number of kernels launched or -1 (*err set).
+int run_view_graph_filter(int n_sets, int n_pairs, const int32_t* pairs, const ps_two_view* d_two_view, const ps_view_graph_params& prm,
+                          uint8_t* keep, ps_cycle_stats* stats, ps_two_view* d_kept, ps_view_graph_report* report, cudaStream_t st,
+                          const char** err);
 
 } // namespace psb
