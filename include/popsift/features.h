@@ -390,6 +390,40 @@ struct ViewGraph
 ViewGraph filterViewGraph(int n_sets, const std::vector<std::pair<int, int>>& pairs, const std::vector<TwoViewPose>& poses,
                           const ViewGraphParams& params = ViewGraphParams());
 
+/// Settings of twoViewGeometries' classification (same fields and rules as ps_two_view_config_params in
+/// popsift_b200_twoview.h; the pure-rotation test uses PoseParams::threshold).
+struct TwoViewConfigParams
+{
+    int    min_inliers = 15;
+    double min_ef_ratio = 0.95;
+    double max_h_ratio = 0.8;
+    double min_rotation_ratio = 0.9;
+};
+
+/// One pair's two-view configuration (ps_two_view_info and the record that replaces ps_relative_pose_batch's): config is
+/// Degenerate, General, Planar, Panoramic or Uncalibrated (PS_TV_*); pose the essential pose (General), the homography's
+/// (Planar), the rotation with t = 0 (Panoramic) or zero; normal the unit plane normal in the left frame (Planar);
+/// tri_angle the median triangulation angle of the rows in front, degrees; the inlier counts of E, F and H and the H
+/// inliers the pure rotation explains.
+struct TwoViewGeometry
+{
+    enum { Degenerate = 0, General = 1, Planar = 2, Panoramic = 3, Uncalibrated = 4 };
+    int         config = Degenerate;
+    TwoViewPose pose;
+    float       normal[3] = {0.0f, 0.0f, 0.0f};
+    float       tri_angle = 0.0f;
+    int         n_e = 0, n_f = 0, n_h = 0, n_rotation = 0;
+};
+
+/// Two-view configuration of matched calibrated pairs on the device (an addition to the reference's interface; C ABI
+/// ps_match_correspondences, ps_verify_batch with the homography and the fundamental matrix, ps_relative_pose_batch, then
+/// ps_two_view_config_batch in popsift_b200_twoview.h): the three RANSACs use `params`.  The poses feed
+/// rotationAveraging and filterViewGraph unchanged.  Throws like relativePoses.
+std::vector<TwoViewGeometry> twoViewGeometries(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                               const std::vector<std::vector<int>>& matches, const std::vector<Camera>& cameras,
+                                               const PoseParams& params = PoseParams(),
+                                               const TwoViewConfigParams& config = TwoViewConfigParams());
+
 /// Settings of globalPositioning (same fields and rules as ps_position_params).
 struct PositionParams
 {

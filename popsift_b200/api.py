@@ -182,6 +182,24 @@ CYCLE_STATS_DTYPE = np.dtype([("n_triangles", "<i4"), ("n_consistent", "<i4"), (
 assert C.sizeof(PsViewGraphParams) == 32 and C.sizeof(PsCycleStats) == 12 and C.sizeof(PsViewGraphReport) == 32
 assert CYCLE_STATS_DTYPE.itemsize == 12
 
+class PsTwoViewConfigParams(C.Structure):
+    """ps_two_view_config_params (32 bytes)"""
+    _fields_ = [("min_inliers", C.c_int32), ("threshold", C.c_float), ("min_ef_ratio", C.c_double), ("max_h_ratio", C.c_double),
+                ("min_rotation_ratio", C.c_double)]
+
+
+class PsTwoViewInfo(C.Structure):
+    """ps_two_view_info (40 bytes)"""
+    _fields_ = [("config", C.c_int32), ("n_e", C.c_int32), ("n_f", C.c_int32), ("n_h", C.c_int32), ("n_rotation", C.c_int32),
+                ("tri_angle", C.c_float), ("normal", C.c_float * 3), ("pad_", C.c_int32)]
+
+
+# ps_two_view_info as a numpy record; TV_CONFIG names its config codes (PS_TV_*)
+TWO_VIEW_INFO_DTYPE = np.dtype([("config", "<i4"), ("n_e", "<i4"), ("n_f", "<i4"), ("n_h", "<i4"), ("n_rotation", "<i4"),
+                                ("tri_angle", "<f4"), ("normal", "<f4", 3), ("pad_", "<i4")])
+TV_CONFIG = ("degenerate", "general", "planar", "panoramic", "uncalibrated")
+assert C.sizeof(PsTwoViewConfigParams) == 32 and C.sizeof(PsTwoViewInfo) == 40 and TWO_VIEW_INFO_DTYPE.itemsize == 40
+
 RA_TERMINATION = ("max_iters", "step_tol", "no_pairs")
 GP_TERMINATION = ("max_iters", "function_tol", "no_observations")
 assert C.sizeof(PsRotationParams) == 40 and C.sizeof(PsRotationReport) == 40
@@ -210,6 +228,8 @@ BUNDLE_EXPORTS = ["ps_bundle_adjust"]
 GLOBAL_EXPORTS = ["ps_rotation_averaging", "ps_global_positioning"]
 # view-graph cleaning, declared in popsift_b200_viewgraph.h (same library)
 VIEWGRAPH_EXPORTS = ["ps_view_graph_filter"]
+# two-view configuration, declared in popsift_b200_twoview.h (same library)
+TWOVIEW_EXPORTS = ["ps_two_view_config_batch"]
 
 _lib = None
 
@@ -287,6 +307,10 @@ def load_library():
     if hasattr(L, "ps_view_graph_filter"):
         L.ps_view_graph_filter.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(PsViewGraphParams), C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.POINTER(PsViewGraphReport)]
+    if hasattr(L, "ps_two_view_config_batch"):
+        L.ps_two_view_config_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsTwoViewConfigParams), C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -1037,6 +1061,113 @@ def relative_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device
     return res
 
 
+TwoViewGeometry = namedtuple("TwoViewGeometry", "config pose normal tri_angle n_e n_f n_h n_rotation inlier_rows front_rows")
+TwoViewGeometry.__doc__ = """One pair's two-view configuration (ps_two_view_config_batch, popsift_b200_twoview.h): config, a name of
+TV_CONFIG; pose, the TwoView that replaces ps_relative_pose_batch's (the essential pose for "general", the homography's
+for "planar", the rotation alone with t = 0 for "panoramic", zero otherwise); the unit plane normal (3,) in the left frame
+("planar", else zero); tri_angle, the median triangulation angle of the bit-1 rows in degrees; the inlier counts of E, F
+and H and the H inliers the pure rotation explains; the rows with bit 0 and with bit 1 (left descriptor rows from
+two_view_geometries, correspondence indices from two_view_config_correspondences)."""
+
+
+def _two_view_config_params(threshold=4.0, min_inliers=15, min_ef_ratio=0.95, max_h_ratio=0.8, min_rotation_ratio=0.9):
+    return PsTwoViewConfigParams(int(min_inliers), float(threshold), float(min_ef_ratio), float(max_h_ratio), float(min_rotation_ratio))
+
+
+def _two_view_config_dev(lib, bufs, device, d_corr, start, n_corr, cams, pprm: PsPoseParams, cprm: PsTwoViewConfigParams, points=False):
+    """The three RANSACs and ps_two_view_config_batch on device correspondences: ps_verify_batch with the homography and the
+    fundamental matrix and ps_relative_pose_batch, all with pprm's threshold, samples, seed and refit.  Returns (d_out,
+    d_mask, host two-view records, mask (rows,) uint8, points or None, info (P,) TWO_VIEW_INFO_DTYPE)."""
+    P = len(start)
+    rows = int(max((int(a) + int(b) for a, b in zip(start, n_corr)), default=0))
+    c_start = np.ascontiguousarray(start, np.int32)
+    c_n = np.ascontiguousarray(n_corr, np.int32)
+    d_h, d_hn, d_hmask = bufs.alloc(P * 36), bufs.alloc(P * 4), bufs.alloc(rows)
+    d_f, d_fn, d_fmask = bufs.alloc(P * 36), bufs.alloc(P * 4), bufs.alloc(rows)
+    for model, dm, dn, dk in ((0, d_h, d_hn, d_hmask), (1, d_f, d_fn, d_fmask)):
+        vp = PsVerifyParams(model, pprm.n_samples, pprm.threshold, pprm.refine, pprm.seed)
+        _check(lib, lib.ps_verify_batch(device, P, d_corr, c_start.ctypes.data, c_n.ctypes.data, C.byref(vp), dm, dn, dk, None),
+               "ps_verify_batch")
+    d_e, d_emask = _pose_dev(lib, bufs, device, d_corr, start, n_corr, cams, pprm)[:2]
+    d_out, d_mask = bufs.alloc(P * 128), bufs.alloc(rows)
+    d_pts = bufs.alloc(rows * 16) if points else None
+    info = np.zeros(max(P, 1), TWO_VIEW_INFO_DTYPE)
+    rc = lib.ps_two_view_config_batch(device, P, d_corr, c_start.ctypes.data, c_n.ctypes.data, cams.ctypes.data, d_e, d_emask, d_fn,
+                                      d_h, d_hmask, C.byref(cprm), d_out, d_mask, d_pts, info.ctypes.data)
+    _check(lib, rc, "ps_two_view_config_batch")
+    return (d_out, d_mask, bufs.download(d_out, P, TWO_VIEW_DTYPE), bufs.download(d_mask, rows, np.uint8),
+            bufs.download(d_pts, (rows, 4), np.float32) if points else None, info[:P].copy())
+
+
+def _two_view_geometry(rec, info, mask, pts, rows) -> "TwoViewGeometry":
+    two = TwoView(rec["E"].copy(), rec["F"].copy(), rec["R"].copy(), rec["t"].copy(), int(rec["n_inliers"]), int(rec["n_front"]),
+                  mask.copy(), pts)
+    return TwoViewGeometry(TV_CONFIG[int(info["config"])], two, info["normal"].copy(), float(info["tri_angle"]), int(info["n_e"]),
+                           int(info["n_f"]), int(info["n_h"]), int(info["n_rotation"]), rows[(mask & 1) != 0].copy(),
+                           rows[(mask & 2) != 0].copy())
+
+
+def two_view_config_correspondences(corrs, cameras, threshold=4.0, n_samples=1024, seed=0, refine=True, points=False, device=0,
+                                    **config):
+    """Two-view configuration on host correspondences (C ABI ps_two_view_config_batch in popsift_b200_twoview.h, after
+    ps_verify_batch's homography and fundamental matrix and ps_relative_pose_batch, all with the given threshold, n_samples,
+    seed and refine; an addition to the reference's interface).  `corrs` and `cameras` as for relative_pose_correspondences;
+    config: min_inliers (15), min_ef_ratio (0.95), max_h_ratio (0.8), min_rotation_ratio (0.9); the pure-rotation test uses
+    `threshold`.  Returns a TwoViewGeometry per pair, its rows the correspondence indices."""
+    lib = load_library()
+    pprm = _pose_params(threshold, n_samples, seed, refine)
+    cprm = _two_view_config_params(threshold, **config)
+    arrs = [np.ascontiguousarray(c, np.float32).reshape(-1, 4) for c in corrs]
+    cams = np.asarray(cameras, np.float32)
+    if cams.shape != (len(arrs), 2, 4):
+        raise PopSiftError("one (left, right) pair of (fx, fy, cx, cy) per correspondence array expected")
+    cams = _c_cameras(cams)
+    n_corr = np.array([len(a) for a in arrs], np.int32)
+    start = np.concatenate([[0], np.cumsum(n_corr)])[:len(arrs)].astype(np.int32)
+    bufs = _DevBuffers(lib)
+    try:
+        allc = np.concatenate(arrs) if arrs else np.zeros((0, 4), np.float32)
+        _, _, tv, mask, pts, info = _two_view_config_dev(lib, bufs, device, bufs.upload(allc), start, n_corr, cams, pprm, cprm, points)
+    finally:
+        bufs.free()
+    out = []
+    for p in range(len(arrs)):
+        a, n = int(start[p]), int(n_corr[p])
+        out.append(_two_view_geometry(tv[p], info[p], mask[a:a + n], pts[a:a + n].copy() if points else None, np.arange(n, dtype=np.int32)))
+    return out
+
+
+def two_view_geometries(sets, pairs, cameras, matches=None, flags=0, u8=False, device=None, points=False, threshold=4.0, n_samples=1024,
+                        seed=0, refine=True, **config):
+    """Two-view configuration of matched pairs without leaving the device: relative_poses' chain (matching unless `matches`
+    is given, ps_match_correspondences), ps_verify_batch with the homography and the fundamental matrix and
+    ps_relative_pose_batch on the same rows (threshold, n_samples, seed and refine for all three), then
+    ps_two_view_config_batch.  `sets` are FeaturesDev objects, `cameras` one (fx, fy, cx, cy) per set, config
+    two_view_config_correspondences'.  Returns a TwoViewGeometry per pair, its rows the left descriptor rows; its pose feeds
+    rotation_averaging and filter_view_graph unchanged."""
+    lib = load_library()
+    pairs = [(int(a), int(b)) for a, b in pairs]
+    pprm = _pose_params(threshold, n_samples, seed, refine)
+    cprm = _two_view_config_params(threshold, **config)
+    cam = np.asarray(cameras, np.float32).reshape(-1, 4)
+    if len(cam) != len(sets):
+        raise PopSiftError("one camera per set expected")
+    bufs = _DevBuffers(lib)
+    try:
+        _, device, rows, _, d_corr, d_src, start, n_corr = _matched_rows(lib, bufs, sets, pairs, matches, flags, u8, device,
+                                                                        u8 and matches is None)
+        cams = _c_cameras([cam[i] for lr in pairs for i in lr])
+        _, _, tv, mask, pts, info = _two_view_config_dev(lib, bufs, device, d_corr, start, n_corr, cams, pprm, cprm, points)
+        src = bufs.download(d_src, rows, np.int32)
+    finally:
+        bufs.free()
+    out = []
+    for p in range(len(pairs)):
+        a, n = int(start[p]), int(n_corr[p])
+        out.append(_two_view_geometry(tv[p], info[p], mask[a:a + n], pts[a:a + n].copy() if points else None, src[a:a + n]))
+    return out
+
+
 Tracks = namedtuple("Tracks", "start set feature track_of n_components n_conflicting n_short")
 Tracks.__doc__ = """Feature tracks: track t's members are set[start[t]:start[t + 1]] / feature[start[t]:start[t + 1]]
 (ascending by set); track_of[i][f] is feature f of set i's track, or -1; the counts of dropped components."""
@@ -1461,7 +1592,7 @@ def global_positioning(sets, tracks, cameras, rotations, registered, device=None
 
 
 def global_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=None, min_length=2, max_pair_error=5.0, pose=None,
-                 rotation=None, position=None, view_graph=None) -> GlobalPoses:
+                 rotation=None, position=None, view_graph=None, two_view=None) -> GlobalPoses:
     """Poses for every image from images and intrinsics alone, without leaving the device: relative_poses' chain
     (matching unless `matches` is given, correspondences, ps_relative_pose_batch with the parameters in the dict `pose`),
     ps_rotation_averaging on its records (dict `rotation`: rotation_averaging's params), ps_tracks_from_matches on the
@@ -1469,7 +1600,11 @@ def global_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=N
     (the other pairs contribute no correspondence), then ps_global_positioning on those tracks (dict `position`:
     global_positioning's params).  A dict `view_graph` (filter_view_graph's params but min_inliers, which is the
     rotation's) cleans the view graph first: ps_view_graph_filter on the relative poses, rotation averaging on the kept
-    pairs only, and the dropped pairs get pair_error +inf (so they contribute no correspondence).  `sets` are FeaturesDev
+    pairs only, and the dropped pairs get pair_error +inf (so they contribute no correspondence).  A dict `two_view`
+    (two_view_config_correspondences' config) classifies the pairs first: ps_verify_batch's homography and fundamental
+    matrix with the pose parameters, then ps_two_view_config_batch, whose records and masks replace ps_relative_pose_batch's
+    for everything after it (planar pairs posed from the homography, panoramic pairs by their rotation alone with the
+    rotation-test rows as tracks, the other non-general pairs dropped).  `sets` are FeaturesDev
     objects and `cameras` one (fx, fy, cx, cy) per set.  The result feeds triangulate() and then bundle_adjust()."""
     lib = load_library()
     pairs = [(int(a), int(b)) for a, b in pairs]
@@ -1480,6 +1615,8 @@ def global_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=N
         if "min_inliers" in view_graph:
             raise PopSiftError("view_graph takes min_inliers from the rotation parameters")
         vgprm = _view_graph_params(min_inliers=rprm.min_inliers, **view_graph)
+    if two_view is not None:
+        cprm = _two_view_config_params(pprm.threshold, **two_view)
     cam = np.asarray(cameras, np.float32).reshape(-1, 4)
     if len(cam) != len(sets):
         raise PopSiftError("one camera per set expected")
@@ -1487,7 +1624,11 @@ def global_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=N
     try:
         _, device, rows, d_match, d_corr, d_src, start, n_corr = _matched_rows(lib, bufs, sets, pairs, matches, flags, u8, device,
                                                                               u8 and matches is None)
-        d_out, d_mask = _pose_dev(lib, bufs, device, d_corr, start, n_corr, _c_cameras([cam[i] for lr in pairs for i in lr]), pprm)[:2]
+        pcams = _c_cameras([cam[i] for lr in pairs for i in lr])
+        if two_view is None:
+            d_out, d_mask = _pose_dev(lib, bufs, device, d_corr, start, n_corr, pcams, pprm)[:2]
+        else:
+            d_out, d_mask = _two_view_config_dev(lib, bufs, device, d_corr, start, n_corr, pcams, pprm, cprm)[:2]
         if view_graph is None:
             R, reg, perr, rrep = _rotation_dev(lib, device, len(sets), pairs, d_out, rprm)
         else:

@@ -12,6 +12,7 @@
 #include "popsift_b200_bundle.h"
 #include "popsift_b200_global.h"
 #include "popsift_b200_viewgraph.h"
+#include "popsift_b200_twoview.h"
 
 #include <algorithm>
 #include <cmath>
@@ -389,6 +390,96 @@ std::vector<TwoViewPose> relativePoses(const std::vector<FeaturesDev*>& sets, co
             if (m & 1) g.inlier_rows.push_back(h_src[b.start[p] + k]);
             if (m & 2) g.front_rows.push_back(h_src[b.start[p] + k]);
         }
+    }
+    return out;
+}
+
+std::vector<TwoViewGeometry> twoViewGeometries(const std::vector<FeaturesDev*>& sets, const std::vector<std::pair<int, int>>& pairs,
+                                               const std::vector<std::vector<int>>& matches, const std::vector<Camera>& cameras,
+                                               const PoseParams& params, const TwoViewConfigParams& config)
+{
+    if (matches.size() != pairs.size()) throw std::runtime_error("popsift::twoViewGeometries: one match list per pair expected");
+    if (cameras.size() != sets.size()) throw std::runtime_error("popsift::twoViewGeometries: one camera per set expected");
+    const Batch b("twoViewGeometries", sets, pairs);
+    std::vector<TwoViewGeometry> out(pairs.size());
+    for (TwoViewGeometry& g : out) {
+        TwoViewPose& v = g.pose;
+        std::fill(v.E, v.E + 9, 0.0f); std::fill(v.F, v.F + 9, 0.0f); std::fill(v.R, v.R + 9, 0.0f); std::fill(v.t, v.t + 3, 0.0f);
+        v.n_inliers = v.n_front = 0;
+    }
+    const size_t nr = std::max<size_t>(b.rows, 1), np = pairs.size();
+    DevBuf match(nr * 3 * sizeof(int32_t), b.who);
+    b.upload(matches, static_cast<int32_t*>(match.p));
+    if (pairs.empty()) return out;
+    DevBuf corr(nr * 4 * sizeof(float), b.who), src(nr * sizeof(int32_t), b.who), hmask(nr, b.who), fmask(nr, b.who), emask(nr, b.who),
+        mask(nr, b.who), hom(np * 9 * sizeof(float), b.who), fund(np * 9 * sizeof(float), b.who), hn(np * sizeof(int32_t), b.who),
+        fn(np * sizeof(int32_t), b.who), ess(np * sizeof(ps_two_view), b.who), two(np * sizeof(ps_two_view), b.who);
+    std::vector<int32_t> start(b.start.begin(), b.start.end()), n_corr(np, 0);
+    check(ps_match_correspondences(b.dev, (int)sets.size(), b.feat.data(), b.rev.data(), b.n_desc.data(), (int)np, b.flat.data(),
+                                   static_cast<const int32_t*>(match.p), static_cast<float*>(corr.p), static_cast<int32_t*>(src.p), n_corr.data()),
+          b.who);
+    std::vector<ps_camera> cams(2 * np);
+    for (size_t p = 0; p < np; ++p)
+        for (int k = 0; k < 2; ++k) {
+            const Camera& c = cameras[k ? pairs[p].second : pairs[p].first];
+            cams[2 * p + k] = ps_camera{c.fx, c.fy, c.cx, c.cy};
+        }
+    const float* d_corr = static_cast<const float*>(corr.p);
+    ps_verify_params vp{};
+    vp.n_samples = params.n_samples;
+    vp.threshold = params.threshold;
+    vp.refine = params.refine ? 1 : 0;
+    vp.seed = params.seed;
+    vp.model = PS_GEOM_HOMOGRAPHY;
+    check(ps_verify_batch(b.dev, (int)np, d_corr, start.data(), n_corr.data(), &vp, static_cast<float*>(hom.p), static_cast<int32_t*>(hn.p),
+                          static_cast<uint8_t*>(hmask.p), nullptr),
+          b.who);
+    vp.model = PS_GEOM_FUNDAMENTAL;
+    check(ps_verify_batch(b.dev, (int)np, d_corr, start.data(), n_corr.data(), &vp, static_cast<float*>(fund.p), static_cast<int32_t*>(fn.p),
+                          static_cast<uint8_t*>(fmask.p), nullptr),
+          b.who);
+    ps_pose_params pp{};
+    pp.n_samples = params.n_samples;
+    pp.threshold = params.threshold;
+    pp.refine = params.refine ? 1 : 0;
+    pp.seed = params.seed;
+    check(ps_relative_pose_batch(b.dev, (int)np, d_corr, start.data(), n_corr.data(), cams.data(), &pp, static_cast<ps_two_view*>(ess.p),
+                                 static_cast<uint8_t*>(emask.p), nullptr, nullptr),
+          b.who);
+    ps_two_view_config_params cp{};
+    cp.min_inliers = config.min_inliers;
+    cp.threshold = params.threshold;
+    cp.min_ef_ratio = config.min_ef_ratio;
+    cp.max_h_ratio = config.max_h_ratio;
+    cp.min_rotation_ratio = config.min_rotation_ratio;
+    std::vector<ps_two_view_info> info(np);
+    check(ps_two_view_config_batch(b.dev, (int)np, d_corr, start.data(), n_corr.data(), cams.data(), static_cast<const ps_two_view*>(ess.p),
+                                   static_cast<const uint8_t*>(emask.p), static_cast<const int32_t*>(fn.p), static_cast<const float*>(hom.p),
+                                   static_cast<const uint8_t*>(hmask.p), &cp, static_cast<ps_two_view*>(two.p), static_cast<uint8_t*>(mask.p),
+                                   nullptr, info.data()),
+          b.who, "ps_two_view_config_batch");
+    std::vector<ps_two_view> h_two(np);
+    std::vector<int32_t> h_src(b.rows);
+    std::vector<uint8_t> h_mask(b.rows);
+    check(ps_dev_to_host(h_two.data(), two.p, np * sizeof(ps_two_view)), b.who);
+    check(ps_dev_to_host(h_src.data(), src.p, b.rows * sizeof(int32_t)), b.who);
+    check(ps_dev_to_host(h_mask.data(), mask.p, b.rows), b.who);
+    for (size_t p = 0; p < np; ++p) {
+        const ps_two_view& v = h_two[p];
+        TwoViewGeometry& g = out[p];
+        std::copy(v.E, v.E + 9, g.pose.E); std::copy(v.F, v.F + 9, g.pose.F); std::copy(v.R, v.R + 9, g.pose.R); std::copy(v.t, v.t + 3, g.pose.t);
+        g.pose.n_inliers = v.n_inliers;
+        g.pose.n_front = v.n_front;
+        for (int k = 0; k < n_corr[p]; ++k) {
+            const uint8_t m = h_mask[b.start[p] + k];
+            if (m & 1) g.pose.inlier_rows.push_back(h_src[b.start[p] + k]);
+            if (m & 2) g.pose.front_rows.push_back(h_src[b.start[p] + k]);
+        }
+        const ps_two_view_info& in = info[p];
+        g.config = in.config;
+        std::copy(in.normal, in.normal + 3, g.normal);
+        g.tri_angle = in.tri_angle;
+        g.n_e = in.n_e; g.n_f = in.n_f; g.n_h = in.n_h; g.n_rotation = in.n_rotation;
     }
     return out;
 }

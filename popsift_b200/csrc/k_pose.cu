@@ -29,7 +29,6 @@ namespace psb {
 
 namespace {
 
-struct PCam { double fxl, fyl, cxl, cyl, fxr, fyr, cxr, cyr; float t2, pad; };
 struct PSolveItem { int pair, s0; };
 struct PScoreItem { int pair, k0, c0, c1; };
 
@@ -46,8 +45,9 @@ __global__ void __launch_bounds__(kCalThreads) pose_calibrate_kernel(const VPair
     const PCam K = cams[blockIdx.x];
     for (int i = threadIdx.x; i < P.n; i += blockDim.x) {
         const float4 v = corr[P.start + i];
-        pts[P.start + i] = make_float4((float)(((double)v.x - K.cxl) / K.fxl), (float)(((double)v.y - K.cyl) / K.fyl),
-                                       (float)(((double)v.z - K.cxr) / K.fxr), (float)(((double)v.w - K.cyr) / K.fyr));
+        float c[4];
+        pose_calibrate(K, v.x, v.y, v.z, v.w, c);
+        pts[P.start + i] = make_float4(c[0], c[1], c[2], c[3]);
     }
 }
 
@@ -140,23 +140,6 @@ __global__ void pose_taps_kernel(const float* __restrict__ models, const int32_t
     const int c = counts[h];
     tap_counts[h] = c;
     for (int e = 0; e < 9; ++e) tap_models[9 * h + e] = c >= 0 ? models[9 * h + e] : 0.0f;
-}
-
-// F = K_r^-T E K_l^-1 (double), scaled like ps_verify_batch's F
-__device__ __forceinline__ void pose_pixels(const double* E, const PCam& K, double* F)
-{
-    double M[9], N[9];
-    for (int r = 0; r < 3; ++r) {
-        M[3 * r] = E[3 * r] / K.fxl;
-        M[3 * r + 1] = E[3 * r + 1] / K.fyl;
-        M[3 * r + 2] = E[3 * r + 2] - (K.cxl / K.fxl) * E[3 * r] - (K.cyl / K.fyl) * E[3 * r + 1];
-    }
-    for (int c = 0; c < 3; ++c) {
-        N[c] = M[c] / K.fxr;
-        N[3 + c] = M[3 + c] / K.fyr;
-        N[6 + c] = M[6 + c] - (K.cxr / K.fxr) * M[c] - (K.cyr / K.fyr) * M[3 + c];
-    }
-    pose_scale(N, F);
 }
 
 __global__ void __launch_bounds__(kSelectThreads, 1) pose_select_kernel(const VPair* __restrict__ pairs, const PCam* __restrict__ cams,
@@ -297,11 +280,7 @@ int run_relative_pose_batch(int n_pairs, const float* corr, const int32_t* corr_
     for (int p = 0; p < n_pairs; ++p) {
         total_rows = std::max(total_rows, (long long)corr_start[p] + n_corr[p]);
         vp[p] = {corr_start[p], n_corr[p], 0};
-        const ps_camera& l = cams[2 * p];
-        const ps_camera& r = cams[2 * p + 1];
-        const double fbar = ((double)l.fx + (double)l.fy + (double)r.fx + (double)r.fy) / 4.0;
-        const double ts = (double)prm.threshold / fbar;
-        pc[p] = {l.fx, l.fy, l.cx, l.cy, r.fx, r.fy, r.cx, r.cy, (float)(ts * ts), 0.0f};
+        pc[p] = pose_cam(cams[2 * p], cams[2 * p + 1], prm.threshold);
         for (int s0 = 0; s0 < ns; s0 += kPoseSolveThreads) solve.push_back({p, s0});
     }
     if (solve.size() > 0x7fffffffu) { *err = "ps_relative_pose_batch: too many work items"; return -1; }

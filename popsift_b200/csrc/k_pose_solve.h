@@ -1,5 +1,6 @@
 // The calibrated two-view math of ps_relative_pose_batch (include/popsift_b200_pose.h), in double: the five-point solver,
-// the 3 x 3 SVD behind the essential-matrix projection and the pose decomposition, and the triangulation / cheirality rule.
+// the 3 x 3 SVD behind the essential-matrix projection and the pose decomposition, the triangulation / cheirality rule,
+// the calibration of the rows and the pixel F.
 // One definition for the kernels (k_pose.cu) and the host check (tests/cpp/pose_solver_check.cpp).  Arrays indexed at
 // run time live in local memory on the device.
 #pragma once
@@ -13,6 +14,28 @@ namespace psb {
 constexpr int kPoseSlots = 10;               // hypotheses per sample: at most ten real solutions
 constexpr double kPoseNullTol = 1e-10;       // 5 x 9 pivot: below this times the largest entry, the sample gives nothing
 constexpr double kPoseElimTol = 1e-12;       // 10 x 20 pivot: below this times the largest entry, the sample gives nothing
+
+// One pair's intrinsics in double (left, right) and the squared calibrated threshold (ps_relative_pose_batch's rule 1)
+struct PCam { double fxl, fyl, cxl, cyl, fxr, fyr, cxr, cyr; float t2, pad; };
+
+// host: the PCam of cameras l, r (ps_camera) at `threshold` pixels: f = (fx_l + fy_l + fx_r + fy_r) / 4 in double,
+// t2 = (float)((threshold / f)^2)
+template <class Cam>
+inline PCam pose_cam(const Cam& l, const Cam& r, float threshold)
+{
+    const double fbar = ((double)l.fx + (double)l.fy + (double)r.fx + (double)r.fy) / 4.0;
+    const double ts = (double)threshold / fbar;
+    return {l.fx, l.fy, l.cx, l.cy, r.fx, r.fy, r.cx, r.cy, (float)(ts * ts), 0.0f};
+}
+
+// rule 1: a pixel row (x_l, y_l, x_r, y_r) in calibrated coordinates, x^ = (x - cx) / fx in double, rounded once
+PSV_HD void pose_calibrate(const PCam& K, float xl, float yl, float xr, float yr, float* c)
+{
+    c[0] = (float)(((double)xl - K.cxl) / K.fxl);
+    c[1] = (float)(((double)yl - K.cyl) / K.fyl);
+    c[2] = (float)(((double)xr - K.cxr) / K.fxr);
+    c[3] = (float)(((double)yr - K.cyr) / K.fyr);
+}
 
 // ---- polynomials in (x, y, z) of E = x X + y Y + z Z + W ----
 // linear: [x, y, z, 1]; quadratic: [x^2, xy, y^2, xz, yz, z^2, x, y, z, 1]; cubic (the elimination order):
@@ -528,6 +551,23 @@ PSV_HD bool pose_scale(const double* m, double* out)
     const double k = (rb < 0.0 ? -1.0 : 1.0) / n;
     for (int j = 0; j < 9; ++j) out[j] = m[j] * k;
     return true;
+}
+
+// F = K_r^-T E K_l^-1 (double), scaled like ps_verify_batch's F
+PSV_HD void pose_pixels(const double* E, const PCam& K, double* F)
+{
+    double M[9], N[9];
+    for (int r = 0; r < 3; ++r) {
+        M[3 * r] = E[3 * r] / K.fxl;
+        M[3 * r + 1] = E[3 * r + 1] / K.fyl;
+        M[3 * r + 2] = E[3 * r + 2] - (K.cxl / K.fxl) * E[3 * r] - (K.cyl / K.fyl) * E[3 * r + 1];
+    }
+    for (int c = 0; c < 3; ++c) {
+        N[c] = M[c] / K.fxr;
+        N[3 + c] = M[3 + c] / K.fyr;
+        N[6 + c] = M[6 + c] - (K.cxr / K.fxr) * M[c] - (K.cyr / K.fyr) * M[3 + c];
+    }
+    pose_scale(N, F);
 }
 
 } // namespace psb

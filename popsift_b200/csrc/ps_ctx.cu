@@ -15,6 +15,7 @@
 #include "popsift_b200_triangulate.h"
 #include "popsift_b200_bundle.h"
 #include "popsift_b200_global.h"
+#include "popsift_b200_twoview.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1646,6 +1647,65 @@ extern "C" int ps_view_graph_filter(int device, int n_sets, int n_pairs, const i
         if (stats) std::memcpy(stats, cs.data(), cs.size() * sizeof(ps_cycle_stats));
         *report = rep;
     }
+    return rc;
+}
+
+// [lo, hi) byte ranges of device arguments; true when two of them intersect
+static bool ranges_overlap(const void* a, size_t na, const void* b, size_t nb)
+{
+    if (!a || !b || na == 0 || nb == 0) return false;
+    const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+    return a0 < b0 + nb && b0 < a0 + na;
+}
+
+extern "C" int ps_two_view_config_batch(int device, int n_pairs, const float* d_corr, const int32_t* corr_start, const int32_t* n_corr,
+                                        const ps_camera* cams, const ps_two_view* d_essential, const uint8_t* d_essential_mask,
+                                        const int32_t* d_f_inliers, const float* d_homography, const uint8_t* d_h_mask,
+                                        const ps_two_view_config_params* prm, ps_two_view* d_out, uint8_t* d_out_mask, float* d_points,
+                                        ps_two_view_info* info)
+{
+    if (n_pairs < 0 || !prm || !info) return PS_ERR_ARG;
+    if (prm->min_inliers < 0 || !std::isfinite(prm->threshold) || !(prm->threshold > 0.0f)) return PS_ERR_ARG;
+    for (const double r : {prm->min_ef_ratio, prm->max_h_ratio, prm->min_rotation_ratio})
+        if (!(r >= 0.0 && r <= 1.0)) return PS_ERR_ARG;
+    if (n_pairs == 0) return PS_OK;
+    if (!corr_start || !n_corr || !cams) return PS_ERR_ARG;
+    int64_t rows = 0;
+    for (int p = 0; p < n_pairs; ++p) {
+        if (corr_start[p] < 0 || n_corr[p] < 0) return PS_ERR_ARG;
+        rows = std::max<int64_t>(rows, (int64_t)corr_start[p] + n_corr[p]);
+    }
+    for (int k = 0; k < 2 * n_pairs; ++k) {
+        const ps_camera& c = cams[k];
+        if (!std::isfinite(c.fx) || !(c.fx > 0.0f) || !std::isfinite(c.fy) || !(c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
+            return PS_ERR_ARG;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    for (const void* d : {(const void*)d_essential, (const void*)d_f_inliers, (const void*)d_homography, (const void*)d_out})
+        if (ps_pointer_device(d) != device) return PS_ERR_ARG;
+    if (d_points && ps_pointer_device(d_points) != device) return PS_ERR_ARG;
+    if (rows > 0) {
+        for (const void* d : {(const void*)d_corr, (const void*)d_essential_mask, (const void*)d_h_mask, (const void*)d_out_mask})
+            if (ps_pointer_device(d) != device) return PS_ERR_ARG;
+        if (reinterpret_cast<uintptr_t>(d_corr) & 15u) return PS_ERR_ARG;
+    }
+    // no output may overlap an input or another output
+    const size_t P = (size_t)n_pairs, R = (size_t)rows;
+    const std::pair<const void*, size_t> in[] = {{d_corr, 16 * R}, {d_essential, sizeof(ps_two_view) * P}, {d_essential_mask, R},
+                                                 {d_f_inliers, 4 * P}, {d_homography, 36 * P}, {d_h_mask, R}};
+    const std::pair<const void*, size_t> out[] = {{d_out, sizeof(ps_two_view) * P}, {d_out_mask, R}, {d_points, d_points ? 16 * R : 0}};
+    for (int o = 0; o < 3; ++o) {
+        for (const auto& i : in)
+            if (ranges_overlap(out[o].first, out[o].second, i.first, i.second)) return PS_ERR_ARG;
+        for (int o2 = o + 1; o2 < 3; ++o2)
+            if (ranges_overlap(out[o].first, out[o].second, out[o2].first, out[o2].second)) return PS_ERR_ARG;
+    }
+    const char* err = nullptr;
+    std::vector<ps_two_view_info> inf(n_pairs);
+    const int n = run_two_view_config_batch(n_pairs, d_corr, corr_start, n_corr, cams, d_essential, d_essential_mask, d_f_inliers,
+                                            d_homography, d_h_mask, *prm, d_out, d_out_mask, d_points, inf.data(), nullptr, &err);
+    const int rc = finish("ps_two_view_config_batch", n, err);
+    if (rc == PS_OK) std::memcpy(info, inf.data(), inf.size() * sizeof(ps_two_view_info));
     return rc;
 }
 

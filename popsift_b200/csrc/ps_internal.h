@@ -7,6 +7,7 @@
 #include "popsift_b200_bundle.h"
 #include "popsift_b200_global.h"
 #include "popsift_b200_viewgraph.h"
+#include "popsift_b200_twoview.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
@@ -320,5 +321,13 @@ int run_global_positioning(int n_sets, const int32_t* n_feat, const ps_feature* 
 int run_view_graph_filter(int n_sets, int n_pairs, const int32_t* pairs, const ps_two_view* d_two_view, const ps_view_graph_params& prm,
                           uint8_t* keep, ps_cycle_stats* stats, ps_two_view* d_kept, ps_view_graph_report* report, cudaStream_t st,
                           const char** err);
+
+// two-view configuration (include/popsift_b200_twoview.h, k_twoview.cu), arguments already validated and n_pairs > 0.
+// Synchronous on `st`; info is written when it returns >= 0.  Returns the number of kernels launched or -1 (*err set).
+int run_two_view_config_batch(int n_pairs, const float* corr, const int32_t* corr_start, const int32_t* n_corr, const ps_camera* cams,
+                              const ps_two_view* d_essential, const uint8_t* d_essential_mask, const int32_t* d_f_inliers,
+                              const float* d_homography, const uint8_t* d_h_mask, const ps_two_view_config_params& prm,
+                              ps_two_view* d_out, uint8_t* d_out_mask, float* d_points, ps_two_view_info* info, cudaStream_t st,
+                              const char** err);
 
 } // namespace psb
