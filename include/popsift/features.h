@@ -390,6 +390,81 @@ struct ViewGraph
 ViewGraph filterViewGraph(int n_sets, const std::vector<std::pair<int, int>>& pairs, const std::vector<TwoViewPose>& poses,
                           const ViewGraphParams& params = ViewGraphParams());
 
+/// A grey image on the device: row-major 8-bit values, `pitch` bytes between rows (ps_image in popsift_b200_depth.h).
+struct DeviceImage
+{
+    const std::uint8_t* data = nullptr;
+    long long           pitch = 0;
+    int                 width = 0, height = 0;
+};
+
+/// Settings of depthMaps (same fields and rules as ps_depth_params in popsift_b200_depth.h).
+struct DepthParams
+{
+    int   n_depths = 128;                // planes, 2 .. 1024
+    int   radius = 3;                    // NCC window half-size, 1 .. 7
+    int   top_k = 3;                     // source costs averaged per plane, 1 .. 32
+    int   min_sources = 1;               // valid sources a plane needs, 1 .. 32
+    float max_cost = 0.5f;               // a depth is kept when its cost is at most this, (0, 2]
+    float min_var = 1.0f;                // window variance floor, grey levels^2
+};
+
+/// One reference's maps, row-major width x height: depth (0 where there is none), cost (+inf without a winner) and the
+/// valid sources at the winning plane.
+struct DepthMap
+{
+    int                       width = 0, height = 0;
+    std::vector<float>        depth, cost;
+    std::vector<std::uint8_t> n_src;
+};
+
+/// depthMaps' maps, one per reference, and the totals of ps_depth_report.
+struct DepthMaps
+{
+    std::vector<DepthMap> maps;
+    long long             n_candidates = 0, n_depths = 0;
+};
+
+/// Dense depth maps by plane sweep on `device` (an addition to the reference's interface; C ABI ps_depth_maps):
+/// `images`, `cameras` and `poses` one per set; for reference j the set refs[j], its source sets sources[j] and its depth
+/// range ranges[j] = (d_min, d_max).  Throws for the arguments ps_depth_maps refuses.
+DepthMaps depthMaps(const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+                    const std::vector<int>& refs, const std::vector<std::vector<int>>& sources,
+                    const std::vector<std::pair<float, float>>& ranges, const DepthParams& params = DepthParams(), int device = 0);
+
+/// Settings of filterDepthMaps (same fields and rules as ps_depth_filter_params).
+struct DepthFilterParams
+{
+    float max_reproj_error = 1.0f;       // pixels
+    float max_depth_diff = 0.01f;        // relative
+    int   min_consistent = 2;            // 1 .. 255
+};
+
+/// One consistent pixel as a world point (ps_dense_point).
+struct DensePoint
+{
+    float         X[3];
+    int           ref;
+    std::uint16_t x, y;
+    std::uint8_t  n_consistent, grey;
+};
+
+/// filterDepthMaps' result: the consistent sources per pixel of each reference, the points in (ref, y, x) order and the
+/// pixels with a depth.
+struct DensePoints
+{
+    std::vector<std::vector<std::uint8_t>> n_consistent;
+    std::vector<DensePoint>                points;
+    long long                              n_tested = 0;
+};
+
+/// Geometric consistency between the maps of one depthMaps call and the consistent pixels as points (C ABI
+/// ps_depth_filter): the same images, cameras, poses, refs and sources; `maps` is uploaded.  Throws for the arguments
+/// ps_depth_filter refuses.
+DensePoints filterDepthMaps(const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+                            const std::vector<int>& refs, const std::vector<std::vector<int>>& sources, const DepthMaps& maps,
+                            const DepthFilterParams& params = DepthFilterParams(), int device = 0);
+
 /// Settings of twoViewGeometries' classification (same fields and rules as ps_two_view_config_params in
 /// popsift_b200_twoview.h; the pure-rotation test uses PoseParams::threshold).
 struct TwoViewConfigParams

@@ -200,6 +200,38 @@ TWO_VIEW_INFO_DTYPE = np.dtype([("config", "<i4"), ("n_e", "<i4"), ("n_f", "<i4"
 TV_CONFIG = ("degenerate", "general", "planar", "panoramic", "uncalibrated")
 assert C.sizeof(PsTwoViewConfigParams) == 32 and C.sizeof(PsTwoViewInfo) == 40 and TWO_VIEW_INFO_DTYPE.itemsize == 40
 
+class PsImage(C.Structure):
+    """ps_image (24 bytes): device grey levels, row-major"""
+    _fields_ = [("data", C.c_void_p), ("pitch", C.c_int64), ("width", C.c_int32), ("height", C.c_int32)]
+
+
+class PsDepthParams(C.Structure):
+    """ps_depth_params (24 bytes)"""
+    _fields_ = [("n_depths", C.c_int32), ("radius", C.c_int32), ("top_k", C.c_int32), ("min_sources", C.c_int32),
+                ("max_cost", C.c_float), ("min_var", C.c_float)]
+
+
+class PsDepthReport(C.Structure):
+    """ps_depth_report (16 bytes)"""
+    _fields_ = [("n_candidates", C.c_int64), ("n_depths", C.c_int64)]
+
+
+class PsDepthFilterParams(C.Structure):
+    """ps_depth_filter_params (16 bytes)"""
+    _fields_ = [("max_reproj_error", C.c_float), ("max_depth_diff", C.c_float), ("min_consistent", C.c_int32), ("pad_", C.c_int32)]
+
+
+class PsDepthFilterReport(C.Structure):
+    """ps_depth_filter_report (16 bytes)"""
+    _fields_ = [("n_tested", C.c_int64), ("n_points", C.c_int64)]
+
+
+# ps_dense_point (24 bytes): one consistent pixel of ps_depth_filter
+DENSE_POINT_DTYPE = np.dtype([("X", "<f4", 3), ("ref", "<i4"), ("x", "<u2"), ("y", "<u2"), ("n_consistent", "u1"), ("grey", "u1"),
+                              ("pad_", "<u2")])
+assert C.sizeof(PsImage) == 24 and C.sizeof(PsDepthParams) == 24 and C.sizeof(PsDepthReport) == 16
+assert C.sizeof(PsDepthFilterParams) == 16 and C.sizeof(PsDepthFilterReport) == 16 and DENSE_POINT_DTYPE.itemsize == 24
+
 RA_TERMINATION = ("max_iters", "step_tol", "no_pairs")
 GP_TERMINATION = ("max_iters", "function_tol", "no_observations")
 assert C.sizeof(PsRotationParams) == 40 and C.sizeof(PsRotationReport) == 40
@@ -230,6 +262,8 @@ GLOBAL_EXPORTS = ["ps_rotation_averaging", "ps_global_positioning"]
 VIEWGRAPH_EXPORTS = ["ps_view_graph_filter"]
 # two-view configuration, declared in popsift_b200_twoview.h (same library)
 TWOVIEW_EXPORTS = ["ps_two_view_config_batch"]
+# dense depth maps, declared in popsift_b200_depth.h (same library)
+DEPTH_EXPORTS = ["ps_depth_maps", "ps_depth_filter"]
 
 _lib = None
 
@@ -311,6 +345,11 @@ def load_library():
         L.ps_two_view_config_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsTwoViewConfigParams), C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p]
+    if hasattr(L, "ps_depth_maps"):
+        L.ps_depth_maps.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.POINTER(PsDepthParams), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsDepthReport)]
+        L.ps_depth_filter.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.POINTER(PsDepthFilterParams), C.c_void_p, C.c_void_p, C.POINTER(PsDepthFilterReport)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -1654,6 +1693,172 @@ def global_poses(sets, pairs, cameras, matches=None, flags=0, u8=False, device=N
     finally:
         bufs.free()
     return GlobalPoses(tr, poses, reg, positioned, rrep, grep, perr)
+
+
+DepthMaps = namedtuple("DepthMaps", "depth cost n_src report n_consistent points filter_report")
+DepthMaps.__doc__ = """depth_maps' result, one entry per reference: depth (h, w) float32 (0 where there is none), cost (h, w) float32 (+inf
+without a winner), n_src (h, w) uint8 and the report {"candidates", "depths"}.  With a filter: n_consistent (h, w) uint8
+per reference, points (a DENSE_POINT_DTYPE array in (ref, y, x) order) and filter_report {"tested", "points"}; None
+otherwise."""
+
+
+def _depth_params(n_depths=128, radius=3, top_k=3, min_sources=1, max_cost=0.5, min_var=1.0) -> PsDepthParams:
+    return PsDepthParams(int(n_depths), int(radius), int(top_k), int(min_sources), float(max_cost), float(min_var))
+
+
+def _depth_filter_params(max_reproj_error=1.0, max_depth_diff=0.01, min_consistent=2) -> PsDepthFilterParams:
+    return PsDepthFilterParams(float(max_reproj_error), float(max_depth_diff), int(min_consistent), 0)
+
+
+def _c_images(lib, bufs, images):
+    """ps_image array of 2-D uint8 images: numpy arrays are uploaded, objects with __cuda_array_interface__ (torch CUDA
+    tensors, for example) are used in place.  Returns (the array, the device of the first device image or None)."""
+    out = (PsImage * max(len(images), 1))()
+    device = None
+    for i, im in enumerate(images):
+        cai = getattr(im, "__cuda_array_interface__", None)
+        if cai is not None:
+            if len(cai["shape"]) != 2 or np.dtype(cai["typestr"]) != np.uint8:
+                raise PopSiftError("image %d: a 2-D uint8 device array expected" % i)
+            h, w = (int(v) for v in cai["shape"])
+            st = cai.get("strides")
+            if st is not None and int(st[1]) != 1:
+                raise PopSiftError("image %d: rows must be contiguous" % i)
+            ptr = int(cai["data"][0])
+            out[i] = PsImage(ptr, int(st[0]) if st is not None else w, w, h)
+            if device is None:
+                device = max(0, lib.ps_pointer_device(ptr))
+        else:
+            a = np.ascontiguousarray(im, np.uint8)
+            if a.ndim != 2:
+                raise PopSiftError("image %d: a 2-D uint8 array expected" % i)
+            out[i] = PsImage(bufs.upload(a), a.shape[1], a.shape[1], a.shape[0])
+    return out, device
+
+
+def _depth_csr(refs, sources):
+    refs = [int(r) for r in refs]
+    if len(sources) != len(refs):
+        raise PopSiftError("one source list per reference expected")
+    start = np.concatenate([[0], np.cumsum([len(s) for s in sources])]).astype(np.int32)
+    flat = np.asarray([int(v) for s in sources for v in s] or [0], np.int32)
+    return np.asarray(refs or [0], np.int32), start, flat
+
+
+def depth_maps(images, cameras, poses, refs, sources, ranges, device=None, filter=None, **params) -> DepthMaps:
+    """Dense depth maps by plane sweep (C ABI ps_depth_maps in popsift_b200_depth.h; an addition to the reference's
+    interface): for each reference set refs[j], a fronto-parallel sweep of params["n_depths"] planes in inverse depth over
+    ranges[j] = (d_min, d_max), a zero-mean NCC window of radius params["radius"] against the sets sources[j], the mean of
+    the top_k best source costs per plane, the winning plane refined by a parabola.  `images` holds one 2-D uint8 image
+    per set: numpy arrays (uploaded) or objects with __cuda_array_interface__ such as torch CUDA tensors (used in place,
+    any row pitch); `cameras` one (fx, fy, cx, cy) and `poses` one world-to-camera (R, t) per set.  params: n_depths (128),
+    radius (3), top_k (3), min_sources (1), max_cost (0.5), min_var (1.0 grey levels^2).  A dict `filter`
+    (max_reproj_error 1.0 px, max_depth_diff 0.01, min_consistent 2) also runs ps_depth_filter on the device maps:
+    the geometric consistency between the references and the consistent pixels as world points."""
+    lib = load_library()
+    prm = _depth_params(**params)
+    fprm = _depth_filter_params(**filter) if filter is not None else None
+    n_sets = len(images)
+    cam = _c_cameras(cameras)
+    if len(cam) != n_sets or len(poses) != n_sets:
+        raise PopSiftError("one camera and one pose per image expected")
+    c_refs, start, flat = _depth_csr(refs, sources)
+    nr = len(refs)
+    rng = np.ascontiguousarray(np.asarray(ranges, np.float32).reshape(-1, 2) if nr else np.zeros((1, 2)), np.float32)
+    bufs = _DevBuffers(lib)
+    try:
+        c_img, dev0 = _c_images(lib, bufs, images)
+        if device is None:
+            device = dev0 if dev0 is not None else 0
+        shapes = [(int(c_img[r].height), int(c_img[r].width)) if 0 <= r < n_sets else (0, 0) for r in c_refs[:nr]]
+        d_depth = [bufs.alloc(h * w * 4) for h, w in shapes]
+        d_cost = [bufs.alloc(h * w * 4) for h, w in shapes]
+        d_nsrc = [bufs.alloc(h * w) for h, w in shapes]
+        n = max(nr, 1)
+        c_depth, c_cost, c_nsrc = (C.c_void_p * n)(*d_depth), (C.c_void_p * n)(*d_cost), (C.c_void_p * n)(*d_nsrc)
+        rig = _c_rigids(poses)
+        rep = PsDepthReport()
+        _check(lib, lib.ps_depth_maps(device, n_sets, c_img, cam.ctypes.data, rig, nr, c_refs.ctypes.data, rng.ctypes.data,
+                                      start.ctypes.data, flat.ctypes.data, C.byref(prm), c_depth, c_cost, c_nsrc, C.byref(rep)),
+               "ps_depth_maps")
+        depth = [bufs.download(d, s, np.float32) for d, s in zip(d_depth, shapes)]
+        cost = [bufs.download(d, s, np.float32) for d, s in zip(d_cost, shapes)]
+        nsrc = [bufs.download(d, s, np.uint8) for d, s in zip(d_nsrc, shapes)]
+        report = {"candidates": int(rep.n_candidates), "depths": int(rep.n_depths)}
+        ncons = points = frep = None
+        if fprm is not None:
+            d_ncons = [bufs.alloc(h * w) for h, w in shapes]
+            cap = sum(h * w for h, w in shapes)
+            d_pts = bufs.alloc(cap * DENSE_POINT_DTYPE.itemsize)
+            fr = PsDepthFilterReport()
+            _check(lib, lib.ps_depth_filter(device, n_sets, c_img, cam.ctypes.data, rig, nr, c_refs.ctypes.data, start.ctypes.data,
+                                            flat.ctypes.data, c_depth, C.byref(fprm), (C.c_void_p * n)(*d_ncons), d_pts, C.byref(fr)),
+                   "ps_depth_filter")
+            ncons = [bufs.download(d, s, np.uint8) for d, s in zip(d_ncons, shapes)]
+            points = bufs.download(d_pts, int(fr.n_points), DENSE_POINT_DTYPE)
+            frep = {"tested": int(fr.n_tested), "points": int(fr.n_points)}
+    finally:
+        bufs.free()
+    return DepthMaps(depth, cost, nsrc, report, ncons, points, frep)
+
+
+def _track_observations(tracks, points, poses):
+    """(track, set, camera-frame depth) of the OK tracks' members with mask 1"""
+    ok = np.asarray(points.status) == 0
+    start = np.asarray(tracks.start, np.int64)
+    tid = np.repeat(np.arange(len(start) - 1), np.diff(start))
+    sel = ok[tid] & (np.asarray(points.mask) == 1)
+    t, s = tid[sel], np.asarray(tracks.set, np.int64)[sel]
+    X = np.asarray(points.X, np.float64)[t]
+    R = np.stack([np.asarray(p[0], np.float64).reshape(3, 3) for p in poses]) if len(poses) else np.zeros((0, 3, 3))
+    tv = np.stack([np.asarray(p[1], np.float64).reshape(3) for p in poses]) if len(poses) else np.zeros((0, 3))
+    z = np.einsum("nj,nj->n", R[s, 2], X) + tv[s, 2]
+    return t, s, z
+
+
+def depth_ranges(tracks, points, poses, n_sets, lo=1.0, hi=99.0, margin=0.25) -> np.ndarray:
+    """Per set, the depth range for depth_maps from a sparse reconstruction: the percentiles lo and hi (numpy's linear
+    rule) of the camera-frame depths of the OK tracks' members with mask 1 in that set, divided and multiplied by
+    1 + margin.  `tracks`, `points` and `poses` are what bundle_adjust / triangulate give.  A set without such depths gets
+    (0, 0), which depth_maps refuses as a reference.  Returns (n_sets, 2) float64."""
+    _, s, z = _track_observations(tracks, points, poses)
+    out = np.zeros((int(n_sets), 2), np.float64)
+    for i in range(int(n_sets)):
+        zi = z[s == i]
+        if len(zi):
+            out[i] = (np.percentile(zi, lo) / (1.0 + margin), np.percentile(zi, hi) * (1.0 + margin))
+    return out
+
+
+def select_sources(tracks, points, poses, n_sources=5, min_angle=1.0) -> list:
+    """Per set, the source sets for depth_maps, as COLMAP chooses them: the other sets ranked by the number of OK tracks
+    both see (members with mask 1) whose viewing rays from the two camera centres meet at the track's point at an angle of
+    at least min_angle degrees; ties to the lower set id, only counts > 0, at most n_sources."""
+    t, s, _ = _track_observations(tracks, points, poses)
+    n_sets = len(poses)
+    Cs = np.stack([-np.asarray(p[0], np.float64).reshape(3, 3).T @ np.asarray(p[1], np.float64).reshape(3) for p in poses])
+    X = np.asarray(points.X, np.float64)
+    cos_min = np.cos(np.radians(float(min_angle)))
+    count = np.zeros((n_sets, n_sets), np.int64)
+    order = np.argsort(t, kind="stable")
+    t, s = t[order], s[order]
+    bounds = np.flatnonzero(np.r_[True, t[1:] != t[:-1], True])
+    for a, b in zip(bounds[:-1], bounds[1:]):
+        ss = s[a:b]
+        if len(ss) < 2:
+            continue
+        u = Cs[ss] - X[t[a]]
+        u /= np.linalg.norm(u, axis=1, keepdims=True)
+        ok = (u @ u.T) <= cos_min
+        np.fill_diagonal(ok, False)
+        count[np.ix_(ss, ss)] += ok
+    out = []
+    for i in range(n_sets):
+        c = count[i].copy()
+        c[i] = 0
+        rank = sorted((j for j in range(n_sets) if c[j] > 0), key=lambda j: (-c[j], j))
+        out.append(rank[:int(n_sources)])
+    return out
 
 
 def _match_guided_dev(lib, bufs, sets, descs, pairs, d_models, model, threshold, flags, u8) -> int:

@@ -13,6 +13,7 @@
 #include "popsift_b200_global.h"
 #include "popsift_b200_viewgraph.h"
 #include "popsift_b200_twoview.h"
+#include "popsift_b200_depth.h"
 
 #include <algorithm>
 #include <cmath>
@@ -22,6 +23,7 @@
 #include <cstdlib>
 #include <iomanip>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <optional>
@@ -854,6 +856,140 @@ Rotations rotationAveraging(int n_sets, const std::vector<std::pair<int, int>>& 
     o.n_pairs = r.n_pairs;
     o.n_registered = r.n_registered;
     o.termination = r.termination;
+    return out;
+}
+
+// the C ABI arguments of a depth call: images, cameras, poses, refs and the source CSR
+struct DepthCall {
+    std::vector<ps_image> img;
+    std::vector<ps_camera> cam;
+    std::vector<ps_rigid> pose;
+    std::vector<int32_t> refs, start, src;
+    DepthCall(const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+              const std::vector<int>& r, const std::vector<std::vector<int>>& sources, const std::string& who)
+    {
+        if (cameras.size() != images.size() || poses.size() != images.size())
+            throw std::runtime_error(who + ": one camera and one pose per image expected");
+        if (sources.size() != r.size()) throw std::runtime_error(who + ": one source list per reference expected");
+        for (const DeviceImage& im : images) img.push_back(ps_image{im.data, im.pitch, im.width, im.height});
+        for (const Camera& c : cameras) cam.push_back(ps_camera{c.fx, c.fy, c.cx, c.cy});
+        for (const Rigid& p : poses) {
+            ps_rigid q;
+            std::copy(p.R, p.R + 9, q.R);
+            std::copy(p.t, p.t + 3, q.t);
+            pose.push_back(q);
+        }
+        refs.assign(r.begin(), r.end());
+        start.push_back(0);
+        for (const auto& s : sources) {
+            src.insert(src.end(), s.begin(), s.end());
+            start.push_back((int32_t)src.size());
+        }
+    }
+    // the reference's image size, 0 x 0 for an index the C ABI refuses
+    std::pair<int, int> size(size_t j) const
+    {
+        const int r = refs[j];
+        return r >= 0 && r < (int)img.size() ? std::make_pair(img[r].width, img[r].height) : std::make_pair(0, 0);
+    }
+};
+
+DepthMaps depthMaps(const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+                    const std::vector<int>& refs, const std::vector<std::vector<int>>& sources,
+                    const std::vector<std::pair<float, float>>& ranges, const DepthParams& params, int device)
+{
+    const std::string who = "popsift::depthMaps";
+    const DepthCall a(images, cameras, poses, refs, sources, who);
+    if (ranges.size() != refs.size()) throw std::runtime_error(who + ": one depth range per reference expected");
+    const size_t nr = refs.size();
+    std::vector<float> rng;
+    for (const auto& r : ranges) rng.insert(rng.end(), {r.first, r.second});
+    std::vector<std::unique_ptr<DevBuf>> bufs;
+    std::vector<float*> d_depth, d_cost;
+    std::vector<uint8_t*> d_nsrc;
+    for (size_t j = 0; j < nr; ++j) {
+        const auto wh = a.size(j);
+        const size_t n = (size_t)wh.first * wh.second;
+        bufs.emplace_back(new DevBuf(n * 4, who));
+        d_depth.push_back(static_cast<float*>(bufs.back()->p));
+        bufs.emplace_back(new DevBuf(n * 4, who));
+        d_cost.push_back(static_cast<float*>(bufs.back()->p));
+        bufs.emplace_back(new DevBuf(n, who));
+        d_nsrc.push_back(static_cast<uint8_t*>(bufs.back()->p));
+    }
+    const ps_depth_params prm{params.n_depths, params.radius, params.top_k, params.min_sources, params.max_cost, params.min_var};
+    ps_depth_report rep;
+    check(ps_depth_maps(device, (int)images.size(), a.img.data(), a.cam.data(), a.pose.data(), (int)nr, a.refs.data(), rng.data(),
+                        a.start.data(), a.src.data(), &prm, d_depth.data(), d_cost.data(), d_nsrc.data(), &rep),
+          who, "ps_depth_maps");
+    DepthMaps out;
+    out.n_candidates = rep.n_candidates;
+    out.n_depths = rep.n_depths;
+    out.maps.resize(nr);
+    for (size_t j = 0; j < nr; ++j) {
+        DepthMap& m = out.maps[j];
+        m.width = a.size(j).first;
+        m.height = a.size(j).second;
+        const size_t n = (size_t)m.width * m.height;
+        m.depth.resize(n);
+        m.cost.resize(n);
+        m.n_src.resize(n);
+        check(ps_dev_to_host(m.depth.data(), d_depth[j], n * 4), who);
+        check(ps_dev_to_host(m.cost.data(), d_cost[j], n * 4), who);
+        check(ps_dev_to_host(m.n_src.data(), d_nsrc[j], n), who);
+    }
+    return out;
+}
+
+DensePoints filterDepthMaps(const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+                            const std::vector<int>& refs, const std::vector<std::vector<int>>& sources, const DepthMaps& maps,
+                            const DepthFilterParams& params, int device)
+{
+    const std::string who = "popsift::filterDepthMaps";
+    const DepthCall a(images, cameras, poses, refs, sources, who);
+    const size_t nr = refs.size();
+    if (maps.maps.size() != nr) throw std::runtime_error(who + ": one depth map per reference expected");
+    std::vector<std::unique_ptr<DevBuf>> bufs;
+    std::vector<const float*> d_depth;
+    std::vector<uint8_t*> d_nc;
+    size_t cap = 0;
+    for (size_t j = 0; j < nr; ++j) {
+        const DepthMap& m = maps.maps[j];
+        const size_t n = (size_t)m.width * m.height;
+        if (a.size(j) != std::make_pair(m.width, m.height) || m.depth.size() != n)
+            throw std::runtime_error(who + ": a depth map does not match its reference image");
+        bufs.emplace_back(new DevBuf(n * 4, who));
+        if (n) check(ps_host_to_dev(bufs.back()->p, m.depth.data(), n * 4), who);
+        d_depth.push_back(static_cast<const float*>(bufs.back()->p));
+        bufs.emplace_back(new DevBuf(n, who));
+        d_nc.push_back(static_cast<uint8_t*>(bufs.back()->p));
+        cap += n;
+    }
+    DevBuf d_pts(cap * sizeof(ps_dense_point), who);
+    const ps_depth_filter_params prm{params.max_reproj_error, params.max_depth_diff, params.min_consistent, 0};
+    ps_depth_filter_report rep;
+    check(ps_depth_filter(device, (int)images.size(), a.img.data(), a.cam.data(), a.pose.data(), (int)nr, a.refs.data(), a.start.data(),
+                          a.src.data(), d_depth.data(), &prm, d_nc.data(), static_cast<ps_dense_point*>(d_pts.p), &rep),
+          who, "ps_depth_filter");
+    DensePoints out;
+    out.n_tested = rep.n_tested;
+    out.n_consistent.resize(nr);
+    for (size_t j = 0; j < nr; ++j) {
+        out.n_consistent[j].resize(maps.maps[j].depth.size());
+        check(ps_dev_to_host(out.n_consistent[j].data(), d_nc[j], out.n_consistent[j].size()), who);
+    }
+    std::vector<ps_dense_point> pts((size_t)rep.n_points);
+    if (!pts.empty()) check(ps_dev_to_host(pts.data(), d_pts.p, pts.size() * sizeof(ps_dense_point)), who);
+    out.points.resize(pts.size());
+    for (size_t i = 0; i < pts.size(); ++i) {
+        DensePoint& q = out.points[i];
+        std::copy(pts[i].X, pts[i].X + 3, q.X);
+        q.ref = pts[i].ref;
+        q.x = pts[i].x;
+        q.y = pts[i].y;
+        q.n_consistent = pts[i].n_consistent;
+        q.grey = pts[i].grey;
+    }
     return out;
 }
 

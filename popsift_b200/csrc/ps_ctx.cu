@@ -16,6 +16,7 @@
 #include "popsift_b200_bundle.h"
 #include "popsift_b200_global.h"
 #include "popsift_b200_twoview.h"
+#include "popsift_b200_depth.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1706,6 +1707,112 @@ extern "C" int ps_two_view_config_batch(int device, int n_pairs, const float* d_
                                             d_homography, d_h_mask, *prm, d_out, d_out_mask, d_points, inf.data(), nullptr, &err);
     const int rc = finish("ps_two_view_config_batch", n, err);
     if (rc == PS_OK) std::memcpy(info, inf.data(), inf.size() * sizeof(ps_two_view_info));
+    return rc;
+}
+
+// The checks ps_depth_maps and ps_depth_filter share (n_refs > 0, the device already set): the sets, the references and
+// the source CSR; the images, cameras and poses of every set they use, each image at least min_side pixels a side
+static bool check_depth_call(int device, int n_sets, const ps_image* images, const ps_camera* cams, const ps_rigid* poses, int n_refs,
+                             const int32_t* refs, const int32_t* src_start, const int32_t* src_sets, int min_side)
+{
+    if (n_sets < 0 || !images || !cams || !poses || !refs || !src_start) return false;
+    if (src_start[0] != 0) return false;
+    for (int j = 0; j < n_refs; ++j)
+        if (src_start[j + 1] < src_start[j]) return false;
+    if (src_start[n_refs] > 0 && !src_sets) return false;
+    std::vector<uint8_t> used(n_sets, 0);
+    for (int j = 0; j < n_refs; ++j) {
+        const int r = refs[j];
+        if (r < 0 || r >= n_sets || (used[r] & 1)) return false;
+        used[r] |= 1;
+    }
+    for (int j = 0; j < n_refs; ++j)
+        for (int s = src_start[j]; s < src_start[j + 1]; ++s) {
+            const int i = src_sets[s];
+            if (i < 0 || i >= n_sets || i == refs[j]) return false;
+            used[i] |= 2;
+        }
+    for (int i = 0; i < n_sets; ++i) {
+        if (!used[i]) continue;
+        const ps_image& im = images[i];
+        if (im.width < min_side || im.height < min_side || im.width > 65535 || im.height > 65535 || im.pitch < im.width) return false;
+        if (ps_pointer_device(im.data) != device) return false;
+        const ps_camera& c = cams[i];
+        if (!std::isfinite(c.fx) || !(c.fx > 0.0f) || !std::isfinite(c.fy) || !(c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
+            return false;
+        if (!rigid_ok(poses[i])) return false;
+    }
+    return true;
+}
+
+// every entry of a host array of n device pointers on `device`
+template <class T>
+static bool device_arrays(int device, T* const* p, int n)
+{
+    if (!p) return false;
+    for (int j = 0; j < n; ++j)
+        if (ps_pointer_device(p[j]) != device) return false;
+    return true;
+}
+
+extern "C" int ps_depth_maps(int device, int n_sets, const ps_image* images, const ps_camera* cams, const ps_rigid* poses, int n_refs,
+                             const int32_t* refs, const float* ranges, const int32_t* src_start, const int32_t* src_sets,
+                             const ps_depth_params* prm, float* const* d_depth, float* const* d_cost, uint8_t* const* d_n_src,
+                             ps_depth_report* report)
+{
+    if (n_sets < 0 || n_refs < 0 || !prm || !report) return PS_ERR_ARG;
+    if (prm->n_depths < 2 || prm->n_depths > 1024 || prm->radius < 1 || prm->radius > 7 || prm->top_k < 1 || prm->top_k > 32 ||
+        prm->min_sources < 1 || prm->min_sources > 32)
+        return PS_ERR_ARG;
+    if (!(prm->max_cost > 0.0f && prm->max_cost <= 2.0f) || !std::isfinite(prm->min_var) || !(prm->min_var >= 0.0f)) return PS_ERR_ARG;
+    if (n_refs == 0) {
+        std::memset(report, 0, sizeof(*report));
+        return PS_OK;
+    }
+    if (!ranges) return PS_ERR_ARG;
+    for (int j = 0; j < n_refs; ++j) {
+        const float lo = ranges[2 * j], hi = ranges[2 * j + 1];
+        if (!std::isfinite(lo) || !std::isfinite(hi) || !(lo > 0.0f) || !(lo < hi)) return PS_ERR_ARG;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (!check_depth_call(device, n_sets, images, cams, poses, n_refs, refs, src_start, src_sets, 2 * prm->radius + 1)) return PS_ERR_ARG;
+    if (!device_arrays(device, d_depth, n_refs) || !device_arrays(device, d_cost, n_refs) || !device_arrays(device, d_n_src, n_refs))
+        return PS_ERR_ARG;
+    const char* err = nullptr;
+    ps_depth_report rep{};
+    const int n = run_depth_maps(n_sets, images, cams, poses, n_refs, refs, ranges, src_start, src_sets, *prm, d_depth, d_cost, d_n_src,
+                                 &rep, nullptr, &err);
+    const int rc = finish("ps_depth_maps", n, err);
+    if (rc == PS_OK) *report = rep;
+    return rc;
+}
+
+extern "C" int ps_depth_filter(int device, int n_sets, const ps_image* images, const ps_camera* cams, const ps_rigid* poses, int n_refs,
+                               const int32_t* refs, const int32_t* src_start, const int32_t* src_sets, const float* const* d_depth,
+                               const ps_depth_filter_params* prm, uint8_t* const* d_n_consistent, ps_dense_point* d_points,
+                               ps_depth_filter_report* report)
+{
+    if (n_sets < 0 || n_refs < 0 || !prm || !report) return PS_ERR_ARG;
+    if (!std::isfinite(prm->max_reproj_error) || !(prm->max_reproj_error > 0.0f) || !std::isfinite(prm->max_depth_diff) ||
+        !(prm->max_depth_diff > 0.0f) || prm->min_consistent < 1 || prm->min_consistent > 255)
+        return PS_ERR_ARG;
+    if (n_refs == 0) {
+        std::memset(report, 0, sizeof(*report));
+        return PS_OK;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (!check_depth_call(device, n_sets, images, cams, poses, n_refs, refs, src_start, src_sets, 1)) return PS_ERR_ARG;
+    if (!device_arrays(device, d_depth, n_refs) || !device_arrays(device, d_n_consistent, n_refs) || ps_pointer_device(d_points) != device)
+        return PS_ERR_ARG;
+    int64_t total = 0;
+    for (int j = 0; j < n_refs; ++j) total += (int64_t)images[refs[j]].width * images[refs[j]].height;
+    if (total >= 0x80000000LL) return PS_ERR_ARG;
+    const char* err = nullptr;
+    ps_depth_filter_report rep{};
+    const int n = run_depth_filter(n_sets, images, cams, poses, n_refs, refs, src_start, src_sets, d_depth, *prm, d_n_consistent, d_points,
+                                   &rep, nullptr, &err);
+    const int rc = finish("ps_depth_filter", n, err);
+    if (rc == PS_OK) *report = rep;
     return rc;
 }
 

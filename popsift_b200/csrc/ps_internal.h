@@ -8,6 +8,7 @@
 #include "popsift_b200_global.h"
 #include "popsift_b200_viewgraph.h"
 #include "popsift_b200_twoview.h"
+#include "popsift_b200_depth.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
@@ -329,5 +330,17 @@ int run_two_view_config_batch(int n_pairs, const float* corr, const int32_t* cor
                               const float* d_homography, const uint8_t* d_h_mask, const ps_two_view_config_params& prm,
                               ps_two_view* d_out, uint8_t* d_out_mask, float* d_points, ps_two_view_info* info, cudaStream_t st,
                               const char** err);
+
+// dense depth maps and their consistency filter (include/popsift_b200_depth.h, k_depth.cu), arguments already validated
+// and n_refs > 0.  Synchronous on `st`; the report is written when they return >= 0.  Return the number of kernels
+// launched or -1 (*err set).
+int run_depth_maps(int n_sets, const ps_image* images, const ps_camera* cams, const ps_rigid* poses, int n_refs, const int32_t* refs,
+                   const float* ranges, const int32_t* src_start, const int32_t* src_sets, const ps_depth_params& prm,
+                   float* const* d_depth, float* const* d_cost, uint8_t* const* d_n_src, ps_depth_report* report, cudaStream_t st,
+                   const char** err);
+int run_depth_filter(int n_sets, const ps_image* images, const ps_camera* cams, const ps_rigid* poses, int n_refs, const int32_t* refs,
+                     const int32_t* src_start, const int32_t* src_sets, const float* const* d_depth, const ps_depth_filter_params& prm,
+                     uint8_t* const* d_n_consistent, ps_dense_point* d_points, ps_depth_filter_report* report, cudaStream_t st,
+                     const char** err);
 
 } // namespace psb
