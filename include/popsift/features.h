@@ -465,6 +465,87 @@ DensePoints filterDepthMaps(const std::vector<DeviceImage>& images, const std::v
                             const std::vector<int>& refs, const std::vector<std::vector<int>>& sources, const DepthMaps& maps,
                             const DepthFilterParams& params = DepthFilterParams(), int device = 0);
 
+/// A dense truncated signed distance volume on `device` (ps_volume in popsift_b200_mesh.h): nx x ny x nz grid points from
+/// `origin` at spacing `voxel`, grid point (i, j, k) at index i + nx (j + ny k) of the three device arrays it owns.
+/// Constructed cleared; throws for the volumes ps_volume_clear refuses or when the allocation fails.
+class DeviceVolume
+{
+public:
+    DeviceVolume(const double origin[3], double voxel, int nx, int ny, int nz, int device = 0);
+    ~DeviceVolume();
+    DeviceVolume(const DeviceVolume&) = delete;
+    DeviceVolume& operator=(const DeviceVolume&) = delete;
+
+    const double* origin() const { return _origin; }
+    double voxel() const { return _voxel; }
+    int nx() const { return _n[0]; }
+    int ny() const { return _n[1]; }
+    int nz() const { return _n[2]; }
+    int device() const { return _device; }
+    float* tsdf() const { return _tsdf; }       // DEVICE
+    float* weight() const { return _weight; }   // DEVICE
+    float* grey() const { return _grey; }       // DEVICE
+
+private:
+    double _origin[3];
+    double _voxel;
+    int    _n[3];
+    int    _device;
+    float* _tsdf = nullptr;
+    float* _weight = nullptr;
+    float* _grey = nullptr;
+};
+
+/// Sets every grid point's tsdf, weight and grey to 0 (C ABI ps_volume_clear).
+void clearVolume(DeviceVolume& volume);
+
+/// Settings of integrateDepthMaps (same fields and rules as ps_tsdf_params in popsift_b200_mesh.h).
+struct TsdfParams
+{
+    float trunc = 0.0f;                  // truncation distance in world units, > 0 (no default: it depends on the scene)
+    int   min_consistent = 0;            // 0 .. 255; > 0: only pixels whose mask value is at least this
+};
+
+/// integrateDepthMaps' totals (ps_tsdf_report).
+struct TsdfReport
+{
+    long long n_updates = 0, n_voxels_touched = 0;
+};
+
+/// Folds depth maps into `volume` (C ABI ps_tsdf_integrate): view v is images[v], cameras[v], poses[v] and the host map
+/// maps[v] (its size that of images[v]), uploaded; masks[v] are the n_consistent values of filterDepthMaps, read when
+/// params.min_consistent > 0 (masks may be empty otherwise).  Throws when the sizes disagree, and for the arguments
+/// ps_tsdf_integrate refuses.
+TsdfReport integrateDepthMaps(DeviceVolume& volume, const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras,
+                              const std::vector<Rigid>& poses, const std::vector<DepthMap>& maps,
+                              const std::vector<std::vector<std::uint8_t>>& masks, const TsdfParams& params);
+
+/// Settings of extractMesh (ps_mesh_params).
+struct MeshParams
+{
+    float min_weight = 1.0f;             // a cell is meshed when its 8 corners have at least this weight
+};
+
+/// One mesh vertex (ps_mesh_vertex): world position and interpolated grey level.
+struct MeshVertex
+{
+    float X[3];
+    float grey;
+};
+
+/// extractMesh's result: the vertices in edge-key order, the triangles as 3 vertex indices each (normals towards the
+/// cameras) and the totals of ps_mesh_report.
+struct Mesh
+{
+    std::vector<MeshVertex> vertices;
+    std::vector<int>        triangles;   // 3 per triangle
+    long long               n_cells = 0;
+};
+
+/// The surface of `volume` by marching tetrahedra (C ABI ps_tsdf_mesh: a count call, then the call that fills outputs of
+/// that size).  Throws for the arguments ps_tsdf_mesh refuses.
+Mesh extractMesh(const DeviceVolume& volume, const MeshParams& params = MeshParams());
+
 /// Settings of twoViewGeometries' classification (same fields and rules as ps_two_view_config_params in
 /// popsift_b200_twoview.h; the pure-rotation test uses PoseParams::threshold).
 struct TwoViewConfigParams

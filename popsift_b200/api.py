@@ -232,6 +232,37 @@ DENSE_POINT_DTYPE = np.dtype([("X", "<f4", 3), ("ref", "<i4"), ("x", "<u2"), ("y
 assert C.sizeof(PsImage) == 24 and C.sizeof(PsDepthParams) == 24 and C.sizeof(PsDepthReport) == 16
 assert C.sizeof(PsDepthFilterParams) == 16 and C.sizeof(PsDepthFilterReport) == 16 and DENSE_POINT_DTYPE.itemsize == 24
 
+class PsVolume(C.Structure):
+    """ps_volume (72 bytes): a dense volume's geometry and its three device arrays"""
+    _fields_ = [("origin", C.c_double * 3), ("voxel", C.c_double), ("nx", C.c_int32), ("ny", C.c_int32), ("nz", C.c_int32),
+                ("pad_", C.c_int32), ("tsdf", C.c_void_p), ("weight", C.c_void_p), ("grey", C.c_void_p)]
+
+
+class PsTsdfParams(C.Structure):
+    """ps_tsdf_params (8 bytes)"""
+    _fields_ = [("trunc", C.c_float), ("min_consistent", C.c_int32)]
+
+
+class PsMeshParams(C.Structure):
+    """ps_mesh_params (8 bytes)"""
+    _fields_ = [("min_weight", C.c_float), ("pad_", C.c_int32)]
+
+
+class PsTsdfReport(C.Structure):
+    """ps_tsdf_report (16 bytes)"""
+    _fields_ = [("n_updates", C.c_int64), ("n_voxels_touched", C.c_int64)]
+
+
+class PsMeshReport(C.Structure):
+    """ps_mesh_report (24 bytes)"""
+    _fields_ = [("n_cells", C.c_int64), ("n_vertices", C.c_int64), ("n_triangles", C.c_int64)]
+
+
+# ps_mesh_vertex (16 bytes): world position and grey level of one mesh vertex
+MESH_VERTEX_DTYPE = np.dtype([("X", "<f4", 3), ("grey", "<f4")])
+assert C.sizeof(PsVolume) == 72 and C.sizeof(PsTsdfParams) == 8 and C.sizeof(PsMeshParams) == 8
+assert C.sizeof(PsTsdfReport) == 16 and C.sizeof(PsMeshReport) == 24 and MESH_VERTEX_DTYPE.itemsize == 16
+
 RA_TERMINATION = ("max_iters", "step_tol", "no_pairs")
 GP_TERMINATION = ("max_iters", "function_tol", "no_observations")
 assert C.sizeof(PsRotationParams) == 40 and C.sizeof(PsRotationReport) == 40
@@ -264,6 +295,8 @@ VIEWGRAPH_EXPORTS = ["ps_view_graph_filter"]
 TWOVIEW_EXPORTS = ["ps_two_view_config_batch"]
 # dense depth maps, declared in popsift_b200_depth.h (same library)
 DEPTH_EXPORTS = ["ps_depth_maps", "ps_depth_filter"]
+# surface meshes, declared in popsift_b200_mesh.h (same library)
+MESH_EXPORTS = ["ps_volume_clear", "ps_tsdf_integrate", "ps_tsdf_mesh"]
 
 _lib = None
 
@@ -350,6 +383,12 @@ def load_library():
                                     C.c_void_p, C.POINTER(PsDepthParams), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PsDepthReport)]
         L.ps_depth_filter.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.POINTER(PsDepthFilterParams), C.c_void_p, C.c_void_p, C.POINTER(PsDepthFilterReport)]
+    if hasattr(L, "ps_tsdf_integrate"):
+        L.ps_volume_clear.argtypes = [C.c_int, C.POINTER(PsVolume)]
+        L.ps_tsdf_integrate.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.POINTER(PsTsdfParams), C.POINTER(PsVolume), C.POINTER(PsTsdfReport)]
+        L.ps_tsdf_mesh.argtypes = [C.c_int, C.POINTER(PsVolume), C.POINTER(PsMeshParams), C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                                   C.POINTER(PsMeshReport)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -1710,29 +1749,31 @@ def _depth_filter_params(max_reproj_error=1.0, max_depth_diff=0.01, min_consiste
     return PsDepthFilterParams(float(max_reproj_error), float(max_depth_diff), int(min_consistent), 0)
 
 
-def _c_images(lib, bufs, images):
-    """ps_image array of 2-D uint8 images: numpy arrays are uploaded, objects with __cuda_array_interface__ (torch CUDA
-    tensors, for example) are used in place.  Returns (the array, the device of the first device image or None)."""
+def _c_images(lib, bufs, images, dtype=np.uint8):
+    """ps_image array of 2-D images of element type dtype (pitch in bytes): numpy arrays are uploaded, objects with
+    __cuda_array_interface__ (torch CUDA tensors, for example) are used in place.  Returns (the array, the device of the
+    first device image or None)."""
+    dtype = np.dtype(dtype)
     out = (PsImage * max(len(images), 1))()
     device = None
     for i, im in enumerate(images):
         cai = getattr(im, "__cuda_array_interface__", None)
         if cai is not None:
-            if len(cai["shape"]) != 2 or np.dtype(cai["typestr"]) != np.uint8:
-                raise PopSiftError("image %d: a 2-D uint8 device array expected" % i)
+            if len(cai["shape"]) != 2 or np.dtype(cai["typestr"]) != dtype:
+                raise PopSiftError("image %d: a 2-D %s device array expected" % (i, dtype))
             h, w = (int(v) for v in cai["shape"])
             st = cai.get("strides")
-            if st is not None and int(st[1]) != 1:
+            if st is not None and int(st[1]) != dtype.itemsize:
                 raise PopSiftError("image %d: rows must be contiguous" % i)
             ptr = int(cai["data"][0])
-            out[i] = PsImage(ptr, int(st[0]) if st is not None else w, w, h)
+            out[i] = PsImage(ptr, int(st[0]) if st is not None else w * dtype.itemsize, w, h)
             if device is None:
                 device = max(0, lib.ps_pointer_device(ptr))
         else:
-            a = np.ascontiguousarray(im, np.uint8)
+            a = np.ascontiguousarray(im, dtype)
             if a.ndim != 2:
-                raise PopSiftError("image %d: a 2-D uint8 array expected" % i)
-            out[i] = PsImage(bufs.upload(a), a.shape[1], a.shape[1], a.shape[0])
+                raise PopSiftError("image %d: a 2-D %s array expected" % (i, dtype))
+            out[i] = PsImage(bufs.upload(a), a.shape[1] * dtype.itemsize, a.shape[1], a.shape[0])
     return out, device
 
 
@@ -1800,6 +1841,118 @@ def depth_maps(images, cameras, poses, refs, sources, ranges, device=None, filte
     finally:
         bufs.free()
     return DepthMaps(depth, cost, nsrc, report, ncons, points, frep)
+
+
+Mesh = namedtuple("Mesh", "vertices triangles report")
+Mesh.__doc__ = """TsdfVolume.mesh's result: vertices (a MESH_VERTEX_DTYPE array in edge-key order), triangles (m, 3) int32 with
+normals (v1 - v0) x (v2 - v0) towards the cameras, and the report {"cells", "vertices", "triangles"}."""
+
+
+class TsdfVolume:
+    """A dense truncated signed distance volume on the device (C ABI ps_volume in popsift_b200_mesh.h; an addition to the
+    reference's interface): shape = (nx, ny, nz) grid points from `origin` at spacing `voxel`, grid point (i, j, k) at
+    index i + nx (j + ny k).  Owns its three float32 arrays (tsdf, weight, grey) and clears them at construction."""
+
+    def __init__(self, origin, voxel, shape, device=0):
+        self._lib = load_library()
+        self.origin = tuple(float(v) for v in origin)
+        self.voxel = float(voxel)
+        self.shape = tuple(int(v) for v in shape)
+        self.device = int(device)
+        if len(self.origin) != 3 or len(self.shape) != 3:
+            raise PopSiftError("origin and shape have three components")
+        n = self.shape[0] * self.shape[1] * self.shape[2]
+        self._ptrs = [self._lib.ps_dev_alloc(max(n, 1) * 4) for _ in range(3)]
+        if not all(self._ptrs):
+            self.free()
+            raise PopSiftError("ps_dev_alloc failed")
+        self.clear()
+
+    def c_volume(self) -> PsVolume:
+        if not self._ptrs:
+            raise PopSiftError("the volume has been freed")
+        return PsVolume((C.c_double * 3)(*self.origin), self.voxel, *self.shape, 0, *self._ptrs)
+
+    def clear(self):
+        """every grid point's tsdf, weight and grey to 0 (ps_volume_clear)"""
+        _check(self._lib, self._lib.ps_volume_clear(self.device, C.byref(self.c_volume())), "ps_volume_clear")
+
+    def integrate(self, images, cameras, poses, depths, masks=None, trunc=None, min_consistent=0) -> dict:
+        """Folds depth maps into the volume (ps_tsdf_integrate): view v is images[v] (2-D uint8), cameras[v] (fx, fy, cx,
+        cy), poses[v] (world-to-camera R, t) and depths[v], a float32 map of the image's size (depth_maps' output);
+        masks[v] is the n_consistent map of depth_maps' filter, used when min_consistent > 0.  Images, depths and masks
+        may be numpy arrays (uploaded) or __cuda_array_interface__ arrays such as torch CUDA tensors (used in place;
+        depths and masks with contiguous rows).  trunc is the truncation distance in world units (default 3 voxels).
+        Returns the report {"updates", "touched"}."""
+        lib = self._lib
+        n = len(images)
+        if len(cameras) != n or len(poses) != n or len(depths) != n or (masks is not None and len(masks) != n):
+            raise PopSiftError("one camera, pose, depth map (and mask) per image expected")
+        if min_consistent > 0 and masks is None:
+            raise PopSiftError("min_consistent > 0 needs masks")
+        prm = PsTsdfParams(float(3.0 * self.voxel if trunc is None else trunc), int(min_consistent))
+        cam = _c_cameras(cameras)
+        bufs = _DevBuffers(lib)
+        try:
+            c_img, _ = _c_images(lib, bufs, images)
+            c_dep, _ = _c_images(lib, bufs, depths, np.float32)
+            c_msk = _c_images(lib, bufs, masks)[0] if masks is not None else None
+            for v in range(n):
+                for arr, size in ((c_dep, 4), (c_msk, 1)):
+                    if arr is not None and (arr[v].width, arr[v].height, arr[v].pitch) != (c_img[v].width, c_img[v].height,
+                                                                                            c_img[v].width * size):
+                        raise PopSiftError("view %d: a depth map or mask must have its image's size and contiguous rows" % v)
+            k = max(n, 1)
+            d_dep = (C.c_void_p * k)(*[c_dep[v].data for v in range(n)])
+            d_msk = (C.c_void_p * k)(*[c_msk[v].data for v in range(n)]) if c_msk is not None else None
+            rep = PsTsdfReport()
+            _check(lib, lib.ps_tsdf_integrate(self.device, n, c_img, cam.ctypes.data, _c_rigids(poses), d_dep, d_msk, C.byref(prm),
+                                              C.byref(self.c_volume()), C.byref(rep)), "ps_tsdf_integrate")
+        finally:
+            bufs.free()
+        return {"updates": int(rep.n_updates), "touched": int(rep.n_voxels_touched)}
+
+    def mesh(self, min_weight=1.0) -> Mesh:
+        """The surface T = 0 by marching tetrahedra over the cells whose 8 corners have weight >= min_weight
+        (ps_tsdf_mesh): a count call, then the call that fills outputs of that size."""
+        lib = self._lib
+        prm = PsMeshParams(float(min_weight), 0)
+        vol = self.c_volume()
+        rep = PsMeshReport()
+        rc = lib.ps_tsdf_mesh(self.device, C.byref(vol), C.byref(prm), 0, 0, None, None, C.byref(rep))
+        if rc not in (0, -5):
+            _check(lib, rc, "ps_tsdf_mesh")
+        report = {"cells": int(rep.n_cells), "vertices": int(rep.n_vertices), "triangles": int(rep.n_triangles)}
+        if rc == 0:
+            return Mesh(np.zeros(0, MESH_VERTEX_DTYPE), np.zeros((0, 3), np.int32), report)
+        if rep.n_vertices < 0:
+            raise PopSiftError("ps_tsdf_mesh: the mesh has 2^31 vertices or more")
+        bufs = _DevBuffers(lib)
+        try:
+            nv, nt = int(rep.n_vertices), int(rep.n_triangles)
+            d_v, d_t = bufs.alloc(nv * MESH_VERTEX_DTYPE.itemsize), bufs.alloc(nt * 12)
+            _check(lib, lib.ps_tsdf_mesh(self.device, C.byref(vol), C.byref(prm), nv, nt, d_v, d_t, C.byref(rep)), "ps_tsdf_mesh")
+            return Mesh(bufs.download(d_v, nv, MESH_VERTEX_DTYPE), bufs.download(d_t, (nt, 3), np.int32), report)
+        finally:
+            bufs.free()
+
+    def download(self):
+        """(tsdf, weight, grey) as float32 numpy arrays of shape (nz, ny, nx)"""
+        nx, ny, nz = self.shape
+        bufs = _DevBuffers(self._lib)
+        self.c_volume()
+        return tuple(bufs.download(p, (nz, ny, nx), np.float32) for p in self._ptrs)
+
+    def free(self):
+        """releases the device arrays now (otherwise when the object is collected)"""
+        lib = getattr(self, "_lib", None)
+        for p in getattr(self, "_ptrs", None) or []:
+            if p and lib is not None:
+                lib.ps_dev_free(p)
+        self._ptrs = []
+
+    def __del__(self):
+        self.free()
 
 
 def _track_observations(tracks, points, poses):

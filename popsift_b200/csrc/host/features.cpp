@@ -14,6 +14,7 @@
 #include "popsift_b200_viewgraph.h"
 #include "popsift_b200_twoview.h"
 #include "popsift_b200_depth.h"
+#include "popsift_b200_mesh.h"
 
 #include <algorithm>
 #include <cmath>
@@ -990,6 +991,128 @@ DensePoints filterDepthMaps(const std::vector<DeviceImage>& images, const std::v
         q.n_consistent = pts[i].n_consistent;
         q.grey = pts[i].grey;
     }
+    return out;
+}
+
+namespace {
+
+ps_volume c_volume(const DeviceVolume& v)
+{
+    ps_volume c;
+    std::copy(v.origin(), v.origin() + 3, c.origin);
+    c.voxel = v.voxel();
+    c.nx = v.nx();
+    c.ny = v.ny();
+    c.nz = v.nz();
+    c.pad_ = 0;
+    c.tsdf = v.tsdf();
+    c.weight = v.weight();
+    c.grey = v.grey();
+    return c;
+}
+
+} // namespace
+
+DeviceVolume::DeviceVolume(const double origin[3], double voxel, int nx, int ny, int nz, int device)
+    : _voxel(voxel), _n{nx, ny, nz}, _device(device)
+{
+    const std::string who = "popsift::DeviceVolume";
+    std::copy(origin, origin + 3, _origin);
+    if (nx < 2 || ny < 2 || nz < 2 || nx > 2048 || ny > 2048 || nz > 2048)
+        throw std::runtime_error(who + ": dimensions must lie in 2 .. 2048");
+    const size_t bytes = (size_t)nx * ny * nz * sizeof(float);
+    _tsdf = static_cast<float*>(ps_dev_alloc(bytes));
+    _weight = static_cast<float*>(ps_dev_alloc(bytes));
+    _grey = static_cast<float*>(ps_dev_alloc(bytes));
+    try {
+        if (!_tsdf || !_weight || !_grey) throw std::runtime_error(who + ": failed to allocate device memory");
+        clearVolume(*this);
+    } catch (...) {
+        ps_dev_free(_tsdf);
+        ps_dev_free(_weight);
+        ps_dev_free(_grey);
+        throw;
+    }
+}
+
+DeviceVolume::~DeviceVolume()
+{
+    ps_dev_free(_tsdf);
+    ps_dev_free(_weight);
+    ps_dev_free(_grey);
+}
+
+void clearVolume(DeviceVolume& volume)
+{
+    const ps_volume c = c_volume(volume);
+    check(ps_volume_clear(volume.device(), &c), "popsift::clearVolume", "ps_volume_clear");
+}
+
+TsdfReport integrateDepthMaps(DeviceVolume& volume, const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras,
+                              const std::vector<Rigid>& poses, const std::vector<DepthMap>& maps,
+                              const std::vector<std::vector<std::uint8_t>>& masks, const TsdfParams& params)
+{
+    const std::string who = "popsift::integrateDepthMaps";
+    const size_t n = images.size();
+    if (cameras.size() != n || poses.size() != n || maps.size() != n)
+        throw std::runtime_error(who + ": one camera, one pose and one depth map per image expected");
+    const bool use_masks = params.min_consistent > 0;
+    if (use_masks && masks.size() != n) throw std::runtime_error(who + ": one mask per image expected");
+    // the images, cameras and poses in the C ABI's layouts (DepthCall with every set its own reference)
+    std::vector<int> refs(n);
+    for (size_t v = 0; v < n; ++v) refs[v] = (int)v;
+    const DepthCall a(images, cameras, poses, refs, std::vector<std::vector<int>>(n), who);
+    std::vector<std::unique_ptr<DevBuf>> bufs;
+    std::vector<const float*> d_depth;
+    std::vector<const uint8_t*> d_mask;
+    for (size_t v = 0; v < n; ++v) {
+        const size_t px = (size_t)std::max(images[v].width, 0) * (size_t)std::max(images[v].height, 0);
+        if (maps[v].width != images[v].width || maps[v].height != images[v].height || maps[v].depth.size() != px)
+            throw std::runtime_error(who + ": a depth map does not match its image");
+        bufs.emplace_back(new DevBuf(px * 4, who));
+        if (px) check(ps_host_to_dev(bufs.back()->p, maps[v].depth.data(), px * 4), who);
+        d_depth.push_back(static_cast<const float*>(bufs.back()->p));
+        if (use_masks) {
+            if (masks[v].size() != px) throw std::runtime_error(who + ": a mask does not match its image");
+            bufs.emplace_back(new DevBuf(px, who));
+            if (px) check(ps_host_to_dev(bufs.back()->p, masks[v].data(), px), who);
+            d_mask.push_back(static_cast<const uint8_t*>(bufs.back()->p));
+        }
+    }
+    const ps_volume c = c_volume(volume);
+    const ps_tsdf_params prm{params.trunc, params.min_consistent};
+    ps_tsdf_report rep;
+    check(ps_tsdf_integrate(volume.device(), (int)n, a.img.data(), a.cam.data(), a.pose.data(), d_depth.data(),
+                            use_masks ? d_mask.data() : nullptr, &prm, &c, &rep),
+          who, "ps_tsdf_integrate");
+    TsdfReport out;
+    out.n_updates = rep.n_updates;
+    out.n_voxels_touched = rep.n_voxels_touched;
+    return out;
+}
+
+Mesh extractMesh(const DeviceVolume& volume, const MeshParams& params)
+{
+    const std::string who = "popsift::extractMesh";
+    const ps_volume c = c_volume(volume);
+    const ps_mesh_params prm{params.min_weight, 0};
+    ps_mesh_report rep;
+    const int rc = ps_tsdf_mesh(volume.device(), &c, &prm, 0, 0, nullptr, nullptr, &rep);
+    if (rc != PS_ERR_OVERFLOW) check(rc, who, "ps_tsdf_mesh");
+    Mesh out;
+    out.n_cells = rep.n_cells;
+    if (rc == PS_OK) return out;   // no triangles
+    if (rep.n_vertices < 0 || rep.n_vertices >= 0x80000000LL)
+        throw std::runtime_error(who + ": the mesh has 2^31 vertices or more");
+    DevBuf d_v((size_t)rep.n_vertices * sizeof(ps_mesh_vertex), who), d_t((size_t)rep.n_triangles * 3 * sizeof(int32_t), who);
+    check(ps_tsdf_mesh(volume.device(), &c, &prm, rep.n_vertices, rep.n_triangles, static_cast<ps_mesh_vertex*>(d_v.p),
+                       static_cast<int32_t*>(d_t.p), &rep),
+          who, "ps_tsdf_mesh");
+    out.vertices.resize((size_t)rep.n_vertices);
+    out.triangles.resize((size_t)rep.n_triangles * 3);
+    static_assert(sizeof(MeshVertex) == sizeof(ps_mesh_vertex), "vertex layout");
+    if (!out.vertices.empty()) check(ps_dev_to_host(out.vertices.data(), d_v.p, out.vertices.size() * sizeof(MeshVertex)), who);
+    if (!out.triangles.empty()) check(ps_dev_to_host(out.triangles.data(), d_t.p, out.triangles.size() * sizeof(int)), who);
     return out;
 }
 

@@ -17,6 +17,7 @@
 #include "popsift_b200_global.h"
 #include "popsift_b200_twoview.h"
 #include "popsift_b200_depth.h"
+#include "popsift_b200_mesh.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1814,6 +1815,92 @@ extern "C" int ps_depth_filter(int device, int n_sets, const ps_image* images, c
     const int rc = finish("ps_depth_filter", n, err);
     if (rc == PS_OK) *report = rep;
     return rc;
+}
+
+// a volume's geometry and arrays (the device already set): finite origin and voxel > 0, dimensions 2 .. 2048 with fewer
+// than 2^31 grid points, three disjoint arrays of device memory on `device`
+static bool volume_ok(int device, const ps_volume* vol)
+{
+    if (!vol) return false;
+    for (double o : vol->origin)
+        if (!std::isfinite(o)) return false;
+    if (!std::isfinite(vol->voxel) || !(vol->voxel > 0.0)) return false;
+    for (int d : {vol->nx, vol->ny, vol->nz})
+        if (d < 2 || d > 2048) return false;
+    const size_t n = (size_t)vol->nx * vol->ny * vol->nz;
+    if (n >= 0x80000000ull) return false;
+    const float* arr[3] = {vol->tsdf, vol->weight, vol->grey};
+    for (int a = 0; a < 3; ++a) {
+        if (ps_pointer_device(arr[a]) != device) return false;
+        for (int b = a + 1; b < 3; ++b)
+            if (ranges_overlap(arr[a], 4 * n, arr[b], 4 * n)) return false;
+    }
+    return true;
+}
+
+extern "C" int ps_volume_clear(int device, const ps_volume* vol)
+{
+    if (!vol) return PS_ERR_ARG;
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (!volume_ok(device, vol)) return PS_ERR_ARG;
+    const char* err = nullptr;
+    return finish("ps_volume_clear", run_volume_clear(*vol, nullptr, &err), err);
+}
+
+extern "C" int ps_tsdf_integrate(int device, int n_views, const ps_image* images, const ps_camera* cams, const ps_rigid* poses,
+                                 const float* const* d_depth, const uint8_t* const* d_n_consistent, const ps_tsdf_params* prm,
+                                 const ps_volume* vol, ps_tsdf_report* report)
+{
+    if (n_views < 0 || !prm || !vol || !report) return PS_ERR_ARG;
+    if (!std::isfinite(prm->trunc) || !(prm->trunc > 0.0f) || prm->min_consistent < 0 || prm->min_consistent > 255) return PS_ERR_ARG;
+    if (n_views > 0 && (!images || !cams || !poses || !d_depth || (prm->min_consistent > 0 && !d_n_consistent))) return PS_ERR_ARG;
+    for (int v = 0; v < n_views; ++v) {
+        const ps_image& im = images[v];
+        if (im.width < 1 || im.height < 1 || im.width > 65535 || im.height > 65535 || im.pitch < im.width) return PS_ERR_ARG;
+        const ps_camera& c = cams[v];
+        if (!std::isfinite(c.fx) || !(c.fx > 0.0f) || !std::isfinite(c.fy) || !(c.fy > 0.0f) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
+            return PS_ERR_ARG;
+        if (!rigid_ok(poses[v])) return PS_ERR_ARG;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (!volume_ok(device, vol)) return PS_ERR_ARG;
+    for (int v = 0; v < n_views; ++v) {
+        if (ps_pointer_device(images[v].data) != device || ps_pointer_device(d_depth[v]) != device) return PS_ERR_ARG;
+        if (prm->min_consistent > 0 && ps_pointer_device(d_n_consistent[v]) != device) return PS_ERR_ARG;
+    }
+    if (n_views == 0) {
+        std::memset(report, 0, sizeof(*report));
+        return PS_OK;
+    }
+    const char* err = nullptr;
+    ps_tsdf_report rep{};
+    const int n = run_tsdf_integrate(n_views, images, cams, poses, d_depth, d_n_consistent, *prm, *vol, &rep, nullptr, &err);
+    const int rc = finish("ps_tsdf_integrate", n, err);
+    if (rc == PS_OK) *report = rep;
+    return rc;
+}
+
+extern "C" int ps_tsdf_mesh(int device, const ps_volume* vol, const ps_mesh_params* prm, int64_t max_vertices, int64_t max_triangles,
+                            ps_mesh_vertex* d_vertices, int32_t* d_triangles, ps_mesh_report* report)
+{
+    if (!vol || !prm || !report || max_vertices < 0 || max_triangles < 0) return PS_ERR_ARG;
+    if (!std::isfinite(prm->min_weight) || !(prm->min_weight > 0.0f)) return PS_ERR_ARG;
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (!volume_ok(device, vol)) return PS_ERR_ARG;
+    if (max_vertices > 0 && ps_pointer_device(d_vertices) != device) return PS_ERR_ARG;
+    if (max_triangles > 0 && ps_pointer_device(d_triangles) != device) return PS_ERR_ARG;
+    const char* err = nullptr;
+    ps_mesh_report rep{};
+    bool overflow = false;
+    const int n = run_tsdf_mesh(*vol, *prm, max_vertices, max_triangles, d_vertices, d_triangles, &rep, &overflow, nullptr, &err);
+    const int rc = finish("ps_tsdf_mesh", n, err);
+    if (rc != PS_OK) return rc;
+    *report = rep;
+    if (overflow) {
+        g_create_error = "ps_tsdf_mesh: the mesh does not fit the outputs' capacities";
+        return PS_ERR_OVERFLOW;
+    }
+    return PS_OK;
 }
 
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)

@@ -9,6 +9,7 @@
 #include "popsift_b200_viewgraph.h"
 #include "popsift_b200_twoview.h"
 #include "popsift_b200_depth.h"
+#include "popsift_b200_mesh.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
@@ -342,5 +343,16 @@ int run_depth_filter(int n_sets, const ps_image* images, const ps_camera* cams, 
                      const int32_t* src_start, const int32_t* src_sets, const float* const* d_depth, const ps_depth_filter_params& prm,
                      uint8_t* const* d_n_consistent, ps_dense_point* d_points, ps_depth_filter_report* report, cudaStream_t st,
                      const char** err);
+
+// surface meshes (include/popsift_b200_mesh.h, k_mesh.cu), arguments already validated.  Asynchronous clear; the other two
+// are synchronous on `st`: the integration writes *report when it returns >= 0 and n_views > 0; the extraction writes
+// *report when it returns >= 0, and the outputs only when *overflow is false.  Return the number of kernels launched or
+// -1 (*err set).
+int run_volume_clear(const ps_volume& vol, cudaStream_t st, const char** err);
+int run_tsdf_integrate(int n_views, const ps_image* images, const ps_camera* cams, const ps_rigid* poses, const float* const* d_depth,
+                       const uint8_t* const* d_n_consistent, const ps_tsdf_params& prm, const ps_volume& vol, ps_tsdf_report* report,
+                       cudaStream_t st, const char** err);
+int run_tsdf_mesh(const ps_volume& vol, const ps_mesh_params& prm, int64_t max_vertices, int64_t max_triangles, ps_mesh_vertex* d_vertices,
+                  int32_t* d_triangles, ps_mesh_report* report, bool* overflow, cudaStream_t st, const char** err);
 
 } // namespace psb

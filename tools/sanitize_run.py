@@ -247,3 +247,15 @@ if only in ("all", "scale"):
     tv["R"], tv["n_front"], tv["n_inliers"] = np.asarray(Rp, np.float32), nf, nf
     out = api.rotation_averaging(257, pairs, tv, max_iters=2, cg_max_iters=50, min_inliers=0)
     print("scale rotations", out[-1], flush=True)
+if only in ("all", "mesh"):
+    # integration over more views than one shared-memory chunk with masks, partial blocks on every axis; extraction of
+    # the result, of an empty volume, and the count-only call
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import test_mesh as tm
+    imgs, cams, poses, depths, masks = tm._random_views(1, 70, w=40, h=30, dist=1.2)
+    vol = api.TsdfVolume((-0.6, -0.5, -0.55), 0.02, (61, 50, 55))
+    print("mesh integrate", vol.integrate(imgs, cams, poses, depths, masks, trunc=0.05, min_consistent=1), flush=True)
+    print("mesh extract", vol.mesh().report, flush=True)
+    vol.clear()
+    print("mesh empty", vol.mesh().report, flush=True)
+    vol.free()
