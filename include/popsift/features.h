@@ -546,6 +546,60 @@ struct Mesh
 /// that size).  Throws for the arguments ps_tsdf_mesh refuses.
 Mesh extractMesh(const DeviceVolume& volume, const MeshParams& params = MeshParams());
 
+/// Settings of renderMesh (ps_render_params in popsift_b200_render.h).
+struct RenderParams
+{
+    float z_near = 1e-3f;                // triangles with a vertex closer than this are not drawn (no clipping)
+};
+
+/// One view's rendered maps, row-major width x height: camera-frame depth (0 where no triangle covers the pixel) and the
+/// nearest triangle (-1 where none).
+struct RenderMap
+{
+    int                width = 0, height = 0;
+    std::vector<float> depth;
+    std::vector<int>   triangle;
+};
+
+/// renderMesh's maps, one per view, and the totals of ps_render_report.
+struct RenderedMesh
+{
+    std::vector<RenderMap> maps;
+    long long              n_drawn = 0, n_big = 0, n_covered = 0;
+};
+
+/// Renders `mesh` into posed views with a z-buffer on `device` (an addition to the reference's interface; C ABI
+/// ps_mesh_render): view v is cameras[v], poses[v] and sizes[v] = (width, height).  The maps are in depthMaps' layout.
+/// Throws when the sizes disagree, and for the arguments ps_mesh_render refuses.
+RenderedMesh renderMesh(const Mesh& mesh, const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+                        const std::vector<std::pair<int, int>>& sizes, const RenderParams& params = RenderParams(), int device = 0);
+
+/// Settings of textureMesh (same fields and rules as ps_texture_params; cells_per_row 0 keeps the atlas close to square).
+struct TextureParams
+{
+    int   cell = 8;                      // texels per cell side, 3 .. 64
+    int   cells_per_row = 0;             // 0: ceil(sqrt(triangles)), at most 65535 / cell
+    float depth_tol = 0.01f;             // relative occlusion tolerance
+    float min_cos = 0.1f;                // facing test, [0, 1)
+    float z_near = 1e-3f;
+};
+
+/// textureMesh's result: the atlas (width x height, row-major grey), the view per triangle (-1: the vertex-grey fallback)
+/// and the totals of ps_texture_report.  Triangle m's corners sit at texel positions (b, b), (cell - b, b), (b, cell - b)
+/// of cell (m mod cells_per_row, m div cells_per_row), b = 1.
+struct TexturedMesh
+{
+    int                       width = 0, height = 0, cell = 0, cells_per_row = 0;
+    std::vector<std::uint8_t> atlas;
+    std::vector<int>          view;
+    long long                 n_viewed = 0, n_fallback = 0;
+};
+
+/// A texture atlas of `mesh` from the images on `device` (C ABI ps_mesh_render, then ps_mesh_texture on the device maps,
+/// with no host copy between them).  Throws when the sizes disagree, and for the arguments either call refuses.
+TexturedMesh textureMesh(const Mesh& mesh, const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras,
+                         const std::vector<Rigid>& poses, const TextureParams& params = TextureParams(), int device = 0);
+
 /// Settings of twoViewGeometries' classification (same fields and rules as ps_two_view_config_params in
 /// popsift_b200_twoview.h; the pure-rotation test uses PoseParams::threshold).
 struct TwoViewConfigParams

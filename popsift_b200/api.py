@@ -263,6 +263,31 @@ MESH_VERTEX_DTYPE = np.dtype([("X", "<f4", 3), ("grey", "<f4")])
 assert C.sizeof(PsVolume) == 72 and C.sizeof(PsTsdfParams) == 8 and C.sizeof(PsMeshParams) == 8
 assert C.sizeof(PsTsdfReport) == 16 and C.sizeof(PsMeshReport) == 24 and MESH_VERTEX_DTYPE.itemsize == 16
 
+
+class PsRenderParams(C.Structure):
+    """ps_render_params (8 bytes)"""
+    _fields_ = [("z_near", C.c_float), ("pad_", C.c_int32)]
+
+
+class PsRenderReport(C.Structure):
+    """ps_render_report (24 bytes)"""
+    _fields_ = [("n_drawn", C.c_int64), ("n_big", C.c_int64), ("n_covered", C.c_int64)]
+
+
+class PsTextureParams(C.Structure):
+    """ps_texture_params (24 bytes)"""
+    _fields_ = [("cell", C.c_int32), ("cells_per_row", C.c_int32), ("depth_tol", C.c_float), ("min_cos", C.c_float),
+                ("z_near", C.c_float), ("pad_", C.c_int32)]
+
+
+class PsTextureReport(C.Structure):
+    """ps_texture_report (16 bytes)"""
+    _fields_ = [("n_viewed", C.c_int64), ("n_fallback", C.c_int64)]
+
+
+assert C.sizeof(PsRenderParams) == 8 and C.sizeof(PsRenderReport) == 24
+assert C.sizeof(PsTextureParams) == 24 and C.sizeof(PsTextureReport) == 16
+
 RA_TERMINATION = ("max_iters", "step_tol", "no_pairs")
 GP_TERMINATION = ("max_iters", "function_tol", "no_observations")
 assert C.sizeof(PsRotationParams) == 40 and C.sizeof(PsRotationReport) == 40
@@ -297,6 +322,8 @@ TWOVIEW_EXPORTS = ["ps_two_view_config_batch"]
 DEPTH_EXPORTS = ["ps_depth_maps", "ps_depth_filter"]
 # surface meshes, declared in popsift_b200_mesh.h (same library)
 MESH_EXPORTS = ["ps_volume_clear", "ps_tsdf_integrate", "ps_tsdf_mesh"]
+# mesh rendering and texturing, declared in popsift_b200_render.h (same library)
+RENDER_EXPORTS = ["ps_mesh_render", "ps_mesh_texture"]
 
 _lib = None
 
@@ -389,6 +416,11 @@ def load_library():
                                         C.POINTER(PsTsdfParams), C.POINTER(PsVolume), C.POINTER(PsTsdfReport)]
         L.ps_tsdf_mesh.argtypes = [C.c_int, C.POINTER(PsVolume), C.POINTER(PsMeshParams), C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                    C.POINTER(PsMeshReport)]
+    if hasattr(L, "ps_mesh_render"):
+        L.ps_mesh_render.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                     C.POINTER(PsRenderParams), C.c_void_p, C.c_void_p, C.POINTER(PsRenderReport)]
+        L.ps_mesh_texture.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                      C.c_int64, C.POINTER(PsTextureParams), C.c_void_p, C.c_void_p, C.POINTER(PsTextureReport)]
     L.ps_pointer_device.argtypes = [C.c_void_p]
     L.ps_host_to_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.ps_debug_plane.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
@@ -1953,6 +1985,175 @@ class TsdfVolume:
 
     def __del__(self):
         self.free()
+
+
+Rendered = namedtuple("Rendered", "depth triangle report")
+Rendered.__doc__ = """render_mesh's result: per view the camera-frame depth (float32 (h, w), 0 where no triangle covers the pixel)
+and the nearest triangle (int32 (h, w), -1 where none), and the report {"drawn", "big", "covered"}."""
+
+TexturedMesh = namedtuple("TexturedMesh", "atlas view uv report")
+TexturedMesh.__doc__ = """texture_mesh's result: the uint8 atlas (H, W), the view each triangle was textured from (int32, -1 for
+the vertex-grey fallback), the corners' texture coordinates uv (m, 3, 2) in atlas texel units (atlas_uv) and the report
+{"viewed", "fallback"}."""
+
+
+def _mesh_arrays(lib, bufs, mesh):
+    """device pointers and counts of a Mesh's vertices and triangles: numpy arrays are uploaded, __cuda_array_interface__
+    arrays (a float32 (n, 4) vertex array and an int32 (m, 3) triangle array, contiguous) are used in place"""
+    out = []
+    for a, dtype, cols in ((mesh.vertices, np.float32, 4), (mesh.triangles, np.int32, 3)):
+        cai = getattr(a, "__cuda_array_interface__", None)
+        if cai is not None:
+            shape = tuple(int(v) for v in cai["shape"])
+            if len(shape) != 2 or shape[1] != cols or np.dtype(cai["typestr"]) != np.dtype(dtype) or cai.get("strides") not in (None, (cols * 4, 4)):
+                raise PopSiftError("a contiguous %s (n, %d) device array expected" % (np.dtype(dtype), cols))
+            out += [int(cai["data"][0]), shape[0]]
+        else:
+            h = np.ascontiguousarray(a)
+            if h.dtype == MESH_VERTEX_DTYPE:
+                h = h.view(np.float32).reshape(-1, 4)
+            h = np.ascontiguousarray(h, dtype).reshape(-1, cols)
+            out += [bufs.upload(h), h.shape[0]]
+    return out
+
+
+def _render_dev(lib, device, mesh_dev, cameras, poses, sizes, z_near, d_depth, d_tri) -> dict:
+    d_v, nv, d_t, nt = mesh_dev
+    n = len(sizes)
+    cam = _c_cameras(cameras)
+    if len(cam) != n or len(poses) != n:
+        raise PopSiftError("one camera, one pose and one size per view expected")
+    sz = np.ascontiguousarray(np.asarray(sizes, np.int32).reshape(-1, 2) if n else np.zeros((1, 2), np.int32))
+    k = max(n, 1)
+    rep = PsRenderReport()
+    _check(lib, lib.ps_mesh_render(device, n, sz.ctypes.data, cam.ctypes.data, _c_rigids(poses), d_v, nv, d_t, nt,
+                                   C.byref(PsRenderParams(float(z_near), 0)), (C.c_void_p * k)(*d_depth), (C.c_void_p * k)(*d_tri),
+                                   C.byref(rep)), "ps_mesh_render")
+    return {"drawn": int(rep.n_drawn), "big": int(rep.n_big), "covered": int(rep.n_covered)}
+
+
+def render_mesh(mesh, cameras, poses, sizes, z_near=1e-3, device=0) -> Rendered:
+    """Renders a triangle mesh into posed views with a z-buffer (C ABI ps_mesh_render in popsift_b200_render.h; an addition
+    to the reference's interface).  `mesh` is TsdfVolume.mesh's Mesh (or any object with vertices, a MESH_VERTEX_DTYPE or
+    float32 (n, 4) array, and triangles, int32 (m, 3)); numpy arrays are uploaded, torch CUDA tensors used in place.
+    View v is cameras[v] (fx, fy, cx, cy), poses[v] (world-to-camera R, t) and sizes[v] = (width, height).  Triangles with a
+    vertex closer than z_near are not drawn (no near-plane clipping).  The maps are in depth_maps' layout and convention."""
+    lib = load_library()
+    bufs = _DevBuffers(lib)
+    try:
+        mesh_dev = _mesh_arrays(lib, bufs, mesh)
+        shapes = [(int(h), int(w)) for w, h in sizes]
+        d_depth = [bufs.alloc(h * w * 4) for h, w in shapes]
+        d_tri = [bufs.alloc(h * w * 4) for h, w in shapes]
+        report = _render_dev(lib, device, mesh_dev, cameras, poses, sizes, z_near, d_depth, d_tri)
+        depth = [bufs.download(d, s, np.float32) for d, s in zip(d_depth, shapes)]
+        tri = [bufs.download(d, s, np.int32) for d, s in zip(d_tri, shapes)]
+    finally:
+        bufs.free()
+    return Rendered(depth, tri, report)
+
+
+def atlas_cells_per_row(n_triangles, cell) -> int:
+    """texture_mesh's default: the atlas close to square, at most 65535 texels wide"""
+    return max(1, min(int(np.ceil(np.sqrt(max(int(n_triangles), 1)))), 65535 // int(cell)))
+
+
+def atlas_uv(n_triangles, cell, cells_per_row):
+    """the corners' positions (m, 3, 2) in atlas texel units (x right, y down) and the atlas size (W, H): triangle m owns
+    cell (m mod cells_per_row, m div cells_per_row), its corners at (b, b), (cell - b, b), (b, cell - b) of the cell, b = 1"""
+    m = np.arange(int(n_triangles))
+    ox, oy = (m % cells_per_row) * cell, (m // cells_per_row) * cell
+    corner = np.array([[1, 1], [cell - 1, 1], [1, cell - 1]], np.float64)
+    uv = np.stack([ox, oy], 1)[:, None, :].astype(np.float64) + corner[None]
+    W, H = int(cells_per_row * cell), int(-(-int(n_triangles) // cells_per_row) * cell)
+    return uv, W, H
+
+
+def texture_mesh(mesh, images, cameras, poses, cell=8, cells_per_row=None, depth_tol=0.01, min_cos=0.1, z_near=1e-3,
+                 device=None) -> TexturedMesh:
+    """A texture atlas of a mesh from posed grey images (C ABI ps_mesh_render, then ps_mesh_texture on the device maps, no
+    host copy between them; popsift_b200_render.h).  Each triangle takes the view that sees it (facing it by at least
+    min_cos, its corners and centroid not occluded beyond depth_tol relative depth) with the largest projected area, and
+    gets a cell x cell cell of the atlas sampled bilinearly from that image; a triangle no view sees falls back to its
+    vertices' grey.  `images` are 2-D uint8 numpy arrays (uploaded) or torch CUDA tensors (used in place, any row pitch),
+    with cameras and poses as render_mesh; `mesh` as render_mesh.  cells_per_row defaults to atlas_cells_per_row."""
+    lib = load_library()
+    n_views = len(images)
+    bufs = _DevBuffers(lib)
+    try:
+        c_img, dev0 = _c_images(lib, bufs, images)
+        if device is None:
+            device = dev0 if dev0 is not None else 0
+        mesh_dev = _mesh_arrays(lib, bufs, mesh)
+        nt = mesh_dev[3]
+        cpr = atlas_cells_per_row(nt, cell) if cells_per_row is None else int(cells_per_row)
+        uv, W, H = atlas_uv(nt, int(cell), max(cpr, 1))
+        sizes = [(int(c_img[v].width), int(c_img[v].height)) for v in range(n_views)]
+        d_depth = [bufs.alloc(w * h * 4) for w, h in sizes]
+        d_tri = [bufs.alloc(w * h * 4) for w, h in sizes]
+        _render_dev(lib, device, mesh_dev, cameras, poses, sizes, z_near, d_depth, d_tri)
+        d_atlas, d_view = bufs.alloc(W * H), bufs.alloc(nt * 4)
+        prm = PsTextureParams(int(cell), cpr, float(depth_tol), float(min_cos), float(z_near), 0)
+        rep = PsTextureReport()
+        k = max(n_views, 1)
+        d_v, nv, d_t, _ = mesh_dev
+        cam = _c_cameras(cameras)
+        _check(lib, lib.ps_mesh_texture(device, n_views, c_img, cam.ctypes.data, _c_rigids(poses), (C.c_void_p * k)(*d_depth),
+                                        d_v, nv, d_t, nt, C.byref(prm), d_atlas, d_view, C.byref(rep)), "ps_mesh_texture")
+        atlas = bufs.download(d_atlas, (H, W), np.uint8)
+        view = bufs.download(d_view, nt, np.int32)
+    finally:
+        bufs.free()
+    return TexturedMesh(atlas, view, uv, {"viewed": int(rep.n_viewed), "fallback": int(rep.n_fallback)})
+
+
+def _png_grey(path, img):
+    """an 8-bit grey PNG (colour type 0, no interlace) with the standard library only"""
+    import struct
+    import zlib
+    img = np.ascontiguousarray(img, np.uint8)
+    h, w = img.shape
+
+    def chunk(tag, data):
+        return struct.pack(">I", len(data)) + tag + data + struct.pack(">I", zlib.crc32(tag + data) & 0xffffffff)
+
+    raw = np.concatenate([np.zeros((h, 1), np.uint8), img], 1).tobytes()   # filter type 0 on every row
+    with open(path, "wb") as f:
+        f.write(b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 8, 0, 0, 0, 0)) +
+                chunk(b"IDAT", zlib.compress(raw, 6)) + chunk(b"IEND", b""))
+
+
+def write_obj(path, mesh, textured=None):
+    """Writes `mesh` as a Wavefront OBJ.  With `textured` (texture_mesh's result for this mesh) it also writes, next to it,
+    an MTL and an 8-bit grey PNG of the atlas, and every face corner gets its texture coordinate (vt, v flipped to OBJ's
+    bottom-left origin).  Returns the paths written."""
+    base = os.path.splitext(path)[0]
+    V = np.asarray(mesh.vertices)
+    X = V["X"] if V.dtype == MESH_VERTEX_DTYPE else np.asarray(V, np.float32).reshape(-1, 4)[:, :3]
+    T = np.asarray(mesh.triangles, np.int64).reshape(-1, 3)
+    lines = []
+    written = [path]
+    if textured is not None:
+        H, W = textured.atlas.shape
+        if len(textured.uv) != len(T):
+            raise PopSiftError("the texture is not this mesh's")
+        name = os.path.basename(base)
+        lines.append("mtllib %s.mtl" % name)
+        with open(base + ".mtl", "w") as f:
+            f.write("newmtl atlas\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd %s.png\n" % name)
+        _png_grey(base + ".png", textured.atlas)
+        written += [base + ".mtl", base + ".png"]
+    lines += ["v %.9g %.9g %.9g" % tuple(x) for x in X.astype(np.float64)]
+    if textured is not None:
+        uv = textured.uv.reshape(-1, 2)
+        lines += ["vt %.9g %.9g" % (u / W, 1.0 - v / H) for u, v in uv]
+        lines.append("usemtl atlas")
+        lines += ["f %d/%d %d/%d %d/%d" % (a + 1, 3 * m + 1, b + 1, 3 * m + 2, c + 1, 3 * m + 3) for m, (a, b, c) in enumerate(T)]
+    else:
+        lines += ["f %d %d %d" % (a + 1, b + 1, c + 1) for a, b, c in T]
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")
+    return written
 
 
 def _track_observations(tracks, points, poses):

@@ -26,7 +26,7 @@ NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "--fmad=false",   # no implicit contraction anywhere; every fma in the kernels is explicit
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu", "k_pose.cu", "k_retrieval.cu", "k_tracks.cu", "k_triangulate.cu", "k_bundle.cu", "k_global.cu", "k_viewgraph.cu", "k_twoview.cu", "k_depth.cu", "k_mesh.cu", "workspace.cu",
+LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu", "k_pose.cu", "k_retrieval.cu", "k_tracks.cu", "k_triangulate.cu", "k_bundle.cu", "k_global.cu", "k_viewgraph.cu", "k_twoview.cu", "k_depth.cu", "k_mesh.cu", "k_render.cu", "workspace.cu",
                "host/sift_conf.cpp", "host/features.cpp", "host/popsift.cpp", "host/device_prop.cpp", "host/log_dump.cpp"]
 DEMO_SOURCES = ["app/popsift_demo.cpp", "app/pgmread.cpp"]
 MATCH_SOURCES = ["app/popsift_match.cpp"]            # + app/pgmread.cpp
@@ -95,6 +95,10 @@ MESH_MATH_CHECK = os.path.join(BIN_DIR, "mesh_math_check")
 MESH_MATH_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "mesh_math_check.cpp")
 MESH_CHECK = os.path.join(BIN_DIR, "mesh_check")
 MESH_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "mesh_check.cpp")
+RENDER_MATH_CHECK = os.path.join(BIN_DIR, "render_math_check")
+RENDER_MATH_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "render_math_check.cpp")
+RENDER_CHECK = os.path.join(BIN_DIR, "render_check")
+RENDER_CHECK_SRC = os.path.join(ROOT, "tests", "cpp", "render_check.cpp")
 
 
 def _newer(target: str, deps) -> bool:
@@ -292,6 +296,16 @@ def build(verbose: bool = False, force: bool = False) -> str:
     if os.path.exists(MESH_CHECK_SRC) and (force or _newer(MESH_CHECK, [MESH_CHECK_SRC, LIB] + hdrs)):
         # popsift::clearVolume / integrateDepthMaps / extractMesh against the C ABI (popsift_b200_mesh.h)
         subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), MESH_CHECK_SRC, "-o", MESH_CHECK,
+                               "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
+    render_hdrs = [os.path.join(CSRC, "k_render.h"), sample_hdr]
+    if os.path.exists(RENDER_MATH_CHECK_SRC) and (force or _newer(RENDER_MATH_CHECK, [RENDER_MATH_CHECK_SRC] + render_hdrs)):
+        # host-only: the rasteriser's projection, edge functions, depth and key, and the texturing's facing test, probe,
+        # texel barycentrics and bilinear sample, the same functions the kernels use (no CUDA, no library); no contraction
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-I" + CSRC, RENDER_MATH_CHECK_SRC, "-o",
+                               RENDER_MATH_CHECK])
+    if os.path.exists(RENDER_CHECK_SRC) and (force or _newer(RENDER_CHECK, [RENDER_CHECK_SRC, LIB] + hdrs)):
+        # popsift::renderMesh / textureMesh against the C ABI (popsift_b200_render.h)
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"), RENDER_CHECK_SRC, "-o", RENDER_CHECK,
                                "-L" + LIB_DIR, "-lpopsift_b200", "-Wl,-rpath," + "$ORIGIN/../lib", "-lpthread"])
     pgm_src = os.path.join(CSRC, "app", "pgmread.cpp")
     if os.path.exists(PGM_CHECK_SRC) and (force or _newer(PGM_CHECK, [PGM_CHECK_SRC, pgm_src, os.path.join(CSRC, "app", "pgmread.h")])):

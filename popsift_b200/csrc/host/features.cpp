@@ -15,6 +15,7 @@
 #include "popsift_b200_twoview.h"
 #include "popsift_b200_depth.h"
 #include "popsift_b200_mesh.h"
+#include "popsift_b200_render.h"
 
 #include <algorithm>
 #include <cmath>
@@ -1113,6 +1114,138 @@ Mesh extractMesh(const DeviceVolume& volume, const MeshParams& params)
     static_assert(sizeof(MeshVertex) == sizeof(ps_mesh_vertex), "vertex layout");
     if (!out.vertices.empty()) check(ps_dev_to_host(out.vertices.data(), d_v.p, out.vertices.size() * sizeof(MeshVertex)), who);
     if (!out.triangles.empty()) check(ps_dev_to_host(out.triangles.data(), d_t.p, out.triangles.size() * sizeof(int)), who);
+    return out;
+}
+
+namespace {
+
+// a mesh on the device for the render calls
+struct DeviceMesh {
+    DevBuf v, t;
+    int64_t nv, nt;
+    DeviceMesh(const Mesh& mesh, const std::string& who)
+        : v(mesh.vertices.size() * sizeof(ps_mesh_vertex), who), t(mesh.triangles.size() * sizeof(int32_t), who),
+          nv((int64_t)mesh.vertices.size()), nt((int64_t)mesh.triangles.size() / 3)
+    {
+        if (mesh.triangles.size() % 3) throw std::runtime_error(who + ": three vertex indices per triangle expected");
+        if (nv) check(ps_host_to_dev(v.p, mesh.vertices.data(), (size_t)nv * sizeof(ps_mesh_vertex)), who);
+        if (nt) check(ps_host_to_dev(t.p, mesh.triangles.data(), (size_t)nt * 3 * sizeof(int32_t)), who);
+    }
+};
+
+std::vector<ps_camera> c_cameras(const std::vector<Camera>& cameras)
+{
+    std::vector<ps_camera> out;
+    for (const Camera& c : cameras) out.push_back(ps_camera{c.fx, c.fy, c.cx, c.cy});
+    return out;
+}
+
+std::vector<ps_rigid> c_rigids(const std::vector<Rigid>& poses)
+{
+    std::vector<ps_rigid> out(poses.size());
+    for (size_t i = 0; i < poses.size(); ++i) {
+        std::copy(poses[i].R, poses[i].R + 9, out[i].R);
+        std::copy(poses[i].t, poses[i].t + 3, out[i].t);
+    }
+    return out;
+}
+
+// ps_mesh_render into device maps (bufs: depth, triangle per view)
+ps_render_report render_dev(const DeviceMesh& m, const std::vector<ps_camera>& cam, const std::vector<ps_rigid>& pose,
+                            const std::vector<int32_t>& sizes, float z_near, std::vector<std::unique_ptr<DevBuf>>& bufs,
+                            std::vector<float*>& d_depth, std::vector<int32_t*>& d_tri, int device, const std::string& who)
+{
+    const size_t n = cam.size();
+    for (size_t v = 0; v < n; ++v) {
+        const size_t px = (size_t)std::max(sizes[2 * v], 0) * (size_t)std::max(sizes[2 * v + 1], 0);
+        bufs.emplace_back(new DevBuf(px * 4, who));
+        d_depth.push_back(static_cast<float*>(bufs.back()->p));
+        bufs.emplace_back(new DevBuf(px * 4, who));
+        d_tri.push_back(static_cast<int32_t*>(bufs.back()->p));
+    }
+    const ps_render_params prm{z_near, 0};
+    ps_render_report rep;
+    check(ps_mesh_render(device, (int)n, sizes.data(), cam.data(), pose.data(), static_cast<const ps_mesh_vertex*>(m.v.p), m.nv,
+                         static_cast<const int32_t*>(m.t.p), m.nt, &prm, d_depth.data(), d_tri.data(), &rep),
+          who, "ps_mesh_render");
+    return rep;
+}
+
+} // namespace
+
+RenderedMesh renderMesh(const Mesh& mesh, const std::vector<Camera>& cameras, const std::vector<Rigid>& poses,
+                        const std::vector<std::pair<int, int>>& sizes, const RenderParams& params, int device)
+{
+    const std::string who = "popsift::renderMesh";
+    const size_t n = sizes.size();
+    if (cameras.size() != n || poses.size() != n) throw std::runtime_error(who + ": one camera, one pose and one size per view expected");
+    static_assert(sizeof(MeshVertex) == sizeof(ps_mesh_vertex), "vertex layout");
+    const DeviceMesh m(mesh, who);
+    std::vector<int32_t> sz;
+    for (const auto& s : sizes) sz.insert(sz.end(), {s.first, s.second});
+    std::vector<std::unique_ptr<DevBuf>> bufs;
+    std::vector<float*> d_depth;
+    std::vector<int32_t*> d_tri;
+    const ps_render_report rep = render_dev(m, c_cameras(cameras), c_rigids(poses), sz, params.z_near, bufs, d_depth, d_tri, device, who);
+    RenderedMesh out;
+    out.n_drawn = rep.n_drawn;
+    out.n_big = rep.n_big;
+    out.n_covered = rep.n_covered;
+    out.maps.resize(n);
+    for (size_t v = 0; v < n; ++v) {
+        RenderMap& r = out.maps[v];
+        r.width = sizes[v].first;
+        r.height = sizes[v].second;
+        const size_t px = (size_t)r.width * r.height;
+        r.depth.resize(px);
+        r.triangle.resize(px);
+        check(ps_dev_to_host(r.depth.data(), d_depth[v], px * 4), who);
+        check(ps_dev_to_host(r.triangle.data(), d_tri[v], px * 4), who);
+    }
+    return out;
+}
+
+TexturedMesh textureMesh(const Mesh& mesh, const std::vector<DeviceImage>& images, const std::vector<Camera>& cameras,
+                         const std::vector<Rigid>& poses, const TextureParams& params, int device)
+{
+    const std::string who = "popsift::textureMesh";
+    const size_t n = images.size();
+    if (cameras.size() != n || poses.size() != n) throw std::runtime_error(who + ": one camera and one pose per image expected");
+    const DeviceMesh m(mesh, who);
+    const std::vector<ps_camera> cam = c_cameras(cameras);
+    const std::vector<ps_rigid> pose = c_rigids(poses);
+    std::vector<ps_image> img;
+    std::vector<int32_t> sz;
+    for (const DeviceImage& im : images) {
+        img.push_back(ps_image{im.data, im.pitch, im.width, im.height});
+        sz.insert(sz.end(), {im.width, im.height});
+    }
+    std::vector<std::unique_ptr<DevBuf>> bufs;
+    std::vector<float*> d_depth;
+    std::vector<int32_t*> d_tri;
+    render_dev(m, cam, pose, sz, params.z_near, bufs, d_depth, d_tri, device, who);
+    TexturedMesh out;
+    out.cell = params.cell;
+    out.cells_per_row = params.cells_per_row;
+    if (out.cells_per_row == 0 && params.cell > 0)
+        out.cells_per_row = std::max(1, std::min((int)std::ceil(std::sqrt((double)std::max<int64_t>(m.nt, 1))), 65535 / params.cell));
+    if (out.cells_per_row < 1) throw std::runtime_error(who + ": cells_per_row must be >= 1");
+    out.width = out.cells_per_row * params.cell;
+    out.height = (int)((m.nt + out.cells_per_row - 1) / out.cells_per_row) * params.cell;
+    DevBuf d_atlas((size_t)std::max(out.width, 0) * std::max(out.height, 0), who), d_view((size_t)m.nt * 4, who);
+    const ps_texture_params prm{params.cell, out.cells_per_row, params.depth_tol, params.min_cos, params.z_near, 0};
+    ps_texture_report rep;
+    std::vector<const float*> c_depth(d_depth.begin(), d_depth.end());
+    check(ps_mesh_texture(device, (int)n, img.data(), cam.data(), pose.data(), c_depth.data(), static_cast<const ps_mesh_vertex*>(m.v.p), m.nv,
+                          static_cast<const int32_t*>(m.t.p), m.nt, &prm, static_cast<uint8_t*>(d_atlas.p), static_cast<int32_t*>(d_view.p),
+                          &rep),
+          who, "ps_mesh_texture");
+    out.n_viewed = rep.n_viewed;
+    out.n_fallback = rep.n_fallback;
+    out.atlas.resize((size_t)out.width * out.height);
+    out.view.resize((size_t)m.nt);
+    if (!out.atlas.empty()) check(ps_dev_to_host(out.atlas.data(), d_atlas.p, out.atlas.size()), who);
+    if (!out.view.empty()) check(ps_dev_to_host(out.view.data(), d_view.p, out.view.size() * 4), who);
     return out;
 }
 

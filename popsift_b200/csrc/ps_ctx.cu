@@ -18,6 +18,7 @@
 #include "popsift_b200_twoview.h"
 #include "popsift_b200_depth.h"
 #include "popsift_b200_mesh.h"
+#include "popsift_b200_render.h"
 
 #include <algorithm>
 #include <atomic>
@@ -1901,6 +1902,92 @@ extern "C" int ps_tsdf_mesh(int device, const ps_volume* vol, const ps_mesh_para
         return PS_ERR_OVERFLOW;
     }
     return PS_OK;
+}
+
+// a camera and a pose ps_triangulate_tracks accepts
+static bool camera_pose_ok(const ps_camera& c, const ps_rigid& p)
+{
+    return std::isfinite(c.fx) && c.fx > 0.0f && std::isfinite(c.fy) && c.fy > 0.0f && std::isfinite(c.cx) && std::isfinite(c.cy) &&
+           rigid_ok(p);
+}
+
+// the counts and mesh arrays ps_mesh_render and ps_mesh_texture share (before the device is set)
+static bool mesh_counts_ok(int n_views, int64_t n_vertices, int64_t n_triangles, const ps_mesh_vertex* d_vertices, const int32_t* d_triangles)
+{
+    if (n_views < 0 || n_vertices < 0 || n_triangles < 0 || n_triangles >= 0x80000000LL) return false;
+    return n_triangles == 0 || (d_vertices && d_triangles);
+}
+
+static int finish_render(const char* name, int launched, bool bad, const char* err)
+{
+    if (launched >= 0 && bad) { g_create_error = std::string(name) + ": a triangle's vertex index is out of range"; return PS_ERR_ARG; }
+    return finish(name, launched, err);
+}
+
+extern "C" int ps_mesh_render(int device, int n_views, const int32_t* sizes, const ps_camera* cams, const ps_rigid* poses,
+                              const ps_mesh_vertex* d_vertices, int64_t n_vertices, const int32_t* d_triangles, int64_t n_triangles,
+                              const ps_render_params* prm, float* const* d_depth, int32_t* const* d_tri, ps_render_report* report)
+{
+    if (!prm || !report || !mesh_counts_ok(n_views, n_vertices, n_triangles, d_vertices, d_triangles)) return PS_ERR_ARG;
+    if (!std::isfinite(prm->z_near) || !(prm->z_near > 0.0f)) return PS_ERR_ARG;
+    if (n_views > 0 && (!sizes || !cams || !poses || !d_depth || !d_tri)) return PS_ERR_ARG;
+    for (int v = 0; v < n_views; ++v) {
+        if (sizes[2 * v] < 1 || sizes[2 * v] > 65535 || sizes[2 * v + 1] < 1 || sizes[2 * v + 1] > 65535) return PS_ERR_ARG;
+        if (!camera_pose_ok(cams[v], poses[v])) return PS_ERR_ARG;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    if (n_triangles > 0 && (ps_pointer_device(d_vertices) != device || ps_pointer_device(d_triangles) != device)) return PS_ERR_ARG;
+    if (!device_arrays(device, d_depth, n_views) && n_views > 0) return PS_ERR_ARG;
+    if (!device_arrays(device, d_tri, n_views) && n_views > 0) return PS_ERR_ARG;
+    if (n_views == 0) {
+        std::memset(report, 0, sizeof(*report));
+        return PS_OK;
+    }
+    const char* err = nullptr;
+    ps_render_report rep{};
+    bool bad = false;
+    const int n = run_mesh_render(n_views, sizes, cams, poses, d_vertices, n_vertices, d_triangles, n_triangles, *prm, d_depth, d_tri, &rep,
+                                  &bad, nullptr, &err);
+    const int rc = finish_render("ps_mesh_render", n, bad, err);
+    if (rc == PS_OK) *report = rep;
+    return rc;
+}
+
+extern "C" int ps_mesh_texture(int device, int n_views, const ps_image* images, const ps_camera* cams, const ps_rigid* poses,
+                               const float* const* d_depth, const ps_mesh_vertex* d_vertices, int64_t n_vertices, const int32_t* d_triangles,
+                               int64_t n_triangles, const ps_texture_params* prm, uint8_t* d_atlas, int32_t* d_view, ps_texture_report* report)
+{
+    if (!prm || !report || !mesh_counts_ok(n_views, n_vertices, n_triangles, d_vertices, d_triangles)) return PS_ERR_ARG;
+    if (!std::isfinite(prm->z_near) || !(prm->z_near > 0.0f) || !std::isfinite(prm->depth_tol) || !(prm->depth_tol >= 0.0f) ||
+        !(prm->min_cos >= 0.0f && prm->min_cos < 1.0f) || prm->cell < 3 || prm->cell > 64 || prm->cells_per_row < 1)
+        return PS_ERR_ARG;
+    if ((int64_t)prm->cells_per_row * prm->cell > 65535) return PS_ERR_ARG;
+    if ((n_triangles + prm->cells_per_row - 1) / prm->cells_per_row * prm->cell > 65535) return PS_ERR_ARG;
+    if (n_views > 0 && (!images || !cams || !poses || !d_depth)) return PS_ERR_ARG;
+    if (n_triangles > 0 && (!d_atlas || !d_view)) return PS_ERR_ARG;
+    for (int v = 0; v < n_views; ++v) {
+        const ps_image& im = images[v];
+        if (im.width < 2 || im.height < 2 || im.width > 65535 || im.height > 65535 || im.pitch < im.width) return PS_ERR_ARG;
+        if (!camera_pose_ok(cams[v], poses[v])) return PS_ERR_ARG;
+    }
+    if (!set_device(device)) return PS_ERR_CUDA;
+    for (int v = 0; v < n_views; ++v)
+        if (ps_pointer_device(images[v].data) != device || ps_pointer_device(d_depth[v]) != device) return PS_ERR_ARG;
+    if (n_triangles > 0 && (ps_pointer_device(d_vertices) != device || ps_pointer_device(d_triangles) != device ||
+                            ps_pointer_device(d_atlas) != device || ps_pointer_device(d_view) != device))
+        return PS_ERR_ARG;
+    if (n_triangles == 0) {
+        std::memset(report, 0, sizeof(*report));
+        return PS_OK;
+    }
+    const char* err = nullptr;
+    ps_texture_report rep{};
+    bool bad = false;
+    const int n = run_mesh_texture(n_views, images, cams, poses, d_depth, d_vertices, n_vertices, d_triangles, n_triangles, *prm, d_atlas,
+                                   d_view, &rep, &bad, nullptr, &err);
+    const int rc = finish_render("ps_mesh_texture", n, bad, err);
+    if (rc == PS_OK) *report = rep;
+    return rc;
 }
 
 extern "C" int ps_dev_to_host(void* dst_host, const void* src_dev, size_t bytes)

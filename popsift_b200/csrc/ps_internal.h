@@ -10,6 +10,7 @@
 #include "popsift_b200_twoview.h"
 #include "popsift_b200_depth.h"
 #include "popsift_b200_mesh.h"
+#include "popsift_b200_render.h"
 
 #include <cuda_runtime.h>
 #include <cmath>
@@ -354,5 +355,17 @@ int run_tsdf_integrate(int n_views, const ps_image* images, const ps_camera* cam
                        cudaStream_t st, const char** err);
 int run_tsdf_mesh(const ps_volume& vol, const ps_mesh_params& prm, int64_t max_vertices, int64_t max_triangles, ps_mesh_vertex* d_vertices,
                   int32_t* d_triangles, ps_mesh_report* report, bool* overflow, cudaStream_t st, const char** err);
+
+// mesh rendering and texturing (include/popsift_b200_render.h, k_render.cu), arguments already validated except the
+// vertex indices, which a first kernel checks: a bad one sets *bad, and the call returns before writing any output.
+// Render needs n_views > 0, texture n_triangles > 0.  Synchronous on `st`; *report is written when they return >= 0 with
+// *bad false.  Return the number of kernels launched or -1 (*err set).
+int run_mesh_render(int n_views, const int32_t* sizes, const ps_camera* cams, const ps_rigid* poses, const ps_mesh_vertex* d_vertices,
+                    int64_t n_vertices, const int32_t* d_triangles, int64_t n_triangles, const ps_render_params& prm, float* const* d_depth,
+                    int32_t* const* d_tri, ps_render_report* report, bool* bad, cudaStream_t st, const char** err);
+int run_mesh_texture(int n_views, const ps_image* images, const ps_camera* cams, const ps_rigid* poses, const float* const* d_depth,
+                     const ps_mesh_vertex* d_vertices, int64_t n_vertices, const int32_t* d_triangles, int64_t n_triangles,
+                     const ps_texture_params& prm, uint8_t* d_atlas, int32_t* d_view, ps_texture_report* report, bool* bad,
+                     cudaStream_t st, const char** err);
 
 } // namespace psb
