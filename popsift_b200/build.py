@@ -26,7 +26,7 @@ NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "--fmad=false",   # no implicit contraction anywhere; every fma in the kernels is explicit
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu", "k_pose.cu", "k_retrieval.cu", "k_tracks.cu", "k_triangulate.cu", "k_bundle.cu", "k_global.cu", "k_viewgraph.cu", "k_twoview.cu", "k_depth.cu", "k_mesh.cu", "k_render.cu", "workspace.cu",
+LIB_SOURCES = ["ps_tables.cpp", "ps_ctx.cu", "ps_batch.cu", "k_pyramid.cu", "k_pyramid_march.cu", "tma_util.cu", "k_match.cu", "k_match_u8.cu", "k_extrema.cu", "k_filter.cu", "k_orient.cu", "k_desc.cu", "k_desc_modes.cu", "k_describe.cu", "k_verify.cu", "k_pose.cu", "k_retrieval.cu", "k_tracks.cu", "k_triangulate.cu", "k_bundle.cu", "k_global.cu", "k_viewgraph.cu", "k_twoview.cu", "k_depth.cu", "k_mesh.cu", "k_render.cu", "workspace.cu",
                "host/sift_conf.cpp", "host/features.cpp", "host/popsift.cpp", "host/device_prop.cpp", "host/log_dump.cpp"]
 DEMO_SOURCES = ["app/popsift_demo.cpp", "app/pgmread.cpp"]
 MATCH_SOURCES = ["app/popsift_match.cpp"]            # + app/pgmread.cpp

@@ -15,6 +15,7 @@
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstdint>
+#include <string>
 #include <vector>
 
 namespace psb {
@@ -119,6 +120,9 @@ inline float extrema_threshold(const Consts& k)
     // float(0.8) * 2 == float(1.6): the VLFeat and PopSift expressions agree bit for bit
     return k.sift_mode == PS_MODE_OPENCV ? floorf(k.threshold) : 1.6f * k.threshold;
 }
+
+// the calling thread's message for ps_last_error(NULL); the stateless entry points (ps_batch.cu) report through it
+void set_last_error(const std::string& msg);
 
 // multiprocessors of the CURRENT device (cudaDeviceProp::multiProcessorCount, cached per device; 132 on H100 SXM):
 // every fixed grid and the one-wave partition of the pyramid kernels are sized from it
